@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- nodes/sec embedded at d=128 (HOPE, node2vec) on B200 vs the reference's CPU path.
+"""bench.py -- nodes/sec embedded at d=128 (HOPE, node2vec) on H100 vs the reference's CPU path.
 
-    python bench.py --gpus N --steps K --warmup W [--workload hope|node2vec] [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--workload hope|node2vec|recon] [--impl reference] [--dump-outputs DIR]
 
 Default (N=1): BASELINE.json configs[1] -- HOPE d=128, beta=0.01 on the synthetic SBM with
-1,000,000 nodes / ~20M directed edges (SURVEY 8(d) config 2), one B200.  A "step" is one complete
+1,000,000 nodes / ~20M directed edges (SURVEY 8(d) config 2), one H100.  A "step" is one complete
 learn_embedding-equivalent pass (norm estimate, Katz/SpMM subspace iteration, Rayleigh-Ritz, X) over
 the graph.
   value : n * K / (sum of the K device times), CSR already resident in HBM, X left on the device;
@@ -14,7 +14,8 @@ the graph.
   N > 1 : launched by torchrun, one rank per GPU; weak scaling: n = N * 1,000,000 (rows per GPU fixed),
           CSR row-sharded; only the rows a shard references travel, stored into the peers' halo slots over NVLink by the
           kernel that produces them (gem_b200/csrc/halo.cu); b x b all-reduce per Gram on NCCL.
-  The default line also carries a "node2vec" sub-record: BASELINE.json configs[2] on the same graph (one epoch).
+  The default line also carries a "node2vec" sub-record: BASELINE.json configs[2] on the same graph (one epoch, its own
+  "steps": 1 -- an epoch takes seconds).
 --workload node2vec: BASELINE.json configs[2] (d=128, p=q=1, 10 walks x 80, context 10, 1 epoch).
 --workload recon: the step after learn_embedding in every reference test (tests/fit_model.py:10, SURVEY 8(f) rank 1):
   evaluateStaticGraphReconstruction of a HOPE embedding (d=128) of an SBM with --recon-n nodes (default 32768):
@@ -25,6 +26,14 @@ the graph.
   form of hope.py:28-36 that fits in memory beyond ~50k nodes, at the FULL 1M-node configuration with the operator on
   all host cores; node2vec: the reference's own SNAP binary from oracle/_ref when present, else
   oracle/n2v_oracle.c, on a bounded sample).
+--steps K sets the number of timed steps of the workload's line: the device-time loop and the end-to-end calls.
+--dump-outputs DIR: after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy
+  (float32 / float64; an n x d embedding is written as a fixed, seeded sample of DUMP_ROWS rows plus their row ids).
+  The inputs depend only on the arguments (seeded generators), and the HOPE and reconstruction paths add across CTAs in a
+  fixed order (no floating-point atomics), so a run reproduces the outputs bit for bit and two builds can be compared output
+  for output.  The default line dumps HOPE's outputs only: node2vec's Hogwild SGNS (like the reference's OpenMP training)
+  applies its updates in the order the warps run, so its embedding differs between runs; `--workload node2vec` still
+  writes it.
 """
 import argparse
 import json
@@ -46,7 +55,7 @@ if REPO not in sys.path:
 # oracle by tests/test_gpu_hope.py::test_bench_solver_setting_against_fp64_oracle): Chebyshev filter degree <= 16,
 # dynamic-range guard 2^14, oversample 8 (block 72), stop when the residual of every wanted Ritz pair, mapped to the
 # Katz operator, is <= 4e-3 sigma_max (stop_rule 1) -- round 1 stopped on a 1e-3 singular-value change and DELIVERED
-# 4.0e-3; this setting delivers 3.0e-3 in 4 rounds instead of 8 (profiles/r02c_solver_sweep.md).
+# 4.0e-3; this setting delivers 3.0e-3 in 4 rounds instead of 8 (scripts/exp_solver.py sweeps the settings).
 HOPE_SOLVER = dict(tol=4e-3, stop_rule=1, cheb_degree=16, cheb_range_log2=14, max_iters=30, min_iters=2, oversample=8, seed=1234)
 CPU_ARPACK_TOL = 1e-3      # tol handed to scipy svds in the CPU arm (the reference's own tol=0 does not terminate at 1M nodes)
 
@@ -58,14 +67,14 @@ def read_peaks():
             return json.load(open(p)), 'measured (MEASURED_PEAKS.json)'
         except Exception:
             pass
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback (B200_PROFILING.md)'
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'H100 SXM data sheet (700 W board power)'
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region, with the card's name and power limit."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,'
          'clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
-         'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
+         'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit')
 
     def __init__(self, device):
         self.device = device
@@ -94,12 +103,13 @@ class ClockSampler:
             self.proc.wait(timeout=5)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, reasons, gpu, plim = [], [], set(), None, None
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
         for ln in self.lines:
             f = [x.strip() for x in ln.split(',')]
-            if len(f) < 9:
+            if len(f) < 11:
                 continue
+            gpu, plim = f[9], f[10]
             try:
                 sm.append(float(f[1])); mx.append(float(f[2]))
             except ValueError:
@@ -107,8 +117,28 @@ class ClockSampler:
             for name, val in zip(names, f[5:9]):
                 if val.lower().startswith('active'):
                     reasons.add(name)
-        return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': float(max(mx)) if mx else None,
-                'samples': len(sm), 'reasons': sorted(reasons)}
+        return {'gpu': gpu, 'power_limit_w': plim, 'sm_mhz': float(np.median(sm)) if sm else None,
+                'sm_max_mhz': float(max(mx)) if mx else None, 'samples': len(sm), 'reasons': sorted(reasons)}
+
+
+DUMP_ROWS = 32768      # rows of an n x d output that --dump-outputs keeps (16 MB at d = 128)
+
+
+def row_sample(X, row0=0):
+    """A fixed, seeded sample of the rows of X (all rows when there are at most DUMP_ROWS): (global row ids as float64,
+    the rows)."""
+    n = X.shape[0]
+    rows = np.arange(n) if n <= DUMP_ROWS else np.sort(np.random.default_rng(0).choice(n, DUMP_ROWS, replace=False))
+    return (rows + row0).astype(np.float64), np.ascontiguousarray(X[rows])
+
+
+def dump_outputs(path, arrays):
+    """--dump-outputs: <path>/<name>.npy for every array (float32 / float64)."""
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(path, name + '.npy'), a)
 
 
 # ----------------------------------------------------------------------------------- distributed glue
@@ -489,8 +519,10 @@ def run_hope(args, dist, rank, world, local):
     launches0 = _native.lib().gemb_launch_count()
     dev_ms, stats = 0.0, None
     t0 = time.perf_counter()
-    for _ in range(args.steps):
-        _, _, st = g.hope(args.d, beta_arg, want_output=False, **solver)
+    for s in range(args.steps):
+        # the last step hands X and sigma back to the host when they are dumped (total_ms ends before that copy)
+        want = bool(args.dump_outputs) and s == args.steps - 1
+        X_last, sig_last, st = g.hope(args.d, beta_arg, want_output=want, **solver)
         dev_ms += st['total_ms']
         stats = st if stats is None else {k: (stats[k] + st[k] if k in ('spmm_ms', 'dense_ms', 'comm_ms', 'spmm_count', 'pushes', 'push_bytes') else st[k])
                                           for k in st}
@@ -501,6 +533,9 @@ def run_hope(args, dist, rank, world, local):
     dev_ms = dist_max(dist, dev_ms, local)
     wall_s = dist_max(dist, wall_s, local)
     value = n_all * args.steps / (dev_ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        rows, Xs = row_sample(X_last, r0)
+        dump_outputs(args.dump_outputs, {'hope_X_rows': rows, 'hope_X': Xs, 'hope_sigma': sig_last})
 
     # accuracy of the timed solution, outside the timed region: one more identical solve that also applies the fp32
     # Katz operator to the result, || S^T u_j - sigma_j v_j || / sigma_max over the k triplets (collective on N > 1)
@@ -514,16 +549,8 @@ def run_hope(args, dist, rank, world, local):
     # roofline of the dominant kernel (CSR SpMM): algorithmic bytes per launch / mean launch time
     spmm_ms_per = stats['spmm_ms'] / max(stats['spmm_count'], 1)
     achieved = stats['spmm_bytes'] / (spmm_ms_per * 1e-3) / 1e9 if spmm_ms_per > 0 else 0.0
-    traffic = None
-    tp = os.path.join(REPO, 'profiles', 'spmm_traffic.json')
-    # the ncu capture is of THIS workload on one GPU (SBM 1M, block 72): no traffic figure for other graphs / shardings
-    if os.path.exists(tp) and not rmat and world == 1 and stats['block'] == 72 and args.n == 1_000_000:
-        try:
-            traffic = json.load(open(tp)).get('dram_bytes_per_launch')
-        except Exception:
-            traffic = None
     roofline = {'kernel': 'spmm (CSR x n-by-%d fp32 block)' % stats['block'], 'bound': 'hbm', 'achieved': achieved,
-                'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': achieved / peaks['hbm_gbs'], 'traffic': traffic,
+                'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': achieved / peaks['hbm_gbs'], 'traffic': None,
                 'peak_source': peak_src, 'bytes_per_launch': stats['spmm_bytes'], 'ms_per_launch': spmm_ms_per,
                 'launches_per_step': stats['spmm_count'] / args.steps,
                 'share_of_step': stats['spmm_ms'] / max(dev_ms, 1e-9)}
@@ -547,7 +574,7 @@ def run_hope(args, dist, rank, world, local):
         # The GPU boxes show bursts of host-side stalls (a 9 ms D2H wait returning after 600 ms, with the device
         # idle) that have nothing to do with this process, so the reported step time is the MEDIAN call; the
         # mean, min and max are given beside it.
-        ksteps = max(3, args.steps) if world == 1 else max(3, min(args.steps, 5))
+        ksteps = args.steps
         step_ms = []
         for _ in range(ksteps):
             dist_barrier(dist, local)
@@ -610,7 +637,7 @@ def run_hope(args, dist, rank, world, local):
                                                                 'blocks_exchanged_per_step': stats.get('pushes', 0) / args.steps,
                                                                 'nvlink_bytes_out_per_step_rank0': stats.get('push_bytes', 0.0) / args.steps,
                                                                 'wire': 'fp16 (x 2^12) for the filter / basis blocks, fp32 for the raw warm-up blocks' if stats.get('mg_mode') == 3 else 'fp32'},
-                           'l2_policy': 'inputs larger than L2 (CSR %.0f MB + 5 blocks of %.0f MB vs 126 MB L2)' % (
+                           'l2_policy': 'inputs larger than L2 (CSR %.0f MB + 5 blocks of %.0f MB vs 50 MB L2)' % (
                                (nnz_all * 4 + n_all * 4) / 1e6 / world, n_all * stats['block'] * 4 / 1e6 / world)},
                 'wall_ms_per_step': wall_s * 1e3 / args.steps, 'graph_gen_s': gen_s,
                 'phases_ms_per_step': {'spmm': stats['spmm_ms'] / args.steps, 'dense': stats['dense_ms'] / args.steps,
@@ -618,14 +645,6 @@ def run_hope(args, dist, rank, world, local):
                 'gpu_launches': int(launches), 'clocks': clocks, 'roofline': roofline, 'e2e': e2e, 'cpu_baseline': cpu}
     ctx.close()
     return line
-
-
-def n2v_traffic():
-    tp = os.path.join(REPO, 'profiles', 'sgns_traffic.json')
-    try:
-        return json.load(open(tp)).get('dram_bytes_per_launch')
-    except Exception:
-        return None
 
 
 def run_node2vec(args, dist, rank, world, local):
@@ -664,8 +683,9 @@ def run_node2vec(args, dist, rank, world, local):
     launches0 = _native.lib().gemb_launch_count()
     dev_ms, agg = 0.0, None
     for s in range(args.steps):
-        _, st = g.node2vec(nids, *hp, seed=1 + s, want_output=False)
-        dev_ms += st['total_ms']
+        want = bool(args.dump_outputs) and s == args.steps - 1
+        X_last, st = g.node2vec(nids, *hp, seed=1 + s, want_output=want)
+        dev_ms += st['total_ms'] - (st['d2h_ms'] if want else 0.0)       # total_ms includes the copy of X to the host
         agg = st if agg is None else {k: agg[k] + st[k] for k in st}
     dist_barrier(dist, local)
     launches = _native.lib().gemb_launch_count() - launches0
@@ -673,11 +693,14 @@ def run_node2vec(args, dist, rank, world, local):
     dev_ms = dist_max(dist, dev_ms, local)
     pairs = dist_sum(dist, float(agg['pairs']), local)
     value = n_emb * args.steps / (dev_ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        rows, Xs = row_sample(X_last)
+        dump_outputs(args.dump_outputs, {'node2vec_X_rows': rows, 'node2vec_X': Xs})
     sg_bytes = pairs * 14 * 4 * args.d
     achieved = sg_bytes / world / (agg['sgns_ms'] * 1e-3) / 1e9 if agg['sgns_ms'] > 0 else 0.0
     roofline = {'kernel': 'sgns (warp per walk, fp32 tables)', 'bound': 'hbm', 'achieved': achieved,
                 'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': achieved / peaks['hbm_gbs'],
-                'traffic': n2v_traffic() if (not rmat and world == 1 and args.n == 1_000_000 and (args.d, args.walk_len, args.num_walks, args.con_size) == (128, 80, 10, 10)) else None,
+                'traffic': None,
                 'peak_source': peak_src, 'bytes_per_launch': sg_bytes / world / args.steps,
                 'ms_per_launch': agg['sgns_ms'] / args.steps, 'share_of_step': agg['sgns_ms'] / max(dev_ms, 1e-9),
                 'note': 'algorithmic bytes = 7168 B per (centre, context) pair (SURVEY 8(d)); rows of the walk and the '
@@ -687,13 +710,16 @@ def run_node2vec(args, dist, rank, world, local):
         node2vec.hyper_params.clear(); node2vec.hyper_params.update({'method_name': 'node2vec_rw'})
         model = node2vec(d=args.d, max_iter=1, walk_len=args.walk_len, num_walks=args.num_walks,
                          con_size=args.con_size, ret_p=1, inout_p=1, device=local)
-        t0 = time.perf_counter()
-        X = model.learn_embedding(graph=(csr, nids))
-        _ = float(X[0, 0])
-        e2e_s = time.perf_counter() - t0
-        e2e = {'value': n_emb / e2e_s, 'unit': 'nodes/s', 'ms_per_step': e2e_s * 1e3,
+        step_ms = []
+        for _ in range(args.steps):
+            t0 = time.perf_counter()
+            X = model.learn_embedding(graph=(csr, nids))
+            _ = float(X[0, 0])
+            step_ms.append((time.perf_counter() - t0) * 1e3)
+        e2e_s = float(np.median(step_ms)) * 1e-3
+        e2e = {'value': n_emb / e2e_s, 'unit': 'nodes/s', 'ms_per_step': e2e_s * 1e3, 'stat': 'median of %d calls' % len(step_ms),
                'h2d_bytes_per_step': int(4 * (csr.n + 1) + 4 * csr.nnz + 4 * n_emb * args.num_walks),
-               'd2h_bytes_per_step': int(4 * csr.n * args.d), 'steps': 1,
+               'd2h_bytes_per_step': int(4 * csr.n * args.d), 'steps': len(step_ms),
                'call': 'gem_b200.embedding.node2vec.node2vec(...).learn_embedding(graph=(CSR, node table))'}
     cpu = None
     if rank == 0 and not args.no_cpu:
@@ -718,7 +744,7 @@ def run_node2vec(args, dist, rank, world, local):
                 'config': {'workload': 'node2vec d=%d p=q=1, %d walks x %d, context %d, 1 epoch, 5 negatives, on %s n=%d, nnz=%d; %d vertices have edges (node table, walks, value)'
                                        % (args.d, args.num_walks, args.walk_len, args.con_size, rmat_name(args) if rmat else 'SBM', n, csr.nnz, n_emb),
                            'parallelism': 'walk-sharded x%d, embedding-delta all-reduce per epoch' % world if world > 1 else 'single GPU',
-                           'l2_policy': 'inputs larger than L2 (two %d MB embedding tables + %d MB walks)' % (
+                           'l2_policy': 'inputs larger than L2 (two %d MB embedding tables + %d MB walks vs 50 MB L2)' % (
                                csr.n * args.d * 4 // 10**6, n_emb * args.num_walks * args.walk_len * 4 // 10**6 // world)},
                 'phases_ms_per_step': {k: agg[k] / args.steps for k in ('alias_ms', 'shuffle_ms', 'walk_ms', 'vocab_ms', 'sgns_ms', 'comm_ms')},
                 'gpu_launches': int(launches), 'clocks': clocks, 'roofline': roofline, 'e2e': e2e, 'cpu_baseline': cpu}
@@ -753,7 +779,7 @@ def run_recon(args, dist, rank, world, local):
         ti, tj, tw = rec.top(True, K)
         ranks, npr = rec.ranks(ip32, ix32, True)
         rec.free()
-        return t_sel, ranks
+        return t_sel, ranks, (ti, tj, tw)
 
     for _ in range(args.warmup):
         step()
@@ -764,8 +790,8 @@ def run_recon(args, dist, rank, world, local):
     l0 = lib.gemb_launch_count()
     t0 = time.perf_counter()
     sel_s = 0.0
-    for _ in range(args.steps):
-        ts, ranks = step()
+    for s in range(args.steps):
+        ts, ranks, top = step()
         sel_s += ts
     dist_barrier(dist, local)
     wall = time.perf_counter() - t0
@@ -773,6 +799,12 @@ def run_recon(args, dist, rank, world, local):
     clocks = sampler.stop() if rank == 0 else None
     wall = dist_max(dist, wall, local)
     value = world * float(n) * n * args.steps / wall
+    if args.dump_outputs and rank == 0:
+        # gemb_recon_top returns the candidates unordered (compaction order); the caller orders them by weight descending,
+        # then i, then j (include/gemb200.h) -- so does the dump
+        o = np.lexsort((top[1], top[0], -top[2]))
+        dump_outputs(args.dump_outputs, {'recon_edge_ranks': ranks.astype(np.float64), 'recon_top_i': top[0][o].astype(np.float64),
+                                         'recon_top_j': top[1][o].astype(np.float64), 'recon_top_w': top[2][o]})
     n_pad = (n + 63) // 64 * 64
     passes = 32                                            # 1 total count + 31 bisection steps per selection
     bytes_per_launch = 4.0 * n * n_pad
@@ -790,7 +822,7 @@ def run_recon(args, dist, rank, world, local):
         model = HOPE(d=args.d, beta=args.beta, device=local)
         evaluateStaticGraphReconstruction(csr, model, X, None, max_k=K)
         step_ms = []
-        for _ in range(max(3, args.steps)):
+        for _ in range(args.steps):
             t1 = time.perf_counter()
             MAP, prec, _, _ = evaluateStaticGraphReconstruction(csr, model, X, None, max_k=K)
             step_ms.append((time.perf_counter() - t1) * 1e3)
@@ -813,7 +845,7 @@ def run_recon(args, dist, rank, world, local):
                 'config': {'workload': 'reconstruction evaluation of a HOPE d=%d embedding, SBM n=%d nnz=%d, undirected, max_k=%d'
                                        % (args.d, n, csr.nnz, K),
                            'parallelism': 'single GPU' if world == 1 else 'replicas only (%d independent evaluations)' % world,
-                           'l2_policy': 'inputs larger than L2 (reconstruction %.1f GB vs 126 MB L2)' % (bytes_per_launch / 1e9)},
+                           'l2_policy': 'inputs larger than L2 (reconstruction %.1f GB vs 50 MB L2)' % (bytes_per_launch / 1e9)},
                 'gpu_launches': int(launches), 'clocks': clocks, 'roofline': roofline, 'e2e': e2e, 'cpu_baseline': cpu}
         print(json.dumps(line), flush=True)
     ctx.close()
@@ -845,9 +877,13 @@ def main():
     ap.add_argument('--no-accuracy', action='store_true', help='skip the fp64 host check of the timed solution')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--no-cpu', action='store_true')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='after the timed steps, write the outputs of the last timed step as DIR/<name>.npy')
     args = ap.parse_args()
     if args.steps is None:
         args.steps = {'hope': 20, 'recon': 5}.get(args.workload, 1)
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
     if args.impl == 'reference':
         args.warmup_requested = args.warmup
         args.warmup = min(args.warmup, 1)      # each CPU step is a bounded 10-30 s sample (HOPE: a full solve, no warm-up)
@@ -858,12 +894,12 @@ def main():
         if args.workload == 'hope':
             line = run_hope(args, dist, rank, world, local)
             if not args.no_node2vec and args.graph != 'rmat':
-                # BASELINE.json configs[2] rides in the same line (one epoch = one step; it takes ~10 s, so it is timed
-                # once whatever --steps says): the driver's bench and scaling runs then see node2vec too
-                steps, warm = args.steps, args.warmup
-                args.steps, args.warmup = 1, min(args.warmup, 3)
+                # BASELINE.json configs[2] rides in the same line: one epoch (= one step, several seconds), whatever --steps
+                # says for the HOPE record; the sub-record states its own "steps"
+                steps, warm, dump = args.steps, args.warmup, args.dump_outputs
+                args.steps, args.warmup, args.dump_outputs = 1, min(args.warmup, 3), None
                 sub = run_node2vec(args, dist, rank, world, local)
-                args.steps, args.warmup = steps, warm
+                args.steps, args.warmup, args.dump_outputs = steps, warm, dump
                 if line is not None:
                     line['node2vec'] = sub
                     line['gpu_launches'] += sub['gpu_launches']

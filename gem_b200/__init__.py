@@ -1,4 +1,4 @@
-"""gem_b200 -- B200 (sm_100a) core for GEM's HOPE and node2vec behind the StaticGraphEmbedding API.
+"""gem_b200 -- H100 (sm_90a) core for GEM's HOPE and node2vec behind the StaticGraphEmbedding API.
 
     from gem_b200.embedding.hope import HOPE
     from gem_b200.embedding.node2vec import node2vec

@@ -1,4 +1,4 @@
-// gem_b200/csrc/common.cuh -- shared declarations of libgemb200.so (sm_100a only).
+// gem_b200/csrc/common.cuh -- shared declarations of libgemb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -80,13 +80,15 @@ struct gemb_halo_pool {
 
 struct gemb_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     // multi-GPU
     int rank = 0, nranks = 1;
     void *comm = nullptr;  // ncclComm_t
     float *spmm_scratch = nullptr;   // chunk partial sums of the heavy rows (n_items x b), grown on demand
     size_t spmm_scratch_bytes = 0;
+    double *red_scratch = nullptr;   // per-CTA partials of the fixed-order reductions (dense.cu), grown on demand
+    size_t red_scratch_bytes = 0;
     gemb::Timer t_spmm, t_dense, t_comm, t_misc;
     gemb_halo_pool halo_pool;
 };
@@ -197,9 +199,13 @@ int apply_fp32_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const fl
 int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_out_dev, double *Minv64 = nullptr);
 //  C (fp64) and/or C32 (fp32) = op(A) * B for b x b fp64 matrices (one CTA)
 int small_gemm_launch(gemb_ctx *ctx, int b, const double *A, int transA, const double *B, double *C, float *C32);
-// CUDA-core Gram (gram_launch prefers the tcgen05 kernel in gram_tc.cu when the shape fits)
+// CUDA-core Gram (gram_launch prefers the wgmma kernel in gram_tc.cu when the shape fits)
 int gram_fp32_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G);
 int gram_tc_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G);
+// Reductions across CTAs never use floating-point atomics: every CTA writes its partial, and
+// out[i] = sum_{c < parts} part[c * count + i] is added in a fixed order, so a result is the same on every run.
+int red_scratch(gemb_ctx *ctx, size_t doubles, double **out);
+int sum_partials_launch(gemb_ctx *ctx, int parts, int64_t count, const double *part, double *out);
 //  eigh: G -> eigenvalues w ascending (b), eigenvectors Z (b x b, column j <-> w[j]); G destroyed.
 // rel_tol: stop the Jacobi sweeps when ||offdiag||_F <= rel_tol * ||G||_F
 int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch /* b x b */, double rel_tol = 1e-11);

@@ -202,8 +202,8 @@ int gemb_ctx_create(int device, gemb_ctx **out) {
     GEMB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     GEMB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        set_error("device %d is sm_%d%d; libgemb200 is built for sm_100a only", device, prop.major,
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("device %d is sm_%d%d; libgemb200 is built for sm_90a (H100) only", device, prop.major,
                   prop.minor);
         return GEMB_ERR_CUDA;
     }
@@ -228,6 +228,7 @@ int gemb_ctx_destroy(gemb_ctx *c) {
     c->t_comm.destroy();
     c->t_misc.destroy();
     dfree(c->spmm_scratch);
+    dfree(c->red_scratch);
     if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
     return GEMB_OK;

@@ -12,11 +12,12 @@
 namespace gemb {
 
 // ------------------------------------------------------------------------------------ gram
-// Output tile (16*TM) x (16*TM) per blockIdx.y, rows strided over blockIdx.x in chunks of KC.
+// Output tile (16*TM) x (16*TM) per blockIdx.y, rows strided over blockIdx.x in chunks of KC; the partial sums of
+// blockIdx.x go to Gpart[blockIdx.x][b1][b2] (added in a fixed order afterwards).
 template <int TM>
 __global__ void __launch_bounds__(256)
 gram_kernel(int64_t n, const float *__restrict__ P, int b1, const float *__restrict__ Q, int b2,
-            double *__restrict__ G, int tiles_n) {
+            double *__restrict__ Gpart, int tiles_n) {
     constexpr int BT = 16 * TM;
     constexpr int KC = 32;
     __shared__ float sP[KC][BT];
@@ -65,7 +66,7 @@ gram_kernel(int64_t n, const float *__restrict__ P, int b1, const float *__restr
 #pragma unroll
         for (int j = 0; j < TM; j++) {
             const int gn = n0 + tx * TM + j;
-            if (gn < b2) atomicAdd(G + (size_t)gm * b2 + gn, (double)acc[i][j]);
+            if (gn < b2) Gpart[(size_t)blockIdx.x * b1 * b2 + (size_t)gm * b2 + gn] = (double)acc[i][j];
         }
     }
 }
@@ -86,7 +87,7 @@ static int pick_tm(int b) {
 
 int gram_tc_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G);
 
-static int gram_mode() {   // GEMB_GRAM=fp32 forces the CUDA-core kernel (A/B testing); default = tcgen05
+static int gram_mode() {   // GEMB_GRAM=fp32 forces the CUDA-core kernel (A/B testing); default = wgmma
     static int mode = -1;
     if (mode < 0) {
         const char *e = getenv("GEMB_GRAM");
@@ -105,9 +106,53 @@ int gram_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q
     return gram_fp32_launch(ctx, n, P, b1, Q, b2, G);
 }
 
+int red_scratch(gemb_ctx *ctx, size_t doubles, double **out) {
+    const size_t need = sizeof(double) * std::max<size_t>(doubles, 1);
+    if (ctx->red_scratch_bytes < need) {
+        GEMB_CUDA(dfree(ctx->red_scratch));
+        ctx->red_scratch = nullptr; ctx->red_scratch_bytes = 0;
+        GEMB_CUDA(dmalloc(&ctx->red_scratch, need));
+        ctx->red_scratch_bytes = need;
+    }
+    *out = ctx->red_scratch;
+    return GEMB_OK;
+}
+
+// block (32, 8): 32 consecutive outputs; warp y adds parts y, y + 8, ... (coalesced rows), then the 8 sums in order
+__global__ void __launch_bounds__(256) sum_partials_kernel(int parts, int64_t count, const double *__restrict__ part,
+                                                           double *__restrict__ out) {
+    __shared__ double s_sum[8][33];
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    for (int64_t i0 = (int64_t)blockIdx.x * 32; i0 < count; i0 += (int64_t)gridDim.x * 32) {
+        const int64_t i = i0 + tx;
+        double s = 0.0;
+        if (i < count)
+            for (int c = ty; c < parts; c += 8) s += part[(size_t)c * count + i];
+        s_sum[ty][tx] = s;
+        __syncthreads();
+        if (ty == 0 && i < count) {
+            double t = 0.0;
+            for (int y = 0; y < 8; y++) t += s_sum[y][tx];
+            out[i] = t;
+        }
+        __syncthreads();
+    }
+}
+
+int sum_partials_launch(gemb_ctx *ctx, int parts, int64_t count, const double *part, double *out) {
+    if (count == 0) return GEMB_OK;
+    const int grid = (int)std::min<int64_t>((count + 31) / 32, (int64_t)ctx->sm_count * 16);
+    sum_partials_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(parts, count, part, out);
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    return GEMB_OK;
+}
+
 int gram_fp32_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G) {
-    GEMB_CUDA(cudaMemsetAsync(G, 0, sizeof(double) * (size_t)b1 * b2, ctx->stream));
-    if (n == 0) return GEMB_OK;
+    if (n == 0) {
+        GEMB_CUDA(cudaMemsetAsync(G, 0, sizeof(double) * (size_t)b1 * b2, ctx->stream));
+        return GEMB_OK;
+    }
     const int bmax = b1 > b2 ? b1 : b2;
     const int TM = pick_tm(bmax);
     const int BT = 16 * TM;
@@ -117,15 +162,17 @@ int gram_fp32_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const flo
     if (gx < 1) gx = 1;
     if (gx > chunks) gx = (int)chunks;
     dim3 grid(gx, tiles_m * tiles_n), block(256);
+    double *part = nullptr;
+    GEMB_TRY(red_scratch(ctx, (size_t)gx * b1 * b2, &part));
     switch (TM) {
-        case 4: gram_kernel<4><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, G, tiles_n); break;
-        case 5: gram_kernel<5><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, G, tiles_n); break;
-        case 6: gram_kernel<6><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, G, tiles_n); break;
-        default: gram_kernel<8><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, G, tiles_n); break;
+        case 4: gram_kernel<4><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
+        case 5: gram_kernel<5><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
+        case 6: gram_kernel<6><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
+        default: gram_kernel<8><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
     }
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    return GEMB_OK;
+    return sum_partials_launch(ctx, gx, (int64_t)b1 * b2, part, G);
 }
 
 // ------------------------------------------------------------------------------------ apply
@@ -186,7 +233,7 @@ apply_kernel(int64_t n, const float *__restrict__ Q, int b1, const float *__rest
 
 int apply_tc_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const float *M, int ldm, int b2, float *Out, int ldo);
 
-static int apply_mode() {   // GEMB_APPLY=fp32 forces the CUDA-core kernel; default = tcgen05 where the shape fits
+static int apply_mode() {   // GEMB_APPLY=fp32 forces the CUDA-core kernel; default = wgmma where the shape fits
     static int mode = -1;
     if (mode < 0) {
         const char *e = getenv("GEMB_APPLY");
@@ -448,7 +495,7 @@ eigh_jacobi_kernel(int b, double *__restrict__ Ag, double *__restrict__ w, doubl
     double *mat = sh + 3 * half + 2;
     double *A = MODE >= 1 ? mat : Ag;
     double *Zt = MODE >= 2 ? mat + (size_t)b * b : Ztg;
-    __shared__ double s_off, s_diag;
+    __shared__ double s_woff[32], s_wdiag[32];   // per-warp partials, added in warp order (same result every run)
     const int tid = threadIdx.x, nt = blockDim.x;
     for (int idx = tid; idx < b * b; idx += nt) {
         if (MODE >= 1) A[idx] = Ag[idx];
@@ -456,8 +503,7 @@ eigh_jacobi_kernel(int b, double *__restrict__ Ag, double *__restrict__ w, doubl
     }
     __syncthreads();
     for (int sweep = 0; sweep < max_sweeps; sweep++) {
-        if (tid == 0) { s_off = 0.0; s_diag = 0.0; }
-        __syncthreads();
+        __syncthreads();                 // the previous sweep has read s_woff / s_wdiag
         double off = 0.0, dg = 0.0;
         for (int idx = tid; idx < b * b; idx += nt) {
             const int i = idx / b, j = idx - i * b;
@@ -468,8 +514,10 @@ eigh_jacobi_kernel(int b, double *__restrict__ Ag, double *__restrict__ w, doubl
             off += __shfl_xor_sync(0xffffffffu, off, o);
             dg += __shfl_xor_sync(0xffffffffu, dg, o);
         }
-        if ((tid & 31) == 0) { atomicAdd(&s_off, off); atomicAdd(&s_diag, dg); }
+        if ((tid & 31) == 0) { s_woff[tid >> 5] = off; s_wdiag[tid >> 5] = dg; }
         __syncthreads();
+        double s_off = 0.0, s_diag = 0.0;
+        for (int w = 0; w < (nt >> 5); w++) { s_off += s_woff[w]; s_diag += s_wdiag[w]; }
         if (s_off <= rel_tol * rel_tol * (s_diag + s_off) || s_diag + s_off == 0.0) break;
         for (int r = 0; r < m - 1; r++) {
             if (tid < half) {
@@ -562,7 +610,7 @@ eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict
     double *A = sh + 3 * half + 2;                // b x ld
     double *ZT = ZT_GLOBAL ? Ztg : A + (size_t)b * ld;   // ZT[j][k] = component k of eigenvector j
     const int ldz = ZT_GLOBAL ? b : ld;
-    __shared__ double s_off, s_diag;
+    __shared__ double s_woff[32], s_wdiag[32];   // per-warp partials, added in warp order (same result every run)
     const int tid = threadIdx.x, nt = blockDim.x;
     for (int idx = tid; idx < b * b; idx += nt) {
         const int i = idx / b, j = idx - i * b;
@@ -574,8 +622,7 @@ eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict
     const int bl_i0 = tid / half, bl_j0 = tid - bl_i0 * half, bl_di = nt / half, bl_dj = nt - bl_di * half;
     __syncthreads();
     for (int sweep = 0; sweep < max_sweeps; sweep++) {
-        if (tid == 0) { s_off = 0.0; s_diag = 0.0; }
-        __syncthreads();
+        __syncthreads();                 // the previous sweep has read s_woff / s_wdiag
         double off = 0.0, dg = 0.0;
         for (int i = zb_i0, j = zb_k0; i < b;) {
             const double v = A[i * ld + j];
@@ -587,8 +634,10 @@ eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict
             off += __shfl_xor_sync(0xffffffffu, off, o);
             dg += __shfl_xor_sync(0xffffffffu, dg, o);
         }
-        if ((tid & 31) == 0) { atomicAdd(&s_off, off); atomicAdd(&s_diag, dg); }
+        if ((tid & 31) == 0) { s_woff[tid >> 5] = off; s_wdiag[tid >> 5] = dg; }
         __syncthreads();
+        double s_off = 0.0, s_diag = 0.0;
+        for (int w = 0; w < (nt >> 5); w++) { s_off += s_woff[w]; s_diag += s_wdiag[w]; }
         if (s_off <= rel_tol * rel_tol * (s_diag + s_off) || s_diag + s_off == 0.0) break;
         for (int r = 0; r < m - 1; r++) {
             if (tid < half) {
@@ -787,7 +836,9 @@ int randn_launch(gemb_ctx *ctx, int64_t n, int b, uint64_t seed, uint64_t row_of
     return GEMB_OK;
 }
 
-__global__ void sumsq_kernel(int64_t count, const float *__restrict__ X, double *__restrict__ out) {
+// block sums of squares -> part[blockIdx.x] (blockDim.x = 256)
+__global__ void sumsq_kernel(int64_t count, const float *__restrict__ X, double *__restrict__ part) {
+    __shared__ double s_w[8];
     double acc = 0.0;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count;
          i += (int64_t)gridDim.x * blockDim.x) {
@@ -795,18 +846,28 @@ __global__ void sumsq_kernel(int64_t count, const float *__restrict__ X, double 
         acc += v * v;
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(out, acc);
+    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int w = 0; w < 8; w++) s += s_w[w];
+        part[blockIdx.x] = s;
+    }
 }
 
 int sumsq_launch(gemb_ctx *ctx, int64_t count, const float *X, double *out_dev) {
-    GEMB_CUDA(cudaMemsetAsync(out_dev, 0, sizeof(double), ctx->stream));
-    if (count == 0) return GEMB_OK;
+    if (count == 0) {
+        GEMB_CUDA(cudaMemsetAsync(out_dev, 0, sizeof(double), ctx->stream));
+        return GEMB_OK;
+    }
     int grid = ctx->sm_count * 8;
     if ((int64_t)grid * 256 > count) grid = (int)((count + 255) / 256);
-    sumsq_kernel<<<grid, 256, 0, ctx->stream>>>(count, X, out_dev);
+    double *part = nullptr;
+    GEMB_TRY(red_scratch(ctx, (size_t)grid, &part));
+    sumsq_kernel<<<grid, 256, 0, ctx->stream>>>(count, X, part);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    return GEMB_OK;
+    return sum_partials_launch(ctx, grid, 1, part, out_dev);
 }
 
 __global__ void scale_kernel(int64_t count, float s, float *__restrict__ X) {
@@ -843,7 +904,7 @@ extern "C" int gemb_gram(gemb_ctx *c, int64_t n, const float *P, int b1, const f
     GEMB_CUDA(dmalloc(&dG, sizeof(double) * (size_t)b1 * b2));
     int s = use_tensor_cores ? gram_tc_launch(c, n, dP, b1, Q ? dQ : dP, b2, dG)
                              : gram_fp32_launch(c, n, dP, b1, Q ? dQ : dP, b2, dG);
-    if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_gram: shape (n=%lld, b1=%d, b2=%d) not supported by the tcgen05 kernel", (long long)n, b1, b2);
+    if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_gram: shape (n=%lld, b1=%d, b2=%d) not supported by the tensor-core kernel", (long long)n, b1, b2);
     if (s == GEMB_OK) {
         cudaError_t e = cudaMemcpyAsync(G_out, dG, sizeof(double) * (size_t)b1 * b2, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -866,7 +927,7 @@ extern "C" int gemb_apply(gemb_ctx *c, int64_t n, const float *Q, int b1, const 
     GEMB_CUDA(cudaMemcpyAsync(dM, M, sizeof(float) * (size_t)b1 * b2, cudaMemcpyHostToDevice, c->stream));
     int s = use_tensor_cores ? apply_tc_launch(c, n, dQ, b1, dM, b2, b2, dO, b2)
                              : apply_fp32_launch(c, n, dQ, b1, dM, b2, b2, dO, b2);
-    if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_apply: shape (n=%lld, b1=%d, b2=%d) not supported by the tcgen05 kernel", (long long)n, b1, b2);
+    if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_apply: shape (n=%lld, b1=%d, b2=%d) not supported by the tensor-core kernel", (long long)n, b1, b2);
     if (s == GEMB_OK) {
         cudaError_t e = cudaMemcpyAsync(Out, dO, sizeof(float) * (size_t)n * b2, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);

@@ -567,6 +567,42 @@ static int orth_rotated(HopeWork &W, const float *F, float *tmp, float *dst) {
     return GEMB_OK;
 }
 
+// V[:, j] <- Rn[:, j] for the columns j whose squared norm G[j][j] is below 1/2 (V orthonormal: the zeroed ones)
+__global__ void refill_cols_kernel(int64_t count, int b, const double *__restrict__ G, const float *__restrict__ Rn,
+                                   float *__restrict__ V) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+        const int j = (int)(i % b);
+        if (G[(size_t)j * b + j] < 0.5) V[i] = Rn[i];
+    }
+}
+
+// Columns that the rank test of the CholeskyQR zeroed stay zero under every later filter, and their Ritz value 0 becomes
+// the smallest |f| of the block, which collapses the damped interval onto 0 and makes further columns dependent.  When the
+// last orthonormalisation of V dropped columns, they are replaced by Gaussian columns (seed per round) and V is
+// orthonormalised again (two CholeskyQR passes); a full-rank V is left untouched.  s1, s2: scratch blocks.
+static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t seed) {
+    gemb_ctx *c = W.c;
+    const int b = W.b;
+    int rank = b;
+    GEMB_CUDA(cudaMemcpyAsync(&rank, W.rank_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    if (rank >= b) return GEMB_OK;      // the Gram is all-reduced: every rank takes the same branch
+    GEMB_TRY(randn_launch(c, W.rows, b, seed, (uint64_t)W.g->row0, s1));
+    GEMB_TRY(gram_full(W, V, V, W.G));
+    const int64_t count = W.rows * (int64_t)b;
+    if (count > 0) {
+        const int grid = (int)std::min<int64_t>((count + 255) / 256, (int64_t)c->sm_count * 8);
+        refill_cols_kernel<<<grid, 256, 0, c->stream>>>(count, b, W.G, s1, V);
+        GEMB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    GEMB_TRY(gram_full(W, V, V, W.G));
+    GEMB_TRY(cholqr_pass(W, W.G, V, s2));
+    GEMB_TRY(gram_full(W, s2, s2, W.G));
+    GEMB_TRY(cholqr_pass(W, W.G, s2, V));
+    return GEMB_OK;
+}
+
 // ------------------------------------------------------------------------------------ symmetric solver
 static inline double katz_f(double beta, double l) { return beta * l / (1.0 - beta * l); }
 constexpr int GEMB_SWITCH_TO_LANCZOS = 1000;   // internal status of hope_symmetric (algorithm = 0 on a skewed spectrum)
@@ -748,7 +784,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         const double growth = xL + sqrt(std::max(xL * xL - 1.0, 0.0));
         np.deg = o.cheb_degree;
         // opts.cheb_range_log2 (default 8; GEMB_CHEB_RANGE_LOG2 overrides it for experiments): the column scaling inside the
-        // Ritz-rotated CholeskyQR tolerates far more than 2^8 on the SBM spectrum -- measured in profiles/r02c_solver_sweep.md:
+        // Ritz-rotated CholeskyQR tolerates far more than 2^8 on the SBM spectrum (scripts/exp_solver.py sweeps the settings):
         // 2^14 with degree 16 reaches a residual of 3.0e-3 in 4 rounds / 42 sweeps (the bench setting) where 2^8 with degree 8
         // needed 8 rounds / 56 sweeps for 4.0e-3.  The library default stays conservative (tight-tolerance solves).
         const double range_log2 = getenv("GEMB_CHEB_RANGE_LOG2") ? atof(getenv("GEMB_CHEB_RANGE_LOG2")) : (double)o.range_log2;
@@ -757,6 +793,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         if (!filtered) {
             if (np.deg < 2) {                                          // A V is already there: one power step
                 GEMB_TRY(orth_rotated(W, AV, pool[0], V));
+                GEMB_TRY(refill_dropped(W, V, pool[0], pool[1], o.seed + 7919ull * (uint64_t)it));
                 GEMB_TRY(publish(W, V, b));
                 plan = np;
                 continue;
@@ -769,6 +806,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         for (float *cand : {pool[0], pool[1], pool[2], AV})
             if (cand != filtered) { tmp = cand; break; }
         GEMB_TRY(orth_rotated(W, filtered, tmp, V));
+        GEMB_TRY(refill_dropped(W, V, tmp, filtered, o.seed + 7919ull * (uint64_t)it));
         GEMB_TRY(publish(W, V, b));
     }
 
@@ -1313,10 +1351,10 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         W.halo = hflag == 1;
         if (W.halo) {
             // Wire format of the halo copies: fp32.  The fp16 format (common.cuh) is an EXPERIMENT that did not pay and is
-            // only reachable with GEMB_WIRE=fp16-experimental: at 2 ranks the branchy mixed-precision gather costs more
-            // than the halved pushes save (63.6 ms against 42.7 ms per solve, one more filter round to reach the same
-            // residual); at 4 and 8 ranks the run returned after 2 rounds with a zero residual (every column dropped by
-            // the rank test of the Cholesky: a non-finite value entered a block) -- not debugged (profiles/r02_multi_gpu.md).
+            // only reachable with GEMB_WIRE=fp16-experimental: at 2 ranks the branchy mixed-precision gather cost more
+            // than the halved pushes saved (and one more filter round to reach the same residual); at 4 and 8 ranks the run
+            // returned after 2 rounds with a zero residual (every column dropped by the rank test of the Cholesky: a
+            // non-finite value entered a block) -- not debugged.
             const char *we = getenv("GEMB_WIRE");
             W.wire_half = we && !strcmp(we, "fp16-experimental");
         }

@@ -3,7 +3,7 @@
 //
 //   reference                                                         here
 //   static_graph_embedding.py:48-65  A_hat[i][j] = get_edge_weight    gemb_recon_create: A_hat = L R^T on the device,
-//     (n^2 Python calls of hope.py:43-44 / node2vec.py:56-57)           64-column panels through the tcgen05 3xTF32
+//     (n^2 Python calls of hope.py:43-44 / node2vec.py:56-57)           64-column panels through the wgmma 3xTF32
 //                                                                       kernel of apply_tc.cu (CUDA-core tile kernel
 //                                                                       when the shape does not fit), diagonal zeroed
 //   evaluation_util.py:20-36   scan adj for entries > 0               never materialised on the host: the kernels
@@ -17,7 +17,7 @@
 //
 // Layout: A_hat is n x n_pad fp32, n_pad = 64 * ceil(n / 64), PANEL-major: element (i, j) at
 // ((j / 64) * n + i) * 64 + j % 64 -- each 64-column panel is the contiguous n x 64 output of one apply launch
-// (the tensor-core kernel stores whole 128-row tiles with one bulk copy).  Padded columns hold 0.
+// (ldo = 64: the rows of one panel are adjacent).  Padded columns hold 0.
 // Roofline: HBM writes of 4 n^2 bytes for the product (k = 64: 32 flop per byte written, far below the tensor
 // pipe), HBM reads of 4 n^2 bytes per counting pass.
 #include "common.cuh"

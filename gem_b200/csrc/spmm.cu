@@ -174,14 +174,13 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
     if (has_push) halo_push_row(P, row, G, c, r);
 }
 
-// ---- v3 (sm_100a): one CTA per row TILE (passes * rows_per_cta consecutive rows); the tile's slice of the column-id
+// ---- v3 (TMA-staged): one CTA per row TILE (passes * rows_per_cta consecutive rows); the tile's slice of the column-id
 // (and value) arrays -- one contiguous range of the CSR -- is staged into shared memory by ONE TMA bulk copy
 // (cp.async.bulk + mbarrier complete_tx) issued by thread 0 while every row group fetches its row offsets; the other
 // resident CTAs of the SM hide the copy's latency.  The row groups then read their column ids from shared memory: the
 // dependent chain per row drops from indptr -> indices -> X (three global round trips) to indptr -> X, and the
-// ~nnz/4 broadcast LDGs of v1 (one L1 wavefront each) leave the L1 data pipe to the gathers.  Measured in
-// scripts/spmm_lab.cu (profiles/r02_spmm_lab.md): on par with v1 at 4 passes; the persistent 2-slot ring this replaced
-// lost 4 % to the per-tile CTA barrier, and evict-first hints on the streaming operands changed nothing.  A tile whose
+// ~nnz/4 broadcast LDGs of v1 (one L1 wavefront each) leave the L1 data pipe to the gathers.  scripts/spmm_lab.cu times
+// the variants against each other (GEMB_SPMM=v1 and GEMB_SPMM_PASSES select them in the library).  A tile whose
 // slice exceeds the staging buffer (hubs) reads its ids from global memory as v1 does; rows above SPMM_HEAVY_DEG still go
 // to the chunk kernels.
 constexpr int BULK_CAP = 3072;                 // staged ids per tile (+ up to 3 of alignment slack + 4 of over-read)

@@ -1,4 +1,4 @@
-"""Graph Factorization on a B200 -- drop-in for reference gem/embedding/gf.py:12-108 (SURVEY 8(f) rank 4).
+"""Graph Factorization on an H100 -- drop-in for reference gem/embedding/gf.py:12-108 (SURVEY 8(f) rank 4).
 
 Same class name, hyper-parameters (d, eta, regu, max_iter, print_step; data_set accepted), method name ('graph_factor_sgd'),
 call signature, error behaviour (ValueError('graph needed')), start (0.01 * np.random.randn(n, d) from NumPy's global RNG, gf.py:94),

@@ -1,10 +1,10 @@
-"""HOPE on a B200 -- drop-in for reference gem/embedding/hope.py:8-44.
+"""HOPE on an H100 -- drop-in for reference gem/embedding/hope.py:8-44.
 
 Same class name, hyper-parameters (d, beta), method name ('hope_gsvd'), call signature
 (learn_embedding(graph=None, is_weighted=False, no_python=False)), error behaviour
 (ValueError('graph needed')), row order (list(graph.nodes), SURVEY F6), column layout
 ([U sqrt(S) | V sqrt(S)], sigma ascending) and get_edge_weight.  The arithmetic runs in
-libgemb200.so (CUDA, sm_100a); there is no CPU path -- without a GPU learn_embedding raises
+libgemb200.so (CUDA, sm_90a); there is no CPU path -- without a GPU learn_embedding raises
 RuntimeError.
 
 Extra, optional hyper-parameters (defaults keep reference call sites working unchanged):

@@ -1,4 +1,4 @@
-"""Laplacian Eigenmaps on a B200 -- drop-in for reference gem/embedding/lap.py:8-42 (SURVEY 8(f) rank 4).
+"""Laplacian Eigenmaps on an H100 -- drop-in for reference gem/embedding/lap.py:8-42 (SURVEY 8(f) rank 4).
 
 Same class name, hyper-parameter (d), method name ('lap_eigmap_svd'), call signature, error behaviour
 (ValueError('graph needed')), row order (list(graph.nodes)), result (eigenvectors 1..d of the normalised Laplacian of the
@@ -6,7 +6,7 @@ UNDIRECTED graph, ascending eigenvalue, the first one dropped -- lap.py:25-32), 
 get_edge_weight (:39-42).  The reference calls scipy.sparse.linalg.eigs(l_sym, k=d+1, which='SM'); here the same
 eigenvectors come from the d+1 LARGEST algebraic eigenpairs of A_hat = D^-1/2 W D^-1/2 (L_sym = I - A_hat on the vertices
 that have edges), computed by the Chebyshev-filtered subspace iteration of libgemb200.so (gemb_hope with
-opts.spectral_mode = 1: the CSR SpMM, tcgen05 Gram / apply and Rayleigh-Ritz kernels HOPE uses) -- no shift-invert, no CPU path.
+opts.spectral_mode = 1: the CSR SpMM, tensor-core Gram / apply and Rayleigh-Ritz kernels HOPE uses) -- no shift-invert, no CPU path.
 
 Extra, optional hyper-parameters: tol (default 1e-6: relative change of every wanted eigenvalue between two Rayleigh-Ritz rounds;
 stop_rule=1 switches to the residual estimate, which fp32 Gram matrices cannot certify below ~3e-4), max_iters, oversample,

@@ -1,4 +1,4 @@
-"""Locally Linear Embedding on a B200 -- drop-in for reference gem/embedding/lle.py:10-40 (SURVEY 8(f) rank 4).
+"""Locally Linear Embedding on an H100 -- drop-in for reference gem/embedding/lle.py:10-40 (SURVEY 8(f) rank 4).
 
 Same class name, hyper-parameter (d), method name ('lle_svd'), call signature, error behaviour (ValueError('graph needed')),
 row order (list(graph.nodes)), result (right singular vectors 1..d of M = I - D^-1 W for the d+1 smallest singular values of
@@ -7,7 +7,7 @@ the UNDIRECTED graph, ascending, the first one dropped -- lle.py:25-32) and get_
 The reference calls scipy.sparse.linalg.svds(I - P, k=d+1, which='SM').  Here: the right singular vectors of M for its smallest
 singular values are the eigenvectors of C = c I - M^T M for its LARGEST eigenvalues (c = ||M||_1 ||M||_inf >= ||M||_2^2), and
 those come from the Chebyshev-filtered subspace iteration of libgemb200.so (gemb_hope, opts.spectral_mode = 1) -- the same CSR SpMM,
-tcgen05 Gram / apply and Rayleigh-Ritz kernels HOPE and LaplacianEigenmaps run on.  First version: C is formed explicitly on the
+tensor-core Gram / apply and Rayleigh-Ritz kernels HOPE and LaplacianEigenmaps run on.  First version: C is formed explicitly on the
 host (scipy.sparse product P^T P, sum_v deg(v)^2 entries -- fine for bounded degrees, not for power-law hubs); applying M and M^T as
 two fused sweeps inside the solver instead is the next step (DESIGN.md section 9).  No CPU path for the solve.
 

@@ -1,4 +1,4 @@
-"""node2vec on a B200 -- drop-in for reference gem/embedding/node2vec.py:8-57.
+"""node2vec on an H100 -- drop-in for reference gem/embedding/node2vec.py:8-57.
 
 The reference writes `tempGraph.graph`, runs the prebuilt SNAP executable gem/c_exe/node2vec with
 `-d -l -r -k -e -p -q -v -dr -w` (node2vec.py:35-46) and parses `tempGraph.emb`

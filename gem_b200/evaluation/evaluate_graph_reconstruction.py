@@ -1,4 +1,4 @@
-"""evaluateStaticGraphReconstruction on a B200 -- drop-in for reference
+"""evaluateStaticGraphReconstruction on an H100 -- drop-in for reference
 gem/evaluation/evaluate_graph_reconstruction.py:8-46 (same arguments, same return tuple).
 
 The reference materialises the n x n reconstruction with n^2 Python calls (static_graph_embedding.py:59-64),

@@ -1,5 +1,5 @@
 /*
- * include/gemb200.h -- C ABI of libgemb200.so, the B200 (sm_100a) core behind GEM's
+ * include/gemb200.h -- C ABI of libgemb200.so, the H100 (sm_90a) core behind GEM's
  * StaticGraphEmbedding plugin API for HOPE and node2vec.
  *
  * The reference has no FFI for this path: HOPE is four NumPy/SciPy lines
@@ -110,13 +110,13 @@ int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, 
               float *Y);
 
 /* Test hook for the tensor-core contraction: G (b1 x b2, fp64, row-major) = P^T Q over n rows; P, Q host
- * fp32 row-major (Q == NULL means Q = P).  use_tensor_cores: 1 = tcgen05 kernel (GEMB_ERR_UNSUPPORTED if the
+ * fp32 row-major (Q == NULL means Q = P).  use_tensor_cores: 1 = wgmma kernel (GEMB_ERR_UNSUPPORTED if the
  * shape does not fit it), 0 = CUDA-core fp32 kernel. */
 int gemb_gram(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, int use_tensor_cores,
               double *G_out);
 
 /* Test hook for the tall-skinny product Out (n x b2) = Q (n x b1) * M (b1 x b2), host fp32 row-major buffers.
- * use_tensor_cores: 1 = tcgen05 kernel, 0 = CUDA-core kernel. */
+ * use_tensor_cores: 1 = wgmma kernel, 0 = CUDA-core kernel. */
 int gemb_apply(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const float *M, int b2, int use_tensor_cores,
                float *Out);
 

@@ -7,7 +7,7 @@
 //   tile  : panel-major + the diagonal block of every R-row tile staged into shared memory by one TMA bulk copy;
 //           neighbours inside the tile are read from shared memory (an SBM community is a diagonal block), the
 //           `gamma * X[row]` term comes from the staged tile for free
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -o /tmp/spmm_lab scripts/spmm_lab.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -o /tmp/spmm_lab scripts/spmm_lab.cu
 // Run:   /tmp/spmm_lab indptr.bin indices.bin   (raw int32 arrays written by scripts/spmm_lab.py)
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -9,7 +9,7 @@ d = '/dev/shm' if os.path.isdir('/dev/shm') else '/tmp'
 csr.indptr.astype(np.int32).tofile(d + '/lab_indptr.bin')
 csr.indices.astype(np.int32).tofile(d + '/lab_indices.bin')
 exe = '/tmp/spmm_lab'
-subprocess.check_call(['nvcc', '-O3', '-std=c++17', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-o', exe,
+subprocess.check_call(['nvcc', '-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-o', exe,
                        os.path.join(os.path.dirname(os.path.abspath(__file__)), 'spmm_lab.cu')])
 mode = sys.argv[2:3]          # 'quick': row-major variants only
 subprocess.check_call([exe, d + '/lab_indptr.bin', d + '/lab_indices.bin'] + mode)

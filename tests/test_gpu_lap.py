@@ -82,7 +82,7 @@ def test_sbm1024_golden_d128(native_lib):
 
 
 def test_large_sbm_against_sparse_oracle(native_lib):
-    """n = 100 000 (tcgen05 Gram / apply path, TMA-staged SpMM with edge weights): eigenvalues against scipy eigsh on the same
+    """n = 100 000 (tensor-core Gram / apply path, TMA-staged SpMM with edge weights): eigenvalues against scipy eigsh on the same
     operator, the community eigenvectors as a subspace."""
     import lap_oracle as lo
     import hope_oracle as ho

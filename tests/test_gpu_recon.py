@@ -92,8 +92,8 @@ def test_evaluation_matches_oracle_and_reference_goldens(gpu_ctx, eval_oracle, n
 
 @pytest.mark.parametrize('split,d,n', [(True, 128, 4500), (False, 128, 4200), (True, 32, 5000)])
 def test_large_reconstruction_tensor_core_path(gpu_ctx, eval_oracle, split, d, n):
-    """n >= 4096: the 64-column panels go through the tcgen05 3xTF32 kernel when the factor width fits (k <= 64 ...
-    k = 128 falls back to the CUDA-core tile kernel); n not a multiple of 64 exercises the padded last panel.
+    """n >= 4096: the 64-column panels go through the wgmma 3xTF32 kernel (128-row tiles for k <= 64, 64-row tiles for
+    k = 128); n not a multiple of 64 exercises the padded last panel.
     Ranks / n_pred / top-k selection are checked exactly against the oracle run on the GPU's own matrix."""
     from gem_b200 import _native
     eo = eval_oracle
