@@ -1,7 +1,6 @@
 // gem_b200/csrc/common.cuh -- shared declarations of libgemb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
-#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
@@ -136,17 +135,7 @@ struct HaloPushArgs {                 // by-value kernel argument: where the row
     const uint32_t *push_dst;
     float4 *peer[GEMB_MAX_RANKS];     // the SAME block on every rank (own rank unused)
     int64_t halo_row0;                // = n_shard: first halo row of a block
-    int half;                         // 1: the halo copies travel and are stored as fp16 (x GEMB_WIRE_SCALE), see below
 };
-// fp16 on the wire (VERDICT r1 "next" #2 allows a 16-bit wire format when the bench-setting parity test still passes).
-// At 8 ranks every SBM row goes to 3.3 peers: 950 MB of fp32 pushes per sweep and rank, 1.28 ms against 0.47 ms of
-// gathering (r02k).  A halo slot then holds `width` halves instead of floats, at the front of the same halo region:
-//   fp32: ((float*)block)[(n_shard + slot) * width + j]      fp16: ((__half*)(block + n_shard * width))[slot * width + j]
-// Values are multiplied by 2^12 on the way out: entries of orthonormalised / Chebyshev-normalised blocks are <= ~1, so the
-// scaled values stay far below 65504 while entries down to 1.5e-8 remain normal numbers (11-bit significand: 4.9e-4
-// relative rounding on the ~17 % of gathers that cross ranks).  Blocks whose entries are not bounded (the raw power
-// steps of the warm-up, the norm estimation, the residual check) always travel as fp32.
-constexpr float GEMB_WIRE_SCALE = 4096.f, GEMB_WIRE_INV_SCALE = 1.f / 4096.f;
 
 struct gemb_graph {
     gemb_ctx *ctx = nullptr;
@@ -169,17 +158,16 @@ namespace gemb {
 int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha,
                 const float *X, const float *X0, float *Y);
 // Y = alpha * A * X + gamma * Xself + delta * X0   (Xself / X0: row shards, may be null)
-// half_from > 0: X is a [local | halo] block whose halo rows (column ids >= half_from) are fp16 slots
 int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
                  float gamma, const float *Xself, float delta, const float *X0, float *Y,
-                 const HaloPushArgs *push = nullptr, int64_t half_from = 0);
+                 const HaloPushArgs *push = nullptr);
 
 // ---- halo.cu (multi-GPU)
 int halo_build(gemb_graph *g);                                   // collective; idempotent
 int halo_buffers(gemb_graph *g, int nbuf, int width);            // collective; (re)allocates + IPC-maps the work blocks
-int halo_push_launch(gemb_graph *g, int buf_index, int width, bool half);   // stand-alone push of a block's local rows
+int halo_push_launch(gemb_graph *g, int buf_index, int width);  // stand-alone push of a block's local rows
 int halo_barrier(gemb_graph *g);                                 // all ranks' pushes issued before it have landed
-void halo_push_args(const gemb_graph *g, int buf_index, HaloPushArgs *out, bool half = false);
+void halo_push_args(const gemb_graph *g, int buf_index, HaloPushArgs *out);
 int halo_free(gemb_graph *g);
 void halo_pool_release(gemb_ctx *c);                              // at context destruction (not collective)
 // Y = a P + c Q over the local rows of halo blocks, pushing Y's rows to the peers (Chebyshev first step)
@@ -220,30 +208,10 @@ int scale_launch(gemb_ctx *ctx, int64_t count, float s, float *X);
 __device__ __forceinline__ void halo_push_row(const HaloPushArgs &P, int64_t row, int G, int c, const float4 &r) {
     const int i0 = P.push_ptr[row], i1 = P.push_ptr[row + 1];
     if (i0 == i1) return;
-    if (P.half) {
-        const __half2 lo = __floats2half2_rn(r.x * GEMB_WIRE_SCALE, r.y * GEMB_WIRE_SCALE);
-        const __half2 hi = __floats2half2_rn(r.z * GEMB_WIRE_SCALE, r.w * GEMB_WIRE_SCALE);
-        uint2 h;
-        h.x = *(const uint32_t *)&lo; h.y = *(const uint32_t *)&hi;
-        for (int i = i0; i < i1; i++) {
-            const uint32_t d = P.push_dst[i];
-            uint2 *base = (uint2 *)(P.peer[d >> 29] + P.halo_row0 * G);
-            base[(int64_t)(d & 0x1fffffffu) * G + c] = h;
-        }
-    } else {
-        for (int i = i0; i < i1; i++) {
-            const uint32_t d = P.push_dst[i];
-            P.peer[d >> 29][(P.halo_row0 + (int64_t)(d & 0x1fffffffu)) * G + c] = r;
-        }
+    for (int i = i0; i < i1; i++) {
+        const uint32_t d = P.push_dst[i];
+        P.peer[d >> 29][(P.halo_row0 + (int64_t)(d & 0x1fffffffu)) * G + c] = r;
     }
-}
-// chunk c of row `col` of a [local | halo] block; HALF: halo rows (col >= n_loc) are fp16 slots
-template <bool HALF>
-__device__ __forceinline__ float4 halo_gather(const float4 *__restrict__ X, int col, int G, int c, int n_loc) {
-    if (!HALF || col < n_loc) return __ldg(X + (int64_t)col * G + c);
-    const uint2 h = __ldg((const uint2 *)(X + (int64_t)n_loc * G) + (int64_t)(col - n_loc) * G + c);
-    const float2 a = __half22float2(*(const __half2 *)&h.x), b = __half22float2(*(const __half2 *)&h.y);
-    return make_float4(a.x * GEMB_WIRE_INV_SCALE, a.y * GEMB_WIRE_INV_SCALE, b.x * GEMB_WIRE_INV_SCALE, b.y * GEMB_WIRE_INV_SCALE);
 }
 #endif
 

@@ -6,7 +6,6 @@
 // These replace numpy.linalg.qr / svd inside scipy's svds (hope.py:33 -> _svds.py:508-533).
 // fp32 data, fp32 FMA inside a CTA's partial sums, fp64 across CTAs and in the b x b algebra.
 #include "common.cuh"
-#include <stdlib.h>
 #include <algorithm>
 
 namespace gemb {
@@ -87,19 +86,10 @@ static int pick_tm(int b) {
 
 int gram_tc_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G);
 
-static int gram_mode() {   // GEMB_GRAM=fp32 forces the CUDA-core kernel (A/B testing); default = wgmma
-    static int mode = -1;
-    if (mode < 0) {
-        const char *e = getenv("GEMB_GRAM");
-        mode = (e && (e[0] == 'f' || e[0] == '0')) ? 0 : 1;
-    }
-    return mode;
-}
-
 int gram_fp32_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G);
 
 int gram_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G) {
-    if (gram_mode() == 1 && n >= 4096) {
+    if (n >= 4096) {
         const int s = gram_tc_launch(ctx, n, P, b1, Q, b2, G);
         if (s != GEMB_ERR_UNSUPPORTED) return s;
     }
@@ -233,19 +223,10 @@ apply_kernel(int64_t n, const float *__restrict__ Q, int b1, const float *__rest
 
 int apply_tc_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const float *M, int ldm, int b2, float *Out, int ldo);
 
-static int apply_mode() {   // GEMB_APPLY=fp32 forces the CUDA-core kernel; default = wgmma where the shape fits
-    static int mode = -1;
-    if (mode < 0) {
-        const char *e = getenv("GEMB_APPLY");
-        mode = (e && (e[0] == 'f' || e[0] == '0')) ? 0 : 1;
-    }
-    return mode;
-}
-
 int apply_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const float *M, int ldm, int b2,
                  float *Out, int ldo) {
     if (n == 0 || b2 == 0) return GEMB_OK;
-    if (apply_mode() == 1 && n >= 4096) {
+    if (n >= 4096) {
         const int s = apply_tc_launch(ctx, n, Q, b1, M, ldm, b2, Out, ldo);
         if (s != GEMB_ERR_UNSUPPORTED) return s;
     }
@@ -454,8 +435,7 @@ int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_
     const size_t small = sizeof(double) * 3 * (size_t)b;
     const size_t big = small + sizeof(double) * (size_t)b * b;
     const size_t fast = small + sizeof(double) * (size_t)b * (b | 1);
-    static const bool generic_only = getenv("GEMB_DENSE_GENERIC") != nullptr;   // A/B switch for the tests
-    if (fast <= 200 * 1024 && b <= 128 && !generic_only) {
+    if (fast <= 200 * 1024 && b <= 128) {
         static bool attr_fast = false;
         if (!attr_fast) {
             GEMB_CUDA(cudaFuncSetAttribute(chol_inverse_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -480,11 +460,10 @@ int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_
 // ------------------------------------------------------------------------------------ eigh
 // Two-sided cyclic Jacobi with round-robin (circle-method) pair ordering, one CTA, fp64.
 // A is destroyed; w ascending; Z column j <-> w[j].  Zt is b x b scratch.
-// MODE 2: A and Zt in shared memory (b <= 116); MODE 1: A in shared memory (b <= 165); MODE 0: global.
-template <int MODE>
+// A and Zt in global memory (eigh_launch takes it where the fast kernel's shared-memory matrix does not fit).
 __global__ void __launch_bounds__(1024)
-eigh_jacobi_kernel(int b, double *__restrict__ Ag, double *__restrict__ w, double *__restrict__ Z,
-                   double *__restrict__ Ztg, int max_sweeps, double rel_tol) {
+eigh_jacobi_kernel(int b, double *__restrict__ A, double *__restrict__ w, double *__restrict__ Z,
+                   double *__restrict__ Zt, int max_sweeps, double rel_tol) {
     extern __shared__ double sh[];
     const int m = (b + 1) & ~1;     // even number of players; index >= b is a dummy
     const int half = m / 2;
@@ -492,15 +471,9 @@ eigh_jacobi_kernel(int b, double *__restrict__ Ag, double *__restrict__ w, doubl
     double *sn = sh + half;         // half
     int *pp = (int *)(sh + 2 * half);
     int *qq = pp + half;
-    double *mat = sh + 3 * half + 2;
-    double *A = MODE >= 1 ? mat : Ag;
-    double *Zt = MODE >= 2 ? mat + (size_t)b * b : Ztg;
     __shared__ double s_woff[32], s_wdiag[32];   // per-warp partials, added in warp order (same result every run)
     const int tid = threadIdx.x, nt = blockDim.x;
-    for (int idx = tid; idx < b * b; idx += nt) {
-        if (MODE >= 1) A[idx] = Ag[idx];
-        Zt[idx] = (idx / b == idx % b) ? 1.0 : 0.0;
-    }
+    for (int idx = tid; idx < b * b; idx += nt) Zt[idx] = (idx / b == idx % b) ? 1.0 : 0.0;
     __syncthreads();
     for (int sweep = 0; sweep < max_sweeps; sweep++) {
         __syncthreads();                 // the previous sweep has read s_woff / s_wdiag
@@ -595,7 +568,8 @@ eigh_jacobi_kernel(int b, double *__restrict__ Ag, double *__restrict__ w, doubl
 //     16-byte and one 8-byte load, the leading dimension is odd (conflict-free row and column walks).
 // ZT_GLOBAL (112 < b <= 164, the Rayleigh-Ritz matrix of the thick-restart Lanczos solver): A alone fills the shared
 // memory, the eigenvector accumulator lives in global memory (L2 resident, 200 KB) and is updated by coalesced row
-// walks -- the generic MODE 1 kernel needed 15.2 ms for b = 160 (10.9 us per Jacobi round, 43 % of an R-MAT solve).
+// walks -- a generic kernel with A in shared memory needed 15.2 ms for b = 160 (10.9 us per Jacobi round, 43 % of an
+// R-MAT solve).
 template <bool ZT_GLOBAL>
 __global__ void __launch_bounds__(1024)
 eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict__ w, double *__restrict__ Z,
@@ -749,12 +723,10 @@ eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict
 int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch, double rel_tol) {
     const int half = ((b + 1) & ~1) / 2;
     const size_t base = sizeof(double) * (3 * half + 2);
-    const size_t one = sizeof(double) * (size_t)b * b;
     const size_t cap = 220 * 1024;
-    static const bool generic_only = getenv("GEMB_DENSE_GENERIC") != nullptr;
     const size_t fast = base + 2 * sizeof(double) * (size_t)b * (b | 1);
     const size_t fast_a = base + sizeof(double) * (size_t)b * (b | 1);       // A only; eigenvectors in global memory
-    if ((fast <= cap || fast_a <= cap) && !generic_only) {
+    if (fast <= cap || fast_a <= cap) {
         static bool attr_fast = false;
         if (!attr_fast) {
             GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_fast_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
@@ -767,18 +739,7 @@ int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Z
         count_launch();
         return GEMB_OK;
     }
-    static bool attr_set = false;
-    if (!attr_set) {
-        GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
-        GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
-        attr_set = true;
-    }
-    if (base + 2 * one <= cap)
-        eigh_jacobi_kernel<2><<<1, 1024, base + 2 * one, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
-    else if (base + one <= cap)
-        eigh_jacobi_kernel<1><<<1, 1024, base + one, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
-    else
-        eigh_jacobi_kernel<0><<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
+    eigh_jacobi_kernel<<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     return GEMB_OK;

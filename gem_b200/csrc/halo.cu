@@ -314,13 +314,12 @@ int halo_buffers(gemb_graph *g, int nbuf, int width) {
     return GEMB_OK;
 }
 
-void halo_push_args(const gemb_graph *g, int bi, HaloPushArgs *out, bool half) {
+void halo_push_args(const gemb_graph *g, int bi, HaloPushArgs *out) {
     const gemb_halo &H = g->halo;
     out->push_ptr = H.push_ptr;
     out->push_dst = H.push_dst;
     for (int q = 0; q < GEMB_MAX_RANKS; q++) out->peer[q] = (float4 *)H.peer_buf[bi][q];
     out->halo_row0 = g->n_shard;
-    out->half = half ? 1 : 0;
 }
 
 // group of G threads per local row: copy the row into every peer slot that references it
@@ -334,14 +333,14 @@ halo_push_kernel(int64_t n_rows, int G, int rows_per_cta, const float4 *__restri
     halo_push_row(P, row, G, c, Y[row * G + c]);
 }
 
-int halo_push_launch(gemb_graph *g, int bi, int width, bool half) {
+int halo_push_launch(gemb_graph *g, int bi, int width) {
     gemb_ctx *c = g->ctx;
     if (g->n_local == 0 || g->halo.push_total == 0) return GEMB_OK;
     const int G = width / 4;
     GEMB_ARG(G >= 1 && G <= 256, "width");
     const int rpc = 256 / G;
     HaloPushArgs P;
-    halo_push_args(g, bi, &P, half);
+    halo_push_args(g, bi, &P);
     halo_push_kernel<<<(unsigned)((g->n_local + rpc - 1) / rpc), 256, 0, c->stream>>>(g->n_local, G, rpc, (const float4 *)g->halo.buf[bi], P);
     GEMB_CUDA(cudaGetLastError());
     count_launch();

@@ -55,10 +55,6 @@ struct HopeWork {
     bool halo = false;       // multi-GPU: needed-rows-only exchange over peer memory (halo.cu); buf[] = g->halo.buf[]
     int64_t pushes = 0;      // blocks whose rows were pushed to the peers
     double push_bytes_per_row = 0.0;   // sum over the pushed blocks of (bytes per pushed row): NVLink bytes out = this * push_rows
-    bool wire_half = false;  // halo mode: blocks with bounded entries travel as fp16 (common.cuh); decided once per call
-    bool wire_full_now = false;   // temporarily force fp32 pushes (raw power steps, norm estimation, residual check)
-    bool blk_half[5] = {false, false, false, false, false};   // wire format of the halo copies each work block holds
-    bool push_half() const { return wire_half && !wire_full_now; }
     int buf_index(const float *p) const { for (int i = 0; i < 5; i++) if (buf[i] == p) return i; return -1; }
     ~HopeWork() {
         if (!halo) for (auto p : buf) dfree(p);
@@ -99,20 +95,24 @@ static int comm_allreduce_f64(HopeWork &W, double *buf, size_t count) {
     return GEMB_OK;
 }
 
+// halo mode: ends the push of a width-wide block to the peers -- launching it first as a stand-alone push of work block
+// `push_bi` when >= 0 -- with the sweep barrier (timed as communication), and counts it
+static int end_push(HopeWork &W, int width, int push_bi = -1) {
+    GEMB_TRY(W.c->t_comm.begin(W.c->stream));
+    if (push_bi >= 0) GEMB_TRY(halo_push_launch(W.g, push_bi, width));
+    GEMB_TRY(halo_barrier(W.g));
+    GEMB_TRY(W.c->t_comm.end(W.c->stream));
+    W.pushes++;
+    W.push_bytes_per_row += 4.0 * width;
+    return GEMB_OK;
+}
+
 // halo mode: the local rows of block `buf` go to the peers that reference them, then the sweep barrier
 static int publish(HopeWork &W, const float *buf, int width) {
     if (!W.halo) return GEMB_OK;
     const int bi = W.buf_index(buf);
     GEMB_ARG(bi >= 0, "publish: not a work block");
-    const bool half = W.push_half();
-    GEMB_TRY(W.c->t_comm.begin(W.c->stream));
-    GEMB_TRY(halo_push_launch(W.g, bi, width, half));
-    GEMB_TRY(halo_barrier(W.g));
-    GEMB_TRY(W.c->t_comm.end(W.c->stream));
-    W.blk_half[bi] = half;
-    W.pushes++;
-    W.push_bytes_per_row += (half ? 2.0 : 4.0) * width;
-    return GEMB_OK;
+    return end_push(W, width, bi);
 }
 
 // Y(shard) = alpha * op(A) * X + gamma * X(shard) + delta * X0(shard).  Sharded: halo mode gathers from the block's own
@@ -126,21 +126,13 @@ static int dist_spmm3(HopeWork &W, bool transpose, int width, float alpha, const
         HaloPushArgs P;
         const int bo = W.buf_index(Y), bin = W.buf_index(Xshard);
         GEMB_ARG(bin >= 0, "spmm input is not a work block");
-        const bool half_out = W.push_half();
-        if (push_out) { GEMB_ARG(bo >= 0, "spmm output is not a work block"); halo_push_args(W.g, bo, &P, half_out); }
+        if (push_out) { GEMB_ARG(bo >= 0, "spmm output is not a work block"); halo_push_args(W.g, bo, &P); }
         if (timed) GEMB_TRY(W.c->t_spmm.begin(W.c->stream));
         GEMB_TRY(spmm3_launch(W.c, A, W.rows, width, alpha, Xshard, gamma, use_self ? Xshard : nullptr, delta, X0, Y,
-                              push_out ? &P : nullptr, W.blk_half[bin] ? W.g->n_shard : 0));
+                              push_out ? &P : nullptr));
         if (timed) { GEMB_TRY(W.c->t_spmm.end(W.c->stream)); W.spmm_wide++; }
         W.spmm_all++;
-        if (push_out) {
-            GEMB_TRY(W.c->t_comm.begin(W.c->stream));
-            GEMB_TRY(halo_barrier(W.g));
-            GEMB_TRY(W.c->t_comm.end(W.c->stream));
-            W.blk_half[bo] = half_out;
-            W.pushes++;
-            W.push_bytes_per_row += (half_out ? 2.0 : 4.0) * width;
-        }
+        if (push_out) return end_push(W, width);
         return GEMB_OK;
     }
     const float *Xfull = Xshard;
@@ -278,21 +270,14 @@ static int axpby_launch(HopeWork &W, float a, const float *P, float c, const flo
         const int G = W.b / 4, rpc = 256 / G, bo = W.buf_index(Y);
         GEMB_ARG(bo >= 0 && G <= 256, "axpby output is not a work block");
         HaloPushArgs H;
-        const bool half = W.push_half();
-        halo_push_args(W.g, bo, &H, half);
-        W.blk_half[bo] = half;
-        W.push_bytes_per_row += (half ? 2.0 : 4.0) * W.b;
+        halo_push_args(W.g, bo, &H);
         if (W.rows > 0) {
             axpby_push_kernel<<<(unsigned)((W.rows + rpc - 1) / rpc), 256, 0, W.c->stream>>>(
                 W.rows, G, rpc, a, (const float4 *)P, c, (const float4 *)Q, (float4 *)Y, H);
             GEMB_CUDA(cudaGetLastError());
             count_launch();
         }
-        GEMB_TRY(W.c->t_comm.begin(W.c->stream));
-        GEMB_TRY(halo_barrier(W.g));
-        GEMB_TRY(W.c->t_comm.end(W.c->stream));
-        W.pushes++;
-        return GEMB_OK;
+        return end_push(W, W.b);
     }
     if (count == 0) return GEMB_OK;
     int grid = W.c->sm_count * 8;
@@ -357,7 +342,6 @@ static int estimate_norm2(HopeWork &W, uint64_t seed, float *x, float *y, float 
     gemb_ctx *c = W.c;
     gemb_graph *g = W.g;
     const int pw = 4;
-    struct FullWire { HopeWork &w; bool old; FullWire(HopeWork &w_) : w(w_), old(w_.wire_full_now) { w.wire_full_now = true; } ~FullWire() { w.wire_full_now = old; } } fw(W);
     GEMB_TRY(randn_launch(c, W.rows, pw, seed ^ 0x5bd1e995u, (uint64_t)g->row0, x));
     double est = 0.0, prev = -1.0;
     for (int it = 0; it < 16; it++) {
@@ -625,26 +609,21 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     // (round 1 orthonormalised after every step: 4 x CholeskyQR2 = 3.5 ms of the 58 ms solve at S, for nothing -- the
     // block's condition number after three steps is (lambda_1 / lambda_b)^3, a few units on a community graph).  Should
     // the first Cholesky drop columns (skewed spectrum, rank-deficient A), the careful form below takes over.
-    bool careful = getenv("GEMB_WARMUP_CAREFUL") != nullptr;
+    GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, pool[0]));
+    GEMB_TRY(publish(W, pool[0], b));
+    GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[0], 0.f, false, 1.f, nullptr, pool[1], true, W.halo));
+    GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[1], 0.f, false, 1.f, nullptr, pool[2], true, W.halo));
+    GEMB_TRY(dist_spmm(W, false, b, 1.f, pool[2], nullptr, AV, true));
+    GEMB_TRY(gram_full(W, AV, AV, W.G));
+    GEMB_TRY(cholqr_pass(W, W.G, AV, pool[0]));
+    int rank1 = b;
+    GEMB_CUDA(cudaMemcpyAsync(&rank1, W.rank_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    const bool careful = rank1 < b;
     if (!careful) {
-        W.wire_full_now = true;     // raw (unnormalised) blocks: entries grow like lambda^3, not for the fp16 wire format
-        GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, pool[0]));
-        GEMB_TRY(publish(W, pool[0], b));
-        GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[0], 0.f, false, 1.f, nullptr, pool[1], true, W.halo));
-        GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[1], 0.f, false, 1.f, nullptr, pool[2], true, W.halo));
-        GEMB_TRY(dist_spmm(W, false, b, 1.f, pool[2], nullptr, AV, true));
-        W.wire_full_now = false;
-        GEMB_TRY(gram_full(W, AV, AV, W.G));
-        GEMB_TRY(cholqr_pass(W, W.G, AV, pool[0]));
-        int rank1 = b;
-        GEMB_CUDA(cudaMemcpyAsync(&rank1, W.rank_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        if (rank1 < b) careful = true;
-        else {
-            GEMB_TRY(gram_full(W, pool[0], pool[0], W.G));
-            GEMB_TRY(cholqr_pass(W, W.G, pool[0], V));
-            GEMB_TRY(publish(W, V, b));
-        }
+        GEMB_TRY(gram_full(W, pool[0], pool[0], W.G));
+        GEMB_TRY(cholqr_pass(W, W.G, pool[0], V));
+        GEMB_TRY(publish(W, V, b));
     }
     if (careful) {
         GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, pool[0]));
@@ -783,12 +762,11 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         const double xL = fabs(aL - np.c0) / np.e;
         const double growth = xL + sqrt(std::max(xL * xL - 1.0, 0.0));
         np.deg = o.cheb_degree;
-        // opts.cheb_range_log2 (default 8; GEMB_CHEB_RANGE_LOG2 overrides it for experiments): the column scaling inside the
+        // opts.cheb_range_log2 (default 8): the column scaling inside the
         // Ritz-rotated CholeskyQR tolerates far more than 2^8 on the SBM spectrum (scripts/exp_solver.py sweeps the settings):
         // 2^14 with degree 16 reaches a residual of 3.0e-3 in 4 rounds / 42 sweeps (the bench setting) where 2^8 with degree 8
         // needed 8 rounds / 56 sweeps for 4.0e-3.  The library default stays conservative (tight-tolerance solves).
-        const double range_log2 = getenv("GEMB_CHEB_RANGE_LOG2") ? atof(getenv("GEMB_CHEB_RANGE_LOG2")) : (double)o.range_log2;
-        if (growth > 1.0 + 1e-9) np.deg = std::min(np.deg, (int)floor(log(2.0 * exp2(range_log2)) / log(growth)));
+        if (growth > 1.0 + 1e-9) np.deg = std::min(np.deg, (int)floor(log(2.0 * exp2((double)o.range_log2)) / log(growth)));
 
         if (!filtered) {
             if (np.deg < 2) {                                          // A V is already there: one power step
@@ -893,7 +871,6 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         GEMB_CUDA(cudaMemsetAsync(STP, 0, blk, c->stream));
         GEMB_CUDA(cudaMemcpyAsync(dMP, MP.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
         GEMB_CUDA(cudaMemcpyAsync(dMQ, MQ.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
-        W.wire_full_now = true;     // the check measures the result against the fp32 operator: no fp16 copies here
         int s = apply_launch(c, W.rows, V, b, dMP, b, b, P, b);
         if (s == GEMB_OK) s = apply_launch(c, W.rows, V, b, dMQ, b, b, Q, b);
         if (s == GEMB_OK) s = publish(W, P, b);
@@ -1349,15 +1326,6 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         dfree(flag);
         if (r != ncclSuccess) { set_error("ncclAllReduce(halo agreement): %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
         W.halo = hflag == 1;
-        if (W.halo) {
-            // Wire format of the halo copies: fp32.  The fp16 format (common.cuh) is an EXPERIMENT that did not pay and is
-            // only reachable with GEMB_WIRE=fp16-experimental: at 2 ranks the branchy mixed-precision gather cost more
-            // than the halved pushes saved (and one more filter round to reach the same residual); at 4 and 8 ranks the run
-            // returned after 2 rounds with a zero residual (every column dropped by the rank test of the Cholesky: a
-            // non-finite value entered a block) -- not debugged.
-            const char *we = getenv("GEMB_WIRE");
-            W.wire_half = we && !strcmp(we, "fp16-experimental");
-        }
         if (!W.halo && o.verbose) fprintf(stderr, "[gemb_hope] halo exchange unavailable (%s); all-gather per sweep\n", gemb_last_error());
     }
     if (W.halo) {
@@ -1492,7 +1460,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         stats->halo_rows = W.halo ? g->halo.halo_rows : 0;
         stats->push_rows = W.halo ? g->halo.push_total : 0;
         stats->pushes = W.pushes;
-        stats->mg_mode = c->nranks == 1 ? 0 : (W.halo ? (W.wire_half ? 3 : 2) : 1);
+        stats->mg_mode = c->nranks == 1 ? 0 : (W.halo ? 2 : 1);
         stats->push_bytes = W.halo ? W.push_bytes_per_row * (double)g->halo.push_total : 0.0;
         stats->resid_est = R.resid_est;
         stats->dense_ms = c->t_dense.total_ms();

@@ -179,13 +179,12 @@ typedef struct {
     float resid_est;       /* stop_rule = 1: the residual estimate the last round stopped on (else -1) */
     int32_t mg_mode;       /* 0 = single GPU; 1 = all-gather of the block per sweep; 2 = needed-rows-only exchange over
                               NVLink peer memory (CUDA IPC): rows are stored into the peers' halo slots by the kernel
-                              that produces them; 3 = the same with fp16 halo copies: an experiment that did not pay
-                              (GEMB_WIRE=fp16-experimental only; see hope.cu) */
+                              that produces them.  3 (fp16 halo copies) is no longer produced. */
     int64_t halo_rows;     /* mg_mode 2: distinct remote rows this shard references */
     int64_t push_rows;     /* mg_mode 2: (row, peer) pairs this rank stores per exchanged block */
     int64_t pushes;        /* mg_mode 2: blocks exchanged in this call (NVLink bytes out = pushes*push_rows*4*block) */
     float beta_used;       /* the beta the solve ran with (differs from the argument when that was negative) */
-    double push_bytes;     /* mg_mode 2/3: bytes this rank stored into its peers over NVLink in this call */
+    double push_bytes;     /* mg_mode 2: bytes this rank stored into its peers over NVLink in this call */
 } gemb_hope_stats;
 
 /* X_out: n_local x d host buffer, or NULL to leave the result on the device (bench `value`).
