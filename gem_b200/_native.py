@@ -17,7 +17,7 @@ UNIQUE_ID_BYTES = 128
 EXPORTS = [
     'gemb_version', 'gemb_last_error', 'gemb_device_count', 'gemb_launch_count', 'gemb_ctx_create', 'gemb_ctx_destroy',
     'gemb_host_alloc', 'gemb_host_free', 'gemb_mem_trim', 'gemb_mem_cached_bytes', 'gemb_comm_unique_id', 'gemb_comm_init', 'gemb_graph_upload',
-    'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
+    'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
 ]
@@ -83,9 +83,11 @@ def lib():
     L.gemb_comm_init.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]
     L.gemb_graph_upload.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, ctypes.POINTER(vp)]
     L.gemb_graph_free.argtypes = [vp]
-    L.gemb_spmm.argtypes = [vp, ctypes.c_int, ctypes.c_int, f32, vp, vp, vp]
+    L.gemb_spmm.argtypes = [vp, ctypes.c_int, ctypes.c_int, f32, vp, f32, vp, f32, vp, vp]
     L.gemb_gram.argtypes = [vp, i64, vp, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp]
     L.gemb_apply.argtypes = [vp, i64, vp, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp]
+    L.gemb_chol_inverse.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.POINTER(ctypes.c_int)]
+    L.gemb_eigh.argtypes = [vp, ctypes.c_int, vp, f64, vp, vp]
     L.gemb_hope.argtypes = [vp, ctypes.c_int, f32, ctypes.POINTER(HopeOpts), vp, vp, ctypes.POINTER(HopeStats)]
     L.gemb_hope_svd_error.argtypes = [vp, ctypes.c_int, f32, vp, ctypes.c_int, ctypes.c_uint64, ctypes.POINTER(f64)]
     L.gemb_n2v_alias.argtypes = [vp, vp, vp, vp]
@@ -193,6 +195,27 @@ class Context:
         check(lib().gemb_apply(self._h, Q.shape[0], _ptr(Q), Q.shape[1], _ptr(M), M.shape[1], int(bool(tensor_cores)), _ptr(out)))
         return out
 
+    def chol_inverse(self, G):
+        """(Minv fp64, Minv fp32, rank): R^-1 of G = R^T R with the rank test of CholeskyQR (test hook)."""
+        G = np.ascontiguousarray(G, dtype=np.float64)
+        b = G.shape[0]
+        assert G.shape == (b, b)
+        M64 = np.empty((b, b), dtype=np.float64)
+        M32 = np.empty((b, b), dtype=np.float32)
+        rank = ctypes.c_int(-1)
+        check(lib().gemb_chol_inverse(self._h, b, _ptr(G), _ptr(M64), _ptr(M32), ctypes.byref(rank)))
+        return M64, M32, int(rank.value)
+
+    def eigh(self, G, rel_tol=1e-13):
+        """(w ascending, Z) of the symmetric G by the device Jacobi solver (test hook)."""
+        G = np.ascontiguousarray(G, dtype=np.float64)
+        b = G.shape[0]
+        assert G.shape == (b, b)
+        w = np.empty(b, dtype=np.float64)
+        Z = np.empty((b, b), dtype=np.float64)
+        check(lib().gemb_eigh(self._h, b, _ptr(G), float(rel_tol), _ptr(w), _ptr(Z)))
+        return w, Z
+
     def close(self):
         if self._h:
             lib().gemb_ctx_destroy(self._h)
@@ -266,12 +289,17 @@ class DeviceGraph:
                                       _ptr(data), _ptr(indptr_t), _ptr(indices_t), _ptr(data_t),
                                       ctypes.byref(self._h)))
 
-    def spmm(self, X, alpha=1.0, X0=None, transpose=False):
+    def spmm(self, X, alpha=1.0, X0=None, transpose=False, gamma=0.0, Xself=None, delta=1.0):
+        """Y = alpha op(A) X + gamma Xself + delta X0 (Xself, X0: n_local x b row shards or None; test hook)."""
         X = np.ascontiguousarray(X, dtype=np.float32)
         b = X.shape[1]
         X0 = None if X0 is None else np.ascontiguousarray(X0, dtype=np.float32)
+        Xself = None if Xself is None else np.ascontiguousarray(Xself, dtype=np.float32)
+        for a in (X0, Xself):
+            assert a is None or a.shape == (self.n_local, b)
         Y = np.empty((self.n_local, b), dtype=np.float32)
-        check(lib().gemb_spmm(self._h, int(bool(transpose)), b, float(alpha), _ptr(X), _ptr(X0), _ptr(Y)))
+        check(lib().gemb_spmm(self._h, int(bool(transpose)), b, float(alpha), _ptr(X), float(gamma), _ptr(Xself),
+                              float(delta), _ptr(X0), _ptr(Y)))
         return Y
 
     def hope(self, d, beta, out=None, want_output=True, **opts):

@@ -255,10 +255,13 @@ int apply_fp32_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const fl
 // scale free.  A pivot below PIV_EPS marks the column numerically dependent: its column of Minv is
 // zero (the orthonormalised block then carries a zero column, which stays zero under S).
 #define GEMB_PIV_EPS 1e-5
-// SMEM: the b x b matrix lives in shared memory for the whole factorization (b <= 160).
+// SMEM: the b x b matrix lives in shared memory for the whole factorization (b <= 166).
+// Gg is not __restrict__: without SMEM it is the work matrix that other threads write between barriers, and with
+// __restrict__ nvcc kept the pivot G[j][j] that every thread loaded before thread 0 replaced it by sqrt(G[j][j]) across
+// the barrier (all entries of a column of L but the first below the diagonal were divided by the pivot, not its root).
 template <bool SMEM>
 __global__ void __launch_bounds__(1024)
-chol_inverse_kernel(int b, double *__restrict__ Gg, float *__restrict__ Minv, double *__restrict__ Minv64,
+chol_inverse_kernel(int b, double *Gg, float *__restrict__ Minv, double *__restrict__ Minv64,
                     int *__restrict__ rank_out) {
     extern __shared__ double sh[];
     double *dscale = sh;           // b : 1/sqrt(G_jj) (0 if G_jj <= 0)
@@ -462,8 +465,8 @@ int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_
 // A is destroyed; w ascending; Z column j <-> w[j].  Zt is b x b scratch.
 // A and Zt in global memory (eigh_launch takes it where the fast kernel's shared-memory matrix does not fit).
 __global__ void __launch_bounds__(1024)
-eigh_jacobi_kernel(int b, double *__restrict__ A, double *__restrict__ w, double *__restrict__ Z,
-                   double *__restrict__ Zt, int max_sweeps, double rel_tol) {
+eigh_jacobi_kernel(int b, double *A, double *__restrict__ w, double *__restrict__ Z,
+                   double *Zt, int max_sweeps, double rel_tol) {   // A, Zt: written by other threads (no __restrict__)
     extern __shared__ double sh[];
     const int m = (b + 1) & ~1;     // even number of players; index >= b is a dummy
     const int half = m / 2;
@@ -557,7 +560,7 @@ eigh_jacobi_kernel(int b, double *__restrict__ A, double *__restrict__ w, double
     }
 }
 
-// Fast variant for b*(b|1)*16 bytes <= shared memory (b <= 112).  The generic kernel is ISSUE bound, not
+// Fast variant for b*(b|1)*16 bytes <= shared memory (b <= 117).  The generic kernel is ISSUE bound, not
 // bandwidth bound (ncu: 558 warp instructions per warp per round, 63 % issue-active, fp64 pipe 11 %): runtime
 // integer divisions and four parameter loads per element.  Here
 //   * the two-sided update A <- J^T A J is done per 2x2 BLOCK {p,q} x {r,s} of two rotation pairs by one thread
@@ -566,14 +569,14 @@ eigh_jacobi_kernel(int b, double *__restrict__ A, double *__restrict__ w, double
 //   * the eigenvector accumulator is kept transposed so that its update is a row walk;
 //   * (pair, column) indices advance incrementally (no division in the loops), rotation parameters are one
 //     16-byte and one 8-byte load, the leading dimension is odd (conflict-free row and column walks).
-// ZT_GLOBAL (112 < b <= 164, the Rayleigh-Ritz matrix of the thick-restart Lanczos solver): A alone fills the shared
+// ZT_GLOBAL (117 < b <= 167, the Rayleigh-Ritz matrix of the thick-restart Lanczos solver): A alone fills the shared
 // memory, the eigenvector accumulator lives in global memory (L2 resident, 200 KB) and is updated by coalesced row
 // walks -- a generic kernel with A in shared memory needed 15.2 ms for b = 160 (10.9 us per Jacobi round, 43 % of an
 // R-MAT solve).
 template <bool ZT_GLOBAL>
 __global__ void __launch_bounds__(1024)
 eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict__ w, double *__restrict__ Z,
-                        double *__restrict__ Ztg, int max_sweeps, double rel_tol) {
+                        double *Ztg, int max_sweeps, double rel_tol) {   // Ztg: as A of eigh_jacobi_kernel
     extern __shared__ __align__(16) unsigned char sh_fast[];
     double *sh = (double *)sh_fast;
     const int m = (b + 1) & ~1;
@@ -872,6 +875,56 @@ extern "C" int gemb_gram(gemb_ctx *c, int64_t n, const float *P, int b1, const f
         if (e != cudaSuccess) { set_error("gemb_gram: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
     }
     dfree(dP); dfree(dQ); dfree(dG);
+    return s;
+}
+
+// The b x b hooks run the solvers' own launchers, so b picks the kernel variant exactly as in a solve.  b is limited to
+// the solvers' block limit (gemb_hope: b <= 1024), which eigh_jacobi_kernel relies on (one rotation per thread).
+extern "C" int gemb_chol_inverse(gemb_ctx *c, int b, const double *G, double *Minv64_out, float *Minv32_out,
+                                 int *rank_out) {
+    using namespace gemb;
+    GEMB_ARG(c && G && Minv64_out && Minv32_out && rank_out && b > 0 && b <= 1024, "ctx/G/Minv/rank/b");
+    GEMB_CUDA(cudaSetDevice(c->device));
+    const size_t bb = (size_t)b * b;
+    double *dG = nullptr, *dM64 = nullptr;
+    float *dM32 = nullptr;
+    int *dRank = nullptr;
+    cudaError_t e = dmalloc(&dG, sizeof(double) * bb);
+    if (e == cudaSuccess) e = dmalloc(&dM64, sizeof(double) * bb);
+    if (e == cudaSuccess) e = dmalloc(&dM32, sizeof(float) * bb);
+    if (e == cudaSuccess) e = dmalloc(&dRank, sizeof(int));
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dG, G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream);
+    int s = e == cudaSuccess ? chol_inverse_launch(c, b, dG, dM32, dRank, dM64) : GEMB_ERR_CUDA;
+    if (s == GEMB_OK) {
+        e = cudaMemcpyAsync(Minv64_out, dM64, sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(Minv32_out, dM32, sizeof(float) * bb, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(rank_out, dRank, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    }
+    if (e != cudaSuccess) { set_error("gemb_chol_inverse: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
+    dfree(dG); dfree(dM64); dfree(dM32); dfree(dRank);
+    return s;
+}
+
+extern "C" int gemb_eigh(gemb_ctx *c, int b, const double *G, double rel_tol, double *w_out, double *Z_out) {
+    using namespace gemb;
+    GEMB_ARG(c && G && w_out && Z_out && b > 0 && b <= 1024 && rel_tol >= 0.0, "ctx/G/w/Z/b/rel_tol");
+    GEMB_CUDA(cudaSetDevice(c->device));
+    const size_t bb = (size_t)b * b;
+    double *dG = nullptr, *dw = nullptr, *dZ = nullptr, *dZs = nullptr;
+    cudaError_t e = dmalloc(&dG, sizeof(double) * bb);
+    if (e == cudaSuccess) e = dmalloc(&dw, sizeof(double) * b);
+    if (e == cudaSuccess) e = dmalloc(&dZ, sizeof(double) * bb);
+    if (e == cudaSuccess) e = dmalloc(&dZs, sizeof(double) * bb);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dG, G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream);
+    int s = e == cudaSuccess ? eigh_launch(c, b, dG, dw, dZ, dZs, rel_tol) : GEMB_ERR_CUDA;
+    if (s == GEMB_OK) {
+        e = cudaMemcpyAsync(w_out, dw, sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(Z_out, dZ, sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    }
+    if (e != cudaSuccess) { set_error("gemb_eigh: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
+    dfree(dG); dfree(dw); dfree(dZ); dfree(dZs);
     return s;
 }
 

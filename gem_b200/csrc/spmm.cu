@@ -290,20 +290,22 @@ int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, 
 
 using namespace gemb;
 
-extern "C" int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X,
-                         const float *X0, float *Y) {
+extern "C" int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma,
+                         const float *Xself, float delta, const float *X0, float *Y) {
     GEMB_ARG(g && X && Y, "graph/X/Y");
     GEMB_ARG(b > 0 && b % 4 == 0, "b must be a positive multiple of 4");
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
-    float *dX = nullptr, *dX0 = nullptr, *dY = nullptr;
+    float *dX = nullptr, *dXs = nullptr, *dX0 = nullptr, *dY = nullptr;
     const size_t full = sizeof(float) * (size_t)g->n * b, shard = sizeof(float) * (size_t)g->n_local * b;
     GEMB_CUDA(dmalloc(&dX, full ? full : 4));
     GEMB_CUDA(dmalloc(&dY, shard ? shard : 4));
+    if (Xself) GEMB_CUDA(dmalloc(&dXs, shard ? shard : 4));
     if (X0) GEMB_CUDA(dmalloc(&dX0, shard ? shard : 4));
     GEMB_CUDA(cudaMemcpyAsync(dX, X, full, cudaMemcpyHostToDevice, c->stream));
+    if (Xself) GEMB_CUDA(cudaMemcpyAsync(dXs, Xself, shard, cudaMemcpyHostToDevice, c->stream));
     if (X0) GEMB_CUDA(cudaMemcpyAsync(dX0, X0, shard, cudaMemcpyHostToDevice, c->stream));
-    int s = spmm_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX, dX0, dY);
+    int s = spmm3_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX, gamma, dXs, delta, dX0, dY);
     if (s == GEMB_OK) {
         cudaError_t e = cudaMemcpyAsync(Y, dY, shard, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -314,6 +316,7 @@ extern "C" int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const
     }
     dfree(dX);
     dfree(dY);
+    dfree(dXs);
     dfree(dX0);
     return s;
 }

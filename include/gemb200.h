@@ -103,11 +103,12 @@ int gemb_graph_upload(gemb_ctx *ctx, int64_t n, int64_t row0, int64_t n_local,
                       gemb_graph **out);
 int gemb_graph_free(gemb_graph *g);
 
-/* Test hook for the dominant kernel:  Y = X0 + alpha * op(A) * X   (X0 may be NULL).
- * X is the full n x b block, X0 and Y are the n_local x b row shards; all HOST, row-major fp32.
- * b must be a multiple of 4. */
-int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, const float *X0,
-              float *Y);
+/* Test hook for the dominant kernel:  Y = alpha * op(A) * X + gamma * Xself + delta * X0
+ * (Xself / X0 may be NULL: that term is left out; the Horner sweep is gamma = 0, delta = 1, the Chebyshev step
+ * passes Xself = the local rows of X).  X is the full n x b block, Xself, X0 and Y are the n_local x b row shards;
+ * all HOST, row-major fp32.  b must be a multiple of 4, <= 1024. */
+int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma, const float *Xself,
+              float delta, const float *X0, float *Y);
 
 /* Test hook for the tensor-core contraction: G (b1 x b2, fp64, row-major) = P^T Q over n rows; P, Q host
  * fp32 row-major (Q == NULL means Q = P).  use_tensor_cores: 1 = wgmma kernel (GEMB_ERR_UNSUPPORTED if the
@@ -119,6 +120,16 @@ int gemb_gram(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, 
  * use_tensor_cores: 1 = wgmma kernel, 0 = CUDA-core kernel. */
 int gemb_apply(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const float *M, int b2, int use_tensor_cores,
                float *Out);
+
+/* Test hooks for the single-CTA fp64 factorizations of the b x b matrices (1 <= b <= 1024; all HOST, row-major).
+ * The kernel variant is chosen by b, as in the solvers.
+ * chol_inverse: G symmetric -> Minv = R^-1 (upper triangular) with G = R^T R, as fp64 and as fp32 (the fp32 copy is
+ *   the fp64 result rounded); a column whose pivot of the diagonally scaled matrix D^-1/2 G D^-1/2 is <= 1e-5 is
+ *   dropped: its column of Minv is 0.  *rank_out = number of kept columns.
+ * eigh: G symmetric -> eigenvalues w (b, ascending) and eigenvectors Z (b x b, column j <-> w[j]) by cyclic Jacobi,
+ *   stopping when ||offdiag||_F <= rel_tol * ||G||_F (at most 30 sweeps). */
+int gemb_chol_inverse(gemb_ctx *ctx, int b, const double *G, double *Minv64_out, float *Minv32_out, int *rank_out);
+int gemb_eigh(gemb_ctx *ctx, int b, const double *G, double rel_tol, double *w_out, double *Z_out);
 
 /* ---- HOPE.  Replaces hope.py:29-36: S = (I - beta A)^-1 beta A is never formed; its top
  * k = d/2 singular triplets come from a block subspace iteration with Rayleigh-Ritz whose
