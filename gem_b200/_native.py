@@ -16,7 +16,7 @@ UNIQUE_ID_BYTES = 128
 
 EXPORTS = [
     'gemb_version', 'gemb_last_error', 'gemb_device_count', 'gemb_launch_count', 'gemb_ctx_create', 'gemb_ctx_destroy',
-    'gemb_host_alloc', 'gemb_host_free', 'gemb_mem_trim', 'gemb_mem_cached_bytes', 'gemb_comm_unique_id', 'gemb_comm_init', 'gemb_graph_upload',
+    'gemb_host_alloc', 'gemb_host_free', 'gemb_mem_trim', 'gemb_mem_cached_bytes', 'gemb_mem_live_blocks', 'gemb_comm_unique_id', 'gemb_comm_init', 'gemb_graph_upload',
     'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
@@ -79,6 +79,8 @@ def lib():
     L.gemb_mem_trim.argtypes = []
     L.gemb_mem_cached_bytes.argtypes = []
     L.gemb_mem_cached_bytes.restype = ctypes.c_size_t
+    L.gemb_mem_live_blocks.argtypes = []
+    L.gemb_mem_live_blocks.restype = ctypes.c_size_t
     L.gemb_comm_unique_id.argtypes = [vp]
     L.gemb_comm_init.argtypes = [vp, ctypes.c_int, ctypes.c_int, vp]
     L.gemb_graph_upload.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, ctypes.POINTER(vp)]
@@ -162,6 +164,11 @@ def mem_trim():
 
 def mem_cached_bytes():
     return int(lib().gemb_mem_cached_bytes())
+
+
+def mem_live_blocks():
+    """Device blocks handed out by the block cache and not yet released (gemb_mem_live_blocks)."""
+    return int(lib().gemb_mem_live_blocks())
 
 
 class Context:

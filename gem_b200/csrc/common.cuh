@@ -51,6 +51,47 @@ cudaError_t dmalloc_bytes(void **p, size_t bytes);
 cudaError_t dfree(void *p);
 template <class T> inline cudaError_t dmalloc(T **p, size_t bytes) { return dmalloc_bytes((void **)p, bytes); }
 
+// Owner of one dmalloc block of `count` T for the scope it is declared in: released by dfree on every return path.
+// Move-only: releasing a block twice would put it on the free list twice, and two later requests would share it.
+// release() hands the block to a longer-lived object, which then frees it itself.
+template <class T> class DeviceBuffer {
+  public:
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer &) = delete;
+    DeviceBuffer &operator=(const DeviceBuffer &) = delete;
+    DeviceBuffer(DeviceBuffer &&o) noexcept : p_(o.release()) {}
+    DeviceBuffer &operator=(DeviceBuffer &&o) noexcept {
+        if (this != &o) { reset(); p_ = o.release(); }
+        return *this;
+    }
+    ~DeviceBuffer() { reset(); }
+    cudaError_t alloc(size_t count) { reset(); return dmalloc(&p_, sizeof(T) * count); }   // count 0: a minimal block
+    T *get() const { return p_; }
+    T *release() { T *p = p_; p_ = nullptr; return p; }
+    void reset() { dfree(p_); p_ = nullptr; }
+
+  private:
+    T *p_ = nullptr;
+};
+
+// The N CUDA events of one call, destroyed on every return path.
+template <int N> class CallEvents {
+  public:
+    CallEvents() = default;
+    CallEvents(const CallEvents &) = delete;
+    CallEvents &operator=(const CallEvents &) = delete;
+    ~CallEvents() { for (cudaEvent_t e : ev_) if (e) cudaEventDestroy(e); }
+    cudaError_t create() {
+        for (cudaEvent_t &e : ev_) { const cudaError_t r = cudaEventCreate(&e); if (r != cudaSuccess) return r; }
+        return cudaSuccess;
+    }
+    cudaEvent_t operator[](int i) const { return ev_[i]; }
+    float ms(int from, int to) const { float t = 0.f; cudaEventElapsedTime(&t, ev_[from], ev_[to]); return t; }  // 0 on error
+
+  private:
+    cudaEvent_t ev_[N] = {};
+};
+
 struct Timer {  // pairs of events on ctx->stream, summed on demand
     std::vector<cudaEvent_t> ev;
     size_t used = 0;

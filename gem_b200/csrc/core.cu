@@ -178,6 +178,11 @@ size_t gemb_mem_cached_bytes(void) {
     return g_cache.cached_bytes;
 }
 
+size_t gemb_mem_live_blocks(void) {
+    std::lock_guard<std::mutex> lk(g_cache.mu);
+    return g_cache.live.size();
+}
+
 int gemb_version(void) { return GEMB_VERSION; }
 int64_t gemb_launch_count(void) { return (int64_t)gemb::launches_total(); }
 const char *gemb_last_error(void) { return g_err; }
@@ -313,14 +318,14 @@ static int upload_csr(gemb_ctx *c, int64_t n, int64_t n_local, const int32_t *in
                                   c->stream));
     }
     {
-        int *flags = nullptr, h = 0;
-        GEMB_CUDA(dmalloc(&flags, sizeof(int)));
-        GEMB_CUDA(cudaMemsetAsync(flags, 0, sizeof(int), c->stream));
-        csr_validate_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n_local, nnz, n, d->indptr, d->indices, flags);
+        DeviceBuffer<int> flags;
+        int h = 0;
+        GEMB_CUDA(flags.alloc(1));
+        GEMB_CUDA(cudaMemsetAsync(flags.get(), 0, sizeof(int), c->stream));
+        csr_validate_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n_local, nnz, n, d->indptr, d->indices, flags.get());
         count_launch();
-        GEMB_CUDA(cudaMemcpyAsync(&h, flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(&h, flags.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        dfree(flags);
         if (h) {
             set_error("malformed CSR:%s%s", (h & 1) ? " row offsets are not monotone;" : "",
                       (h & 2) ? " a column id lies outside [0, n)" : "");

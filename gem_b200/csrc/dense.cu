@@ -857,25 +857,23 @@ extern "C" int gemb_gram(gemb_ctx *c, int64_t n, const float *P, int b1, const f
     using namespace gemb;
     GEMB_ARG(c && P && G_out && n >= 0 && b1 > 0 && b2 > 0, "ctx/P/G/n/b");
     GEMB_CUDA(cudaSetDevice(c->device));
-    float *dP = nullptr, *dQ = nullptr;
-    double *dG = nullptr;
-    GEMB_CUDA(dmalloc(&dP, sizeof(float) * (size_t)std::max<int64_t>(n, 1) * b1));
-    GEMB_CUDA(cudaMemcpyAsync(dP, P, sizeof(float) * (size_t)n * b1, cudaMemcpyHostToDevice, c->stream));
+    DeviceBuffer<float> dP, dQ;
+    DeviceBuffer<double> dG;
+    GEMB_CUDA(dP.alloc((size_t)std::max<int64_t>(n, 1) * b1));
+    GEMB_CUDA(cudaMemcpyAsync(dP.get(), P, sizeof(float) * (size_t)n * b1, cudaMemcpyHostToDevice, c->stream));
     if (Q) {
-        GEMB_CUDA(dmalloc(&dQ, sizeof(float) * (size_t)std::max<int64_t>(n, 1) * b2));
-        GEMB_CUDA(cudaMemcpyAsync(dQ, Q, sizeof(float) * (size_t)n * b2, cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(dQ.alloc((size_t)std::max<int64_t>(n, 1) * b2));
+        GEMB_CUDA(cudaMemcpyAsync(dQ.get(), Q, sizeof(float) * (size_t)n * b2, cudaMemcpyHostToDevice, c->stream));
     }
-    GEMB_CUDA(dmalloc(&dG, sizeof(double) * (size_t)b1 * b2));
-    int s = use_tensor_cores ? gram_tc_launch(c, n, dP, b1, Q ? dQ : dP, b2, dG)
-                             : gram_fp32_launch(c, n, dP, b1, Q ? dQ : dP, b2, dG);
+    GEMB_CUDA(dG.alloc((size_t)b1 * b2));
+    const float *dQP = Q ? dQ.get() : dP.get();
+    const int s = use_tensor_cores ? gram_tc_launch(c, n, dP.get(), b1, dQP, b2, dG.get())
+                                   : gram_fp32_launch(c, n, dP.get(), b1, dQP, b2, dG.get());
     if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_gram: shape (n=%lld, b1=%d, b2=%d) not supported by the tensor-core kernel", (long long)n, b1, b2);
-    if (s == GEMB_OK) {
-        cudaError_t e = cudaMemcpyAsync(G_out, dG, sizeof(double) * (size_t)b1 * b2, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) { set_error("gemb_gram: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
-    }
-    dfree(dP); dfree(dQ); dfree(dG);
-    return s;
+    if (s != GEMB_OK) return s;
+    GEMB_CUDA(cudaMemcpyAsync(G_out, dG.get(), sizeof(double) * (size_t)b1 * b2, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }
 
 // The b x b hooks run the solvers' own launchers, so b picks the kernel variant exactly as in a solve.  b is limited to
@@ -886,24 +884,20 @@ extern "C" int gemb_chol_inverse(gemb_ctx *c, int b, const double *G, double *Mi
     GEMB_ARG(c && G && Minv64_out && Minv32_out && rank_out && b > 0 && b <= 1024, "ctx/G/Minv/rank/b");
     GEMB_CUDA(cudaSetDevice(c->device));
     const size_t bb = (size_t)b * b;
-    double *dG = nullptr, *dM64 = nullptr;
-    float *dM32 = nullptr;
-    int *dRank = nullptr;
-    cudaError_t e = dmalloc(&dG, sizeof(double) * bb);
-    if (e == cudaSuccess) e = dmalloc(&dM64, sizeof(double) * bb);
-    if (e == cudaSuccess) e = dmalloc(&dM32, sizeof(float) * bb);
-    if (e == cudaSuccess) e = dmalloc(&dRank, sizeof(int));
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dG, G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream);
-    int s = e == cudaSuccess ? chol_inverse_launch(c, b, dG, dM32, dRank, dM64) : GEMB_ERR_CUDA;
-    if (s == GEMB_OK) {
-        e = cudaMemcpyAsync(Minv64_out, dM64, sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(Minv32_out, dM32, sizeof(float) * bb, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(rank_out, dRank, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    }
-    if (e != cudaSuccess) { set_error("gemb_chol_inverse: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
-    dfree(dG); dfree(dM64); dfree(dM32); dfree(dRank);
-    return s;
+    DeviceBuffer<double> dG, dM64;
+    DeviceBuffer<float> dM32;
+    DeviceBuffer<int> dRank;
+    GEMB_CUDA(dG.alloc(bb));
+    GEMB_CUDA(dM64.alloc(bb));
+    GEMB_CUDA(dM32.alloc(bb));
+    GEMB_CUDA(dRank.alloc(1));
+    GEMB_CUDA(cudaMemcpyAsync(dG.get(), G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream));
+    GEMB_TRY(chol_inverse_launch(c, b, dG.get(), dM32.get(), dRank.get(), dM64.get()));
+    GEMB_CUDA(cudaMemcpyAsync(Minv64_out, dM64.get(), sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(Minv32_out, dM32.get(), sizeof(float) * bb, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(rank_out, dRank.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }
 
 extern "C" int gemb_eigh(gemb_ctx *c, int b, const double *G, double rel_tol, double *w_out, double *Z_out) {
@@ -911,21 +905,17 @@ extern "C" int gemb_eigh(gemb_ctx *c, int b, const double *G, double rel_tol, do
     GEMB_ARG(c && G && w_out && Z_out && b > 0 && b <= 1024 && rel_tol >= 0.0, "ctx/G/w/Z/b/rel_tol");
     GEMB_CUDA(cudaSetDevice(c->device));
     const size_t bb = (size_t)b * b;
-    double *dG = nullptr, *dw = nullptr, *dZ = nullptr, *dZs = nullptr;
-    cudaError_t e = dmalloc(&dG, sizeof(double) * bb);
-    if (e == cudaSuccess) e = dmalloc(&dw, sizeof(double) * b);
-    if (e == cudaSuccess) e = dmalloc(&dZ, sizeof(double) * bb);
-    if (e == cudaSuccess) e = dmalloc(&dZs, sizeof(double) * bb);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dG, G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream);
-    int s = e == cudaSuccess ? eigh_launch(c, b, dG, dw, dZ, dZs, rel_tol) : GEMB_ERR_CUDA;
-    if (s == GEMB_OK) {
-        e = cudaMemcpyAsync(w_out, dw, sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(Z_out, dZ, sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    }
-    if (e != cudaSuccess) { set_error("gemb_eigh: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
-    dfree(dG); dfree(dw); dfree(dZ); dfree(dZs);
-    return s;
+    DeviceBuffer<double> dG, dw, dZ, dZs;
+    GEMB_CUDA(dG.alloc(bb));
+    GEMB_CUDA(dw.alloc(b));
+    GEMB_CUDA(dZ.alloc(bb));
+    GEMB_CUDA(dZs.alloc(bb));
+    GEMB_CUDA(cudaMemcpyAsync(dG.get(), G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream));
+    GEMB_TRY(eigh_launch(c, b, dG.get(), dw.get(), dZ.get(), dZs.get(), rel_tol));
+    GEMB_CUDA(cudaMemcpyAsync(w_out, dw.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(Z_out, dZ.get(), sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }
 
 extern "C" int gemb_apply(gemb_ctx *c, int64_t n, const float *Q, int b1, const float *M, int b2,
@@ -933,20 +923,17 @@ extern "C" int gemb_apply(gemb_ctx *c, int64_t n, const float *Q, int b1, const 
     using namespace gemb;
     GEMB_ARG(c && Q && M && Out && n >= 0 && b1 > 0 && b2 > 0, "ctx/Q/M/Out/n/b");
     GEMB_CUDA(cudaSetDevice(c->device));
-    float *dQ = nullptr, *dM = nullptr, *dO = nullptr;
-    GEMB_CUDA(dmalloc(&dQ, sizeof(float) * (size_t)std::max<int64_t>(n, 1) * b1));
-    GEMB_CUDA(dmalloc(&dM, sizeof(float) * (size_t)b1 * b2));
-    GEMB_CUDA(dmalloc(&dO, sizeof(float) * (size_t)std::max<int64_t>(n, 1) * b2));
-    GEMB_CUDA(cudaMemcpyAsync(dQ, Q, sizeof(float) * (size_t)n * b1, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(dM, M, sizeof(float) * (size_t)b1 * b2, cudaMemcpyHostToDevice, c->stream));
-    int s = use_tensor_cores ? apply_tc_launch(c, n, dQ, b1, dM, b2, b2, dO, b2)
-                             : apply_fp32_launch(c, n, dQ, b1, dM, b2, b2, dO, b2);
+    DeviceBuffer<float> dQ, dM, dO;
+    GEMB_CUDA(dQ.alloc((size_t)std::max<int64_t>(n, 1) * b1));
+    GEMB_CUDA(dM.alloc((size_t)b1 * b2));
+    GEMB_CUDA(dO.alloc((size_t)std::max<int64_t>(n, 1) * b2));
+    GEMB_CUDA(cudaMemcpyAsync(dQ.get(), Q, sizeof(float) * (size_t)n * b1, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(dM.get(), M, sizeof(float) * (size_t)b1 * b2, cudaMemcpyHostToDevice, c->stream));
+    const int s = use_tensor_cores ? apply_tc_launch(c, n, dQ.get(), b1, dM.get(), b2, b2, dO.get(), b2)
+                                   : apply_fp32_launch(c, n, dQ.get(), b1, dM.get(), b2, b2, dO.get(), b2);
     if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_apply: shape (n=%lld, b1=%d, b2=%d) not supported by the tensor-core kernel", (long long)n, b1, b2);
-    if (s == GEMB_OK) {
-        cudaError_t e = cudaMemcpyAsync(Out, dO, sizeof(float) * (size_t)n * b2, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) { set_error("gemb_apply: %s", cudaGetErrorString(e)); s = GEMB_ERR_CUDA; }
-    }
-    dfree(dQ); dfree(dM); dfree(dO);
-    return s;
+    if (s != GEMB_OK) return s;
+    GEMB_CUDA(cudaMemcpyAsync(Out, dO.get(), sizeof(float) * (size_t)n * b2, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }

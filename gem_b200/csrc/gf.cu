@@ -89,70 +89,60 @@ extern "C" int gemb_gf(gemb_ctx *ctx, int64_t n, int64_t m, const int32_t *src, 
         GEMB_ARG(src[e] >= 0 && src[e] < n && dst[e] >= 0 && dst[e] < n, "edge endpoint outside [0, n)");
         if (mode == 1 && e > 0) GEMB_ARG(src[e] >= src[e - 1], "mode 1 needs the edges grouped by source row (non-decreasing src)");
     }
-    int32_t *d_src = nullptr, *d_dst = nullptr;
-    float *d_w = nullptr, *Xa = nullptr, *Xb = nullptr;
-    int64_t *d_rp = nullptr;
+    DeviceBuffer<int32_t> d_src, d_dst;
+    DeviceBuffer<float> d_w, Xa, Xb;
+    DeviceBuffer<int64_t> d_rp;
     const size_t xb = sizeof(float) * (size_t)n * d;
-    int status = GEMB_OK;
-    auto body = [&]() -> int {
-        GEMB_CUDA(dmalloc(&d_dst, sizeof(int32_t) * std::max<int64_t>(m, 1)));
-        GEMB_CUDA(cudaMemcpyAsync(d_dst, dst, sizeof(int32_t) * m, cudaMemcpyHostToDevice, st));
-        if (w) { GEMB_CUDA(dmalloc(&d_w, sizeof(float) * std::max<int64_t>(m, 1))); GEMB_CUDA(cudaMemcpyAsync(d_w, w, sizeof(float) * m, cudaMemcpyHostToDevice, st)); }
-        GEMB_CUDA(dmalloc(&Xa, xb));
-        GEMB_CUDA(cudaMemcpyAsync(Xa, X0, xb, cudaMemcpyHostToDevice, st));
-        if (mode == 0) {
-            GEMB_CUDA(dmalloc(&d_src, sizeof(int32_t) * std::max<int64_t>(m, 1)));
-            GEMB_CUDA(cudaMemcpyAsync(d_src, src, sizeof(int32_t) * m, cudaMemcpyHostToDevice, st));
-        } else {
-            rowptr.assign(n + 1, 0);
-            for (int64_t e = 0; e < m; e++) rowptr[src[e] + 1]++;
-            for (int64_t i = 0; i < n; i++) rowptr[i + 1] += rowptr[i];
-            GEMB_CUDA(dmalloc(&d_rp, sizeof(int64_t) * (n + 1)));
-            GEMB_CUDA(cudaMemcpyAsync(d_rp, rowptr.data(), sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice, st));
-            GEMB_CUDA(dmalloc(&Xb, xb));
-        }
-        cudaEvent_t e0, e1;
-        GEMB_CUDA(cudaEventCreate(&e0)); GEMB_CUDA(cudaEventCreate(&e1));
-        GEMB_CUDA(cudaEventRecord(e0, st));
-        const int nv = (d + 31) / 32;
-        float *cur = Xa;
+    GEMB_CUDA(d_dst.alloc(std::max<int64_t>(m, 1)));
+    GEMB_CUDA(cudaMemcpyAsync(d_dst.get(), dst, sizeof(int32_t) * m, cudaMemcpyHostToDevice, st));
+    if (w) { GEMB_CUDA(d_w.alloc(std::max<int64_t>(m, 1))); GEMB_CUDA(cudaMemcpyAsync(d_w.get(), w, sizeof(float) * m, cudaMemcpyHostToDevice, st)); }
+    GEMB_CUDA(Xa.alloc((size_t)n * d));
+    GEMB_CUDA(cudaMemcpyAsync(Xa.get(), X0, xb, cudaMemcpyHostToDevice, st));
+    if (mode == 0) {
+        GEMB_CUDA(d_src.alloc(std::max<int64_t>(m, 1)));
+        GEMB_CUDA(cudaMemcpyAsync(d_src.get(), src, sizeof(int32_t) * m, cudaMemcpyHostToDevice, st));
+    } else {
+        rowptr.assign(n + 1, 0);
+        for (int64_t e = 0; e < m; e++) rowptr[src[e] + 1]++;
+        for (int64_t i = 0; i < n; i++) rowptr[i + 1] += rowptr[i];
+        GEMB_CUDA(d_rp.alloc(n + 1));
+        GEMB_CUDA(cudaMemcpyAsync(d_rp.get(), rowptr.data(), sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice, st));
+        GEMB_CUDA(Xb.alloc((size_t)n * d));
+    }
+    CallEvents<2> ev;
+    GEMB_CUDA(ev.create());
+    GEMB_CUDA(cudaEventRecord(ev[0], st));
+    const int nv = (d + 31) / 32;
+    float *cur = Xa.get();
 #define GF_DISPATCH(CALL)                                                                     \
-        do {                                                                                  \
-            if (nv <= 1) { CALL(1); } else if (nv <= 2) { CALL(2); } else if (nv <= 4) { CALL(4); } \
-            else if (nv <= 8) { CALL(8); } else if (nv <= 16) { CALL(16); } else { CALL(32); } \
-        } while (0)
-        if (mode == 0) {
-            if (m > 0 && max_iter > 0) {
-#define SEQ(NV) gf_sequential_kernel<NV><<<1, 32, 0, st>>>(m, d_src, d_dst, d_w, d, eta, regu, max_iter, Xa)
-                GF_DISPATCH(SEQ);
+    do {                                                                                      \
+        if (nv <= 1) { CALL(1); } else if (nv <= 2) { CALL(2); } else if (nv <= 4) { CALL(4); } \
+        else if (nv <= 8) { CALL(8); } else if (nv <= 16) { CALL(16); } else { CALL(32); } \
+    } while (0)
+    if (mode == 0) {
+        if (m > 0 && max_iter > 0) {
+#define SEQ(NV) gf_sequential_kernel<NV><<<1, 32, 0, st>>>(m, d_src.get(), d_dst.get(), d_w.get(), d, eta, regu, max_iter, Xa.get())
+            GF_DISPATCH(SEQ);
 #undef SEQ
-                GEMB_CUDA(cudaGetLastError());
-                count_launch();
-            }
-        } else {
-            const int grid = (int)std::min<int64_t>((n * 32 + 255) / 256, (int64_t)ctx->sm_count * 16);
-            float *nxt = Xb;
-            for (int ep = 0; ep < max_iter; ep++) {
-#define ROWS(NV) gf_rows_kernel<NV><<<grid, 256, 0, st>>>(n, d_rp, d_dst, d_w, d, eta, regu, cur, nxt)
-                GF_DISPATCH(ROWS);
-#undef ROWS
-                std::swap(cur, nxt);
-            }
             GEMB_CUDA(cudaGetLastError());
-            count_launch(max_iter);
+            count_launch();
         }
+    } else {
+        const int grid = (int)std::min<int64_t>((n * 32 + 255) / 256, (int64_t)ctx->sm_count * 16);
+        float *nxt = Xb.get();
+        for (int ep = 0; ep < max_iter; ep++) {
+#define ROWS(NV) gf_rows_kernel<NV><<<grid, 256, 0, st>>>(n, d_rp.get(), d_dst.get(), d_w.get(), d, eta, regu, cur, nxt)
+            GF_DISPATCH(ROWS);
+#undef ROWS
+            std::swap(cur, nxt);
+        }
+        GEMB_CUDA(cudaGetLastError());
+        count_launch(max_iter);
+    }
 #undef GF_DISPATCH
-        GEMB_CUDA(cudaEventRecord(e1, st));
-        GEMB_CUDA(cudaMemcpyAsync(X_out, cur, xb, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        if (device_ms_out) *device_ms_out = ms;
-        cudaEventDestroy(e0); cudaEventDestroy(e1);
-        return GEMB_OK;
-    };
-    status = body();
-    cudaStreamSynchronize(st);
-    dfree(d_src); dfree(d_dst); dfree(d_w); dfree(Xa); dfree(Xb); dfree(d_rp);
-    return status;
+    GEMB_CUDA(cudaEventRecord(ev[1], st));
+    GEMB_CUDA(cudaMemcpyAsync(X_out, cur, xb, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaStreamSynchronize(st));
+    if (device_ms_out) *device_ms_out = ev.ms(0, 1);
+    return GEMB_OK;
 }

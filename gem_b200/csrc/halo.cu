@@ -76,15 +76,15 @@ static int ipc_exchange(gemb_ctx *c, void *const *mine, int count, void **peers 
     const int P = c->nranks;
     std::vector<cudaIpcMemHandle_t> h(count), all((size_t)count * P);
     for (int i = 0; i < count; i++) GEMB_CUDA(cudaIpcGetMemHandle(&h[i], mine[i]));
-    char *dsend = nullptr, *drecv = nullptr;
+    DeviceBuffer<char> dsend, drecv;
     const size_t bytes = sizeof(cudaIpcMemHandle_t) * count;
-    GEMB_CUDA(dmalloc(&dsend, bytes));
-    GEMB_CUDA(dmalloc(&drecv, bytes * P));
-    GEMB_CUDA(cudaMemcpyAsync(dsend, h.data(), bytes, cudaMemcpyHostToDevice, c->stream));
-    NCCL_TRY(api->AllGather(dsend, drecv, bytes, ncclChar, (ncclComm_t)c->comm, c->stream), "ncclAllGather(ipc handles)");
-    GEMB_CUDA(cudaMemcpyAsync(all.data(), drecv, bytes * P, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(dsend.alloc(bytes));
+    GEMB_CUDA(drecv.alloc(bytes * P));
+    GEMB_CUDA(cudaMemcpyAsync(dsend.get(), h.data(), bytes, cudaMemcpyHostToDevice, c->stream));
+    NCCL_TRY(api->AllGather(dsend.get(), drecv.get(), bytes, ncclChar, (ncclComm_t)c->comm, c->stream), "ncclAllGather(ipc handles)");
+    GEMB_CUDA(cudaMemcpyAsync(all.data(), drecv.get(), bytes * P, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    dfree(dsend); dfree(drecv);
+    dsend.reset(); drecv.reset();
     for (int i = 0; i < count; i++)
         for (int q = 0; q < P; q++) {
             void **slot = peers + (size_t)i * GEMB_MAX_RANKS + q;
@@ -102,12 +102,121 @@ static int ipc_exchange(gemb_ctx *c, void *const *mine, int count, void **peers 
 static int nccl_barrier(gemb_ctx *c) {
     NcclApi *api = nccl_api();
     if (!api) return GEMB_ERR_NCCL;
-    int *d = nullptr;
-    GEMB_CUDA(dmalloc(&d, sizeof(int)));
-    GEMB_CUDA(cudaMemsetAsync(d, 0, sizeof(int), c->stream));
-    NCCL_TRY(api->AllReduce(d, d, 1, ncclInt, ncclSum, (ncclComm_t)c->comm, c->stream), "ncclAllReduce(barrier)");
+    DeviceBuffer<int> d;
+    GEMB_CUDA(d.alloc(1));
+    GEMB_CUDA(cudaMemsetAsync(d.get(), 0, sizeof(int), c->stream));
+    NCCL_TRY(api->AllReduce(d.get(), d.get(), 1, ncclInt, ncclSum, (ncclComm_t)c->comm, c->stream), "ncclAllReduce(barrier)");
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    dfree(d);
+    return GEMB_OK;
+}
+
+// the exchange plan of halo_build (indices_ext, push_ptr, push_dst, halo_rows, push_total); its scratch is released
+// when it returns
+static int halo_plan(gemb_graph *g, NcclApi *api) {
+    gemb_halo &H = g->halo;
+    gemb_ctx *c = g->ctx;
+    const int P = c->nranks;
+    const int64_t nnz = g->A.nnz;
+    const int32_t lo = (int32_t)g->row0, hi = (int32_t)std::min<int64_t>(g->row0 + g->n_shard, g->n);
+    cudaStream_t st = c->stream;
+
+    // ---- distinct remote columns, sorted
+    DeviceBuffer<int32_t> rem, rem_sorted, Hd;
+    DeviceBuffer<long long> d_num;
+    GEMB_CUDA(rem.alloc(std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(rem_sorted.alloc(std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(Hd.alloc(std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(d_num.alloc(2 * GEMB_MAX_RANKS + 2));
+    size_t tb = 0, need = 0;
+    DeviceBuffer<char> tmp;
+    IsRemote pred{lo, hi};
+    cub::DeviceSelect::If(nullptr, need, g->A.indices, rem.get(), d_num.get(), nnz, pred, st); tb = need;
+    cub::DeviceRadixSort::SortKeys(nullptr, need, rem.get(), rem_sorted.get(), nnz, 0, 32, st); tb = std::max(tb, need);
+    cub::DeviceSelect::Unique(nullptr, need, rem_sorted.get(), Hd.get(), d_num.get(), nnz, st); tb = std::max(tb, need);
+    GEMB_CUDA(tmp.alloc(tb));
+    long long n_rem = 0, n_H = 0;
+    if (nnz > 0) {
+        GEMB_CUDA(cub::DeviceSelect::If(tmp.get(), tb, g->A.indices, rem.get(), d_num.get(), nnz, pred, st));
+        GEMB_CUDA(cudaMemcpyAsync(&n_rem, d_num.get(), sizeof n_rem, cudaMemcpyDeviceToHost, st));
+        GEMB_CUDA(cudaStreamSynchronize(st));
+        if (n_rem > 0) {
+            GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.get(), tb, rem.get(), rem_sorted.get(), n_rem, 0, 32, st));
+            GEMB_CUDA(cub::DeviceSelect::Unique(tmp.get(), tb, rem_sorted.get(), Hd.get(), d_num.get(), n_rem, st));
+            GEMB_CUDA(cudaMemcpyAsync(&n_H, d_num.get(), sizeof n_H, cudaMemcpyDeviceToHost, st));
+            GEMB_CUDA(cudaStreamSynchronize(st));
+        }
+    }
+    count_launch(3);
+    H.halo_rows = n_H;
+    GEMB_ARG(n_H < ((int64_t)1 << 29), "halo too large for 29-bit slots");
+
+    // ---- remapped column ids
+    GEMB_CUDA(dmalloc(&H.indices_ext, sizeof(int32_t) * (std::max<int64_t>(nnz, 1) + 4)));   // + the x4 padding the bulk copies of spmm.cu read
+    if (nnz > 0) {
+        halo_remap_kernel<<<c->sm_count * 8, 256, 0, st>>>(nnz, g->A.indices, lo, hi, Hd.get(), n_H, (int32_t)g->n_shard, H.indices_ext);
+        GEMB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+
+    // ---- everyone's halo lists -> who needs my rows
+    long long *d_cnt_all = d_num.get() + 2;                 // [P]
+    long long h_cnt_all[GEMB_MAX_RANKS];
+    GEMB_CUDA(cudaMemcpyAsync(d_num.get(), &n_H, sizeof n_H, cudaMemcpyHostToDevice, st));
+    NCCL_TRY(api->AllGather(d_num.get(), d_cnt_all, 1, ncclInt64, (ncclComm_t)c->comm, st), "ncclAllGather(halo counts)");
+    GEMB_CUDA(cudaMemcpyAsync(h_cnt_all, d_cnt_all, sizeof(long long) * P, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaStreamSynchronize(st));
+    long long maxH = 1;
+    for (int q = 0; q < P; q++) maxH = std::max(maxH, h_cnt_all[q]);
+    DeviceBuffer<int32_t> Hpad, Hall;
+    GEMB_CUDA(Hpad.alloc(maxH));
+    GEMB_CUDA(Hall.alloc(maxH * P));
+    GEMB_CUDA(cudaMemsetAsync(Hpad.get(), 0x7f, sizeof(int32_t) * maxH, st));
+    if (n_H) GEMB_CUDA(cudaMemcpyAsync(Hpad.get(), Hd.get(), sizeof(int32_t) * n_H, cudaMemcpyDeviceToDevice, st));
+    NCCL_TRY(api->AllGather(Hpad.get(), Hall.get(), (size_t)maxH, ncclInt32, (ncclComm_t)c->comm, st), "ncclAllGather(halo lists)");
+    DeviceBuffer<long long> seg_dev;
+    GEMB_CUDA(seg_dev.alloc(2 * GEMB_MAX_RANKS));
+    halo_segments_kernel<<<1, 32, 0, st>>>(P, Hall.get(), maxH, d_cnt_all, lo, hi, seg_dev.get());
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    long long seg[2 * GEMB_MAX_RANKS];
+    GEMB_CUDA(cudaMemcpyAsync(seg, seg_dev.get(), sizeof(long long) * 2 * P, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaStreamSynchronize(st));
+
+    DeviceBuffer<int32_t> cnt;
+    const int64_t nl = g->n_local;
+    GEMB_CUDA(cnt.alloc(nl + 1));
+    GEMB_CUDA(dmalloc(&H.push_ptr, sizeof(int32_t) * (nl + 1)));
+    GEMB_CUDA(cudaMemsetAsync(cnt.get(), 0, sizeof(int32_t) * (nl + 1), st));
+    long long total = 0;
+    for (int q = 0; q < P; q++) {
+        if (q == c->rank) continue;
+        const long long m = seg[2 * q + 1] - seg[2 * q];
+        total += m;
+        if (m <= 0) continue;
+        const int grid = (int)std::min<long long>((m + 255) / 256, c->sm_count * 8);
+        halo_pushlist_kernel<0><<<grid, 256, 0, st>>>(q, Hall.get() + (int64_t)q * maxH, seg[2 * q], seg[2 * q + 1], lo, cnt.get(), nullptr, nullptr);
+        GEMB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    GEMB_ARG(total < ((long long)1 << 31), "push list too long");
+    H.push_total = total;
+    size_t sb = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, sb, cnt.get(), H.push_ptr, (int)(nl + 1), st);
+    DeviceBuffer<char> stmp;
+    GEMB_CUDA(stmp.alloc(sb));
+    GEMB_CUDA(cub::DeviceScan::ExclusiveSum(stmp.get(), sb, cnt.get(), H.push_ptr, (int)(nl + 1), st));
+    GEMB_CUDA(cudaMemsetAsync(cnt.get(), 0, sizeof(int32_t) * (nl + 1), st));
+    GEMB_CUDA(dmalloc(&H.push_dst, sizeof(uint32_t) * std::max<long long>(total, 1)));
+    for (int q = 0; q < P; q++) {
+        if (q == c->rank) continue;
+        const long long m = seg[2 * q + 1] - seg[2 * q];
+        if (m <= 0) continue;
+        const int grid = (int)std::min<long long>((m + 255) / 256, c->sm_count * 8);
+        halo_pushlist_kernel<1><<<grid, 256, 0, st>>>(q, Hall.get() + (int64_t)q * maxH, seg[2 * q], seg[2 * q + 1], lo, cnt.get(), H.push_ptr, H.push_dst);
+        GEMB_CUDA(cudaGetLastError());
+        count_launch();
+    }
+    GEMB_CUDA(cudaStreamSynchronize(st));
     return GEMB_OK;
 }
 
@@ -121,111 +230,7 @@ int halo_build(gemb_graph *g) {
     GEMB_ARG(g->symmetric && !g->replicated, "halo exchange needs a symmetric row shard");
     GEMB_ARG(g->n_shard + 1 < (int64_t)1 << 29, "shard too large for 29-bit halo slots");
     const int P = c->nranks;
-    const int64_t nnz = g->A.nnz;
-    const int32_t lo = (int32_t)g->row0, hi = (int32_t)std::min<int64_t>(g->row0 + g->n_shard, g->n);
-    cudaStream_t st = c->stream;
-
-    // ---- distinct remote columns, sorted
-    int32_t *rem = nullptr, *rem_sorted = nullptr, *Hd = nullptr;
-    long long *d_num = nullptr;
-    GEMB_CUDA(dmalloc(&rem, sizeof(int32_t) * std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(dmalloc(&rem_sorted, sizeof(int32_t) * std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(dmalloc(&Hd, sizeof(int32_t) * std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(dmalloc(&d_num, sizeof(long long) * (2 * GEMB_MAX_RANKS + 2)));
-    size_t tb = 0, need = 0;
-    void *tmp = nullptr;
-    IsRemote pred{lo, hi};
-    cub::DeviceSelect::If(nullptr, need, g->A.indices, rem, d_num, nnz, pred, st); tb = need;
-    cub::DeviceRadixSort::SortKeys(nullptr, need, rem, rem_sorted, nnz, 0, 32, st); tb = std::max(tb, need);
-    cub::DeviceSelect::Unique(nullptr, need, rem_sorted, Hd, d_num, nnz, st); tb = std::max(tb, need);
-    GEMB_CUDA(dmalloc(&tmp, tb ? tb : 4));
-    long long n_rem = 0, n_H = 0;
-    if (nnz > 0) {
-        GEMB_CUDA(cub::DeviceSelect::If(tmp, tb, g->A.indices, rem, d_num, nnz, pred, st));
-        GEMB_CUDA(cudaMemcpyAsync(&n_rem, d_num, sizeof n_rem, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
-        if (n_rem > 0) {
-            GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, rem, rem_sorted, n_rem, 0, 32, st));
-            GEMB_CUDA(cub::DeviceSelect::Unique(tmp, tb, rem_sorted, Hd, d_num, n_rem, st));
-            GEMB_CUDA(cudaMemcpyAsync(&n_H, d_num, sizeof n_H, cudaMemcpyDeviceToHost, st));
-            GEMB_CUDA(cudaStreamSynchronize(st));
-        }
-    }
-    count_launch(3);
-    H.halo_rows = n_H;
-    GEMB_ARG(n_H < ((int64_t)1 << 29), "halo too large for 29-bit slots");
-
-    // ---- remapped column ids
-    GEMB_CUDA(dmalloc(&H.indices_ext, sizeof(int32_t) * (std::max<int64_t>(nnz, 1) + 4)));   // + the x4 padding the bulk copies of spmm.cu read
-    if (nnz > 0) {
-        halo_remap_kernel<<<c->sm_count * 8, 256, 0, st>>>(nnz, g->A.indices, lo, hi, Hd, n_H, (int32_t)g->n_shard, H.indices_ext);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
-
-    // ---- everyone's halo lists -> who needs my rows
-    long long *d_cnt_all = d_num + 2;                       // [P]
-    long long h_cnt_all[GEMB_MAX_RANKS];
-    GEMB_CUDA(cudaMemcpyAsync(d_num, &n_H, sizeof n_H, cudaMemcpyHostToDevice, st));
-    NCCL_TRY(api->AllGather(d_num, d_cnt_all, 1, ncclInt64, (ncclComm_t)c->comm, st), "ncclAllGather(halo counts)");
-    GEMB_CUDA(cudaMemcpyAsync(h_cnt_all, d_cnt_all, sizeof(long long) * P, cudaMemcpyDeviceToHost, st));
-    GEMB_CUDA(cudaStreamSynchronize(st));
-    long long maxH = 1;
-    for (int q = 0; q < P; q++) maxH = std::max(maxH, h_cnt_all[q]);
-    int32_t *Hpad = nullptr, *Hall = nullptr;
-    GEMB_CUDA(dmalloc(&Hpad, sizeof(int32_t) * maxH));
-    GEMB_CUDA(dmalloc(&Hall, sizeof(int32_t) * maxH * P));
-    GEMB_CUDA(cudaMemsetAsync(Hpad, 0x7f, sizeof(int32_t) * maxH, st));
-    if (n_H) GEMB_CUDA(cudaMemcpyAsync(Hpad, Hd, sizeof(int32_t) * n_H, cudaMemcpyDeviceToDevice, st));
-    NCCL_TRY(api->AllGather(Hpad, Hall, (size_t)maxH, ncclInt32, (ncclComm_t)c->comm, st), "ncclAllGather(halo lists)");
-    long long *d_seg = d_cnt_all + GEMB_MAX_RANKS;          // needs 2P entries: allocate separately
-    long long *seg_dev = nullptr;
-    GEMB_CUDA(dmalloc(&seg_dev, sizeof(long long) * 2 * GEMB_MAX_RANKS));
-    (void)d_seg;
-    halo_segments_kernel<<<1, 32, 0, st>>>(P, Hall, maxH, d_cnt_all, lo, hi, seg_dev);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    long long seg[2 * GEMB_MAX_RANKS];
-    GEMB_CUDA(cudaMemcpyAsync(seg, seg_dev, sizeof(long long) * 2 * P, cudaMemcpyDeviceToHost, st));
-    GEMB_CUDA(cudaStreamSynchronize(st));
-
-    int32_t *cnt = nullptr;
-    const int64_t nl = g->n_local;
-    GEMB_CUDA(dmalloc(&cnt, sizeof(int32_t) * (nl + 1)));
-    GEMB_CUDA(dmalloc(&H.push_ptr, sizeof(int32_t) * (nl + 1)));
-    GEMB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (nl + 1), st));
-    long long total = 0;
-    for (int q = 0; q < P; q++) {
-        if (q == c->rank) continue;
-        const long long m = seg[2 * q + 1] - seg[2 * q];
-        total += m;
-        if (m <= 0) continue;
-        const int grid = (int)std::min<long long>((m + 255) / 256, c->sm_count * 8);
-        halo_pushlist_kernel<0><<<grid, 256, 0, st>>>(q, Hall + (int64_t)q * maxH, seg[2 * q], seg[2 * q + 1], lo, cnt, nullptr, nullptr);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
-    GEMB_ARG(total < ((long long)1 << 31), "push list too long");
-    H.push_total = total;
-    size_t sb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, sb, cnt, H.push_ptr, (int)(nl + 1), st);
-    void *stmp = nullptr;
-    GEMB_CUDA(dmalloc(&stmp, sb ? sb : 4));
-    GEMB_CUDA(cub::DeviceScan::ExclusiveSum(stmp, sb, cnt, H.push_ptr, (int)(nl + 1), st));
-    GEMB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (nl + 1), st));
-    GEMB_CUDA(dmalloc(&H.push_dst, sizeof(uint32_t) * std::max<long long>(total, 1)));
-    for (int q = 0; q < P; q++) {
-        if (q == c->rank) continue;
-        const long long m = seg[2 * q + 1] - seg[2 * q];
-        if (m <= 0) continue;
-        const int grid = (int)std::min<long long>((m + 255) / 256, c->sm_count * 8);
-        halo_pushlist_kernel<1><<<grid, 256, 0, st>>>(q, Hall + (int64_t)q * maxH, seg[2 * q], seg[2 * q + 1], lo, cnt, H.push_ptr, H.push_dst);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
-    GEMB_CUDA(cudaStreamSynchronize(st));
-    dfree(rem); dfree(rem_sorted); dfree(Hd); dfree(d_num); dfree(tmp); dfree(Hpad); dfree(Hall); dfree(seg_dev);
-    dfree(cnt); dfree(stmp);
+    GEMB_TRY(halo_plan(g, api));
 
     // ---- barrier flags: owned by the context (plain cudaMalloc: exported through CUDA IPC, never recycled by the block
     //      cache), set up once and shared by every graph of this context
@@ -272,13 +277,14 @@ int halo_buffers(gemb_graph *g, int nbuf, int width) {
     const size_t rows = (size_t)(g->n_shard + H.halo_rows);
     // the pool is (re)built only when some rank needs more than it holds: the decision comes from an all-reduce (max)
     // of the need, so every rank takes the same branch
-    long long need = (long long)(rows * (size_t)width), *d_need = nullptr;
-    GEMB_CUDA(dmalloc(&d_need, sizeof(long long)));
-    GEMB_CUDA(cudaMemcpyAsync(d_need, &need, sizeof need, cudaMemcpyHostToDevice, c->stream));
-    NCCL_TRY(api->AllReduce(d_need, d_need, 1, ncclInt64, ncclMax, (ncclComm_t)c->comm, c->stream), "ncclAllReduce(halo block size)");
-    GEMB_CUDA(cudaMemcpyAsync(&need, d_need, sizeof need, cudaMemcpyDeviceToHost, c->stream));
+    long long need = (long long)(rows * (size_t)width);
+    DeviceBuffer<long long> d_need;
+    GEMB_CUDA(d_need.alloc(1));
+    GEMB_CUDA(cudaMemcpyAsync(d_need.get(), &need, sizeof need, cudaMemcpyHostToDevice, c->stream));
+    NCCL_TRY(api->AllReduce(d_need.get(), d_need.get(), 1, ncclInt64, ncclMax, (ncclComm_t)c->comm, c->stream), "ncclAllReduce(halo block size)");
+    GEMB_CUDA(cudaMemcpyAsync(&need, d_need.get(), sizeof need, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    dfree(d_need);
+    d_need.reset();
     if (PL.nbuf < nbuf || PL.cap_floats < (size_t)need) {
         GEMB_TRY(halo_pool_drop_blocks(c));
         const size_t cap = (size_t)std::max<long long>(need, 1);

@@ -46,20 +46,25 @@ struct HopeWork {
     int b;
     int64_t rows;    // n_local
     int64_t shard;   // n_shard (buffer rows)
-    float *buf[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // n_shard x b each
-    float *full = nullptr;   // n_pad x b (multi-GPU all-gather target)
-    double *G = nullptr, *G2 = nullptr, *w = nullptr, *Z = nullptr, *Zs = nullptr, *scal = nullptr;
-    float *Minv = nullptr, *M1 = nullptr, *M2 = nullptr;
-    int *rank_dev = nullptr;
+    float *buf[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // n_shard x b each: own_buf[], or g->halo.buf[] in halo mode
+    DeviceBuffer<float> own_buf[5];
+    DeviceBuffer<float> full;   // n_pad x b (multi-GPU all-gather target)
+    DeviceBuffer<double> G, G2, w, Z, Zs, scal;
+    DeviceBuffer<float> Minv, M1, M2;
+    DeviceBuffer<int> rank_dev;
     int64_t spmm_wide = 0, spmm_all = 0;
     bool halo = false;       // multi-GPU: needed-rows-only exchange over peer memory (halo.cu); buf[] = g->halo.buf[]
     int64_t pushes = 0;      // blocks whose rows were pushed to the peers
     double push_bytes_per_row = 0.0;   // sum over the pushed blocks of (bytes per pushed row): NVLink bytes out = this * push_rows
     int buf_index(const float *p) const { for (int i = 0; i < 5; i++) if (buf[i] == p) return i; return -1; }
-    ~HopeWork() {
-        if (!halo) for (auto p : buf) dfree(p);
-        dfree(full); dfree(G); dfree(G2); dfree(w); dfree(Z); dfree(Zs); dfree(scal);
-        dfree(Minv); dfree(M1); dfree(M2); dfree(rank_dev);
+    // the five work blocks of `count` floats each, zero-filled (padded rows stay 0)
+    int alloc_blocks(size_t count) {
+        for (int i = 0; i < 5; i++) {
+            GEMB_CUDA(own_buf[i].alloc(count));
+            buf[i] = own_buf[i].get();
+            GEMB_CUDA(cudaMemsetAsync(buf[i], 0, sizeof(float) * count, c->stream));
+        }
+        return GEMB_OK;
     }
 };
 
@@ -68,7 +73,7 @@ struct HopeResult {
     double change = 0.0;
     float resid_max = -1.f, resid_est = -1.f;
     float *Xd = nullptr;       // device n_local x d (points into a work buffer or Xalloc)
-    float *Xalloc = nullptr;   // owned
+    DeviceBuffer<float> Xalloc;
     float *sig_dev = nullptr;  // k floats
     double sigma_max = 0.0;
 };
@@ -77,7 +82,7 @@ static int comm_allgather(HopeWork &W, const float *shard_src, int width) {
     NcclApi *api = nccl_api();
     if (!api) return GEMB_ERR_NCCL;
     GEMB_TRY(W.c->t_comm.begin(W.c->stream));
-    ncclResult_t r = api->AllGather(shard_src, W.full, (size_t)W.shard * width, ncclFloat,
+    ncclResult_t r = api->AllGather(shard_src, W.full.get(), (size_t)W.shard * width, ncclFloat,
                                     (ncclComm_t)W.c->comm, W.c->stream);
     if (r != ncclSuccess) { set_error("ncclAllGather: %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
     GEMB_TRY(W.c->t_comm.end(W.c->stream));
@@ -138,7 +143,7 @@ static int dist_spmm3(HopeWork &W, bool transpose, int width, float alpha, const
     const float *Xfull = Xshard;
     if (W.c->nranks > 1) {
         GEMB_TRY(comm_allgather(W, Xshard, width));
-        Xfull = W.full;
+        Xfull = W.full.get();
     }
     if (timed) GEMB_TRY(W.c->t_spmm.begin(W.c->stream));
     GEMB_TRY(spmm3_launch(W.c, transpose ? W.g->AT : W.g->A, W.rows, width, alpha, Xfull, gamma,
@@ -180,18 +185,18 @@ static int gram_full(HopeWork &W, const float *P, const float *Q, double *G) {
 // one CholeskyQR pass: dst = src * R^-1 with R^T R = G (G destroyed). G must hold src^T src.
 static int cholqr_pass(HopeWork &W, double *G, const float *src, float *dst) {
     GEMB_TRY(W.c->t_dense.begin(W.c->stream));
-    GEMB_TRY(chol_inverse_launch(W.c, W.b, G, W.Minv, W.rank_dev));
-    GEMB_TRY(apply_launch(W.c, W.rows, src, W.b, W.Minv, W.b, W.b, dst, W.b));
+    GEMB_TRY(chol_inverse_launch(W.c, W.b, G, W.Minv.get(), W.rank_dev.get()));
+    GEMB_TRY(apply_launch(W.c, W.rows, src, W.b, W.Minv.get(), W.b, W.b, dst, W.b));
     GEMB_TRY(W.c->t_dense.end(W.c->stream));
     return GEMB_OK;
 }
 
 // dst = orth(src) by CholeskyQR2; tmp is scratch; src, tmp, dst pairwise distinct
 static int cholqr2(HopeWork &W, const float *src, float *tmp, float *dst) {
-    GEMB_TRY(gram_full(W, src, src, W.G));
-    GEMB_TRY(cholqr_pass(W, W.G, src, tmp));
-    GEMB_TRY(gram_full(W, tmp, tmp, W.G));
-    GEMB_TRY(cholqr_pass(W, W.G, tmp, dst));
+    GEMB_TRY(gram_full(W, src, src, W.G.get()));
+    GEMB_TRY(cholqr_pass(W, W.G.get(), src, tmp));
+    GEMB_TRY(gram_full(W, tmp, tmp, W.G.get()));
+    GEMB_TRY(cholqr_pass(W, W.G.get(), tmp, dst));
     return GEMB_OK;
 }
 
@@ -322,15 +327,15 @@ static int comm_allreduce_max_f64(HopeWork &W, double *buf, size_t count) {
 // ||A||_inf and the sign of the weights in one pass over the CSR shard
 static int rowsum_bound(HopeWork &W, double *norm_inf, bool *nonneg) {
     gemb_ctx *c = W.c;
-    GEMB_CUDA(cudaMemsetAsync(W.scal, 0, 2 * sizeof(double), c->stream));
+    GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, 2 * sizeof(double), c->stream));
     if (W.rows > 0) {
-        csr_rowsum_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(W.rows, W.g->A.indptr, W.g->A.data, W.scal);
+        csr_rowsum_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(W.rows, W.g->A.indptr, W.g->A.data, W.scal.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
     }
-    GEMB_TRY(comm_allreduce_max_f64(W, W.scal, 2));
+    GEMB_TRY(comm_allreduce_max_f64(W, W.scal.get(), 2));
     double h[2];
-    GEMB_CUDA(cudaMemcpyAsync(h, W.scal, sizeof h, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     *norm_inf = h[0];
     *nonneg = (h[1] == 0.0);
@@ -346,13 +351,13 @@ static int estimate_norm2(HopeWork &W, uint64_t seed, float *x, float *y, float 
     double est = 0.0, prev = -1.0;
     for (int it = 0; it < 16; it++) {
         double h[2];
-        GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal));
+        GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal.get()));
         GEMB_TRY(publish(W, x, pw));
         GEMB_TRY(dist_spmm3(W, false, pw, 1.f, x, 0.f, false, 1.f, nullptr, y, false, true));
         GEMB_TRY(dist_spmm(W, true, pw, 1.f, y, nullptr, z, false));
-        GEMB_TRY(sumsq_launch(c, W.rows * pw, z, W.scal + 1));
-        GEMB_TRY(comm_allreduce_f64(W, W.scal, 2));
-        GEMB_CUDA(cudaMemcpyAsync(h, W.scal, sizeof h, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_TRY(sumsq_launch(c, W.rows * pw, z, W.scal.get() + 1));
+        GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 2));
+        GEMB_CUDA(cudaMemcpyAsync(h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }  // A^T A x = 0 (empty graph)
         est = sqrt(sqrt(h[1] / h[0]));   // ||A^T A x|| / ||x|| -> sigma_max^2
@@ -383,9 +388,9 @@ static int probe_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t s
         for (j = 1; j <= Jmax; j++) {
             double h = 0.0;
             GEMB_TRY(dist_spmm(W, tr == 1, pw, beta, x, nullptr, y, false));
-            GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal));
-            GEMB_TRY(comm_allreduce_f64(W, W.scal, 1));
-            GEMB_CUDA(cudaMemcpyAsync(&h, W.scal, sizeof h, cudaMemcpyDeviceToHost, c->stream));
+            GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get()));
+            GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 1));
+            GEMB_CUDA(cudaMemcpyAsync(&h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost, c->stream));
             GEMB_CUDA(cudaStreamSynchronize(c->stream));
             const double nt = sqrt(h);
             if (prev > 0.0) *rho_est = std::max(*rho_est * (j > 8 ? 0.0 : 1.0), nt / prev / (double)beta);
@@ -424,14 +429,14 @@ static int residual_check(HopeWork &W, float beta, int J, const float *P, const 
     gemb_ctx *c = W.c;
     const int b = W.b;
     GEMB_TRY(katz(W, true, beta, J, P, scr0, scr1, scr2));       // scr0 = S^T P
-    GEMB_CUDA(cudaMemsetAsync(W.scal, 0, sizeof(double) * b, c->stream));
+    GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, sizeof(double) * b, c->stream));
     const int threads = (256 / b) * b > 0 ? (256 / b) * b : b;
-    coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(W.rows, b, scr0, Qs, W.scal);
+    coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(W.rows, b, scr0, Qs, W.scal.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    GEMB_TRY(comm_allreduce_f64(W, W.scal, b));
+    GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), b));
     std::vector<double> rs(b);
-    GEMB_CUDA(cudaMemcpyAsync(rs.data(), W.scal, sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(rs.data(), W.scal.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     double rm = 0.0;
     for (int j : cols) rm = std::max(rm, sqrt(rs[j]) / std::max(smax, 1e-300));
@@ -453,14 +458,14 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
     for (int it = 1; it <= o.max_iters; it++) {
         R.iters = it;
         GEMB_TRY(katz(W, false, beta, J, V, U, T1, T2));              // U = S V
-        GEMB_TRY(gram_full(W, U, U, W.G));                            // T = U^T U
-        GEMB_CUDA(cudaMemcpyAsync(W.G2, W.G, sizeof(double) * b * b, cudaMemcpyDeviceToDevice, c->stream));
+        GEMB_TRY(gram_full(W, U, U, W.G.get()));                            // T = U^T U
+        GEMB_CUDA(cudaMemcpyAsync(W.G2.get(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToDevice, c->stream));
         GEMB_TRY(c->t_dense.begin(c->stream));
         // Jacobi accuracy follows the requested tolerance (Z only pre-rotates the CholeskyQR and forms the Ritz vectors:
         // an off-diagonal remainder of 1e-2 tol is invisible at tol; one sweep less per round at the bench setting)
-        GEMB_TRY(eigh_launch(c, b, W.G2, W.w, W.Z, W.Zs, std::min(1e-5, std::max(1e-13, 1e-2 * (double)o.tol))));
+        GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)o.tol))));
         GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(theta.data(), W.w, sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(theta.data(), W.w.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         const double tmax = std::max(theta[b - 1], 1e-300);
         double change = 0.0;
@@ -480,10 +485,10 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         // T1 = U Z Theta^-1/2: exactly orthonormal columns (Z diagonalises U^T U), ordered by sigma, so the
         // next block S^T T1 ~ V Z Sigma has nearly orthogonal columns whatever the spread of sigma is
         GEMB_TRY(c->t_dense.begin(c->stream));
-        ritz_maps_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, b, W.w, W.Z, W.M1, W.M2, -0.5, 0.5, 1e-10);
+        ritz_maps_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, b, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.5, 0.5, 1e-10);
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-        GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1, b, b, T1, b));
+        GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), b, b, T1, b));
         GEMB_TRY(c->t_dense.end(c->stream));
         GEMB_TRY(katz(W, true, beta, J, T1, Wk, U, T2));              // Wk = S^T T1   (U is scratch now)
         GEMB_TRY(cholqr2(W, Wk, T1, V));                              // V = orth(S^T orth(S V))
@@ -493,40 +498,41 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
     // extraction: X = [U Z_k theta^-1/4 | V Z_k theta^1/4]; U = S V (un-normalised), V orthonormal
     R.Xd = T1;
     if ((size_t)d > (size_t)b) {
-        GEMB_CUDA(dmalloc(&R.Xalloc, sizeof(float) * (size_t)std::max<int64_t>(W.rows, 1) * d));
-        R.Xd = R.Xalloc;
+        GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(W.rows, 1) * d));
+        R.Xd = R.Xalloc.get();
     }
     GEMB_TRY(c->t_dense.begin(c->stream));
-    ritz_maps_kernel<<<(b * k + 255) / 256, 256, 0, c->stream>>>(b, k, W.w, W.Z, W.M1, W.M2, -0.25, 0.25);
+    ritz_maps_kernel<<<(b * k + 255) / 256, 256, 0, c->stream>>>(b, k, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.25, 0.25);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1, k, k, R.Xd, d));
-    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2, k, k, R.Xd + k, d));
-    R.sig_dev = (float *)W.G2;  // G2 is free after eigh
-    sqrt_top_kernel<<<(k + 127) / 128, 128, 0, c->stream>>>(b, k, W.w, R.sig_dev);
+    GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), k, k, R.Xd, d));
+    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));
+    R.sig_dev = (float *)W.G2.get();  // G2 is free after eigh
+    sqrt_top_kernel<<<(k + 127) / 128, 128, 0, c->stream>>>(b, k, W.w.get(), R.sig_dev);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     GEMB_TRY(c->t_dense.end(c->stream));
 
     if (o.compute_residual) {
         // left vectors P = U Z theta^-1/2 (all b Ritz pairs), right Q sigma = V Z theta^1/2
-        ritz_maps_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, b, W.w, W.Z, W.M1, W.M2, -0.5, 0.5);
+        ritz_maps_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, b, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.5, 0.5);
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-        float *Pm = Wk, *Qs = nullptr, *Qalloc = nullptr, *STP = nullptr;
-        const size_t blk = sizeof(float) * (size_t)W.shard * b;
-        if (R.Xalloc) Qs = T1;
-        else { GEMB_CUDA(dmalloc(&Qalloc, blk ? blk : 4)); GEMB_CUDA(cudaMemsetAsync(Qalloc, 0, blk, c->stream)); Qs = Qalloc; }
-        GEMB_CUDA(dmalloc(&STP, blk ? blk : 4));
-        GEMB_CUDA(cudaMemsetAsync(STP, 0, blk, c->stream));
-        int s = apply_launch(c, W.rows, U, b, W.M1, b, b, Pm, b);
-        if (s == GEMB_OK) s = apply_launch(c, W.rows, V, b, W.M2, b, b, Qs, b);
+        float *Pm = Wk, *Qs = T1;
+        const size_t blk = (size_t)W.shard * b;
+        DeviceBuffer<float> Qalloc, STP;
+        if (!R.Xalloc.get()) {
+            GEMB_CUDA(Qalloc.alloc(blk));
+            GEMB_CUDA(cudaMemsetAsync(Qalloc.get(), 0, sizeof(float) * blk, c->stream));
+            Qs = Qalloc.get();
+        }
+        GEMB_CUDA(STP.alloc(blk));
+        GEMB_CUDA(cudaMemsetAsync(STP.get(), 0, sizeof(float) * blk, c->stream));
+        GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), b, b, Pm, b));
+        GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), b, b, Qs, b));
         std::vector<int> cols;
         for (int j = b - k; j < b; j++) cols.push_back(j);
-        if (s == GEMB_OK) s = residual_check(W, beta, J, Pm, Qs, STP, U, T2, cols, R.sigma_max, &R.resid_max);
-        dfree(STP);
-        dfree(Qalloc);
-        if (s != GEMB_OK) return s;
+        GEMB_TRY(residual_check(W, beta, J, Pm, Qs, STP.get(), U, T2, cols, R.sigma_max, &R.resid_max));
     }
     return GEMB_OK;
 }
@@ -538,16 +544,16 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
 static int orth_rotated(HopeWork &W, const float *F, float *tmp, float *dst) {
     gemb_ctx *c = W.c;
     const int b = W.b;
-    GEMB_TRY(gram_full(W, F, F, W.G));
+    GEMB_TRY(gram_full(W, F, F, W.G.get()));
     GEMB_TRY(c->t_dense.begin(c->stream));
-    GEMB_TRY(small_gemm_launch(c, b, W.G, 0, W.Z, W.Zs, nullptr));        // Zs = G Z
-    GEMB_TRY(small_gemm_launch(c, b, W.Z, 1, W.Zs, W.G, nullptr));        // G  = Z^T G Z
-    GEMB_TRY(chol_inverse_launch(c, b, W.G, W.Minv, W.rank_dev, W.G2));   // G2 = R^-1 (fp64)
-    GEMB_TRY(small_gemm_launch(c, b, W.Z, 0, W.G2, nullptr, W.M1));       // M1 = Z R^-1
-    GEMB_TRY(apply_launch(c, W.rows, F, b, W.M1, b, b, tmp, b));
+    GEMB_TRY(small_gemm_launch(c, b, W.G.get(), 0, W.Z.get(), W.Zs.get(), nullptr));        // Zs = G Z
+    GEMB_TRY(small_gemm_launch(c, b, W.Z.get(), 1, W.Zs.get(), W.G.get(), nullptr));        // G  = Z^T G Z
+    GEMB_TRY(chol_inverse_launch(c, b, W.G.get(), W.Minv.get(), W.rank_dev.get(), W.G2.get()));   // G2 = R^-1 (fp64)
+    GEMB_TRY(small_gemm_launch(c, b, W.Z.get(), 0, W.G2.get(), nullptr, W.M1.get()));       // M1 = Z R^-1
+    GEMB_TRY(apply_launch(c, W.rows, F, b, W.M1.get(), b, b, tmp, b));
     GEMB_TRY(c->t_dense.end(c->stream));
-    GEMB_TRY(gram_full(W, tmp, tmp, W.G));
-    GEMB_TRY(cholqr_pass(W, W.G, tmp, dst));
+    GEMB_TRY(gram_full(W, tmp, tmp, W.G.get()));
+    GEMB_TRY(cholqr_pass(W, W.G.get(), tmp, dst));
     return GEMB_OK;
 }
 
@@ -568,22 +574,22 @@ static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t 
     gemb_ctx *c = W.c;
     const int b = W.b;
     int rank = b;
-    GEMB_CUDA(cudaMemcpyAsync(&rank, W.rank_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(&rank, W.rank_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     if (rank >= b) return GEMB_OK;      // the Gram is all-reduced: every rank takes the same branch
     GEMB_TRY(randn_launch(c, W.rows, b, seed, (uint64_t)W.g->row0, s1));
-    GEMB_TRY(gram_full(W, V, V, W.G));
+    GEMB_TRY(gram_full(W, V, V, W.G.get()));
     const int64_t count = W.rows * (int64_t)b;
     if (count > 0) {
         const int grid = (int)std::min<int64_t>((count + 255) / 256, (int64_t)c->sm_count * 8);
-        refill_cols_kernel<<<grid, 256, 0, c->stream>>>(count, b, W.G, s1, V);
+        refill_cols_kernel<<<grid, 256, 0, c->stream>>>(count, b, W.G.get(), s1, V);
         GEMB_CUDA(cudaGetLastError());
         count_launch();
     }
-    GEMB_TRY(gram_full(W, V, V, W.G));
-    GEMB_TRY(cholqr_pass(W, W.G, V, s2));
-    GEMB_TRY(gram_full(W, s2, s2, W.G));
-    GEMB_TRY(cholqr_pass(W, W.G, s2, V));
+    GEMB_TRY(gram_full(W, V, V, W.G.get()));
+    GEMB_TRY(cholqr_pass(W, W.G.get(), V, s2));
+    GEMB_TRY(gram_full(W, s2, s2, W.G.get()));
+    GEMB_TRY(cholqr_pass(W, W.G.get(), s2, V));
     return GEMB_OK;
 }
 
@@ -614,15 +620,15 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[0], 0.f, false, 1.f, nullptr, pool[1], true, W.halo));
     GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[1], 0.f, false, 1.f, nullptr, pool[2], true, W.halo));
     GEMB_TRY(dist_spmm(W, false, b, 1.f, pool[2], nullptr, AV, true));
-    GEMB_TRY(gram_full(W, AV, AV, W.G));
-    GEMB_TRY(cholqr_pass(W, W.G, AV, pool[0]));
+    GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
+    GEMB_TRY(cholqr_pass(W, W.G.get(), AV, pool[0]));
     int rank1 = b;
-    GEMB_CUDA(cudaMemcpyAsync(&rank1, W.rank_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(&rank1, W.rank_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     const bool careful = rank1 < b;
     if (!careful) {
-        GEMB_TRY(gram_full(W, pool[0], pool[0], W.G));
-        GEMB_TRY(cholqr_pass(W, W.G, pool[0], V));
+        GEMB_TRY(gram_full(W, pool[0], pool[0], W.G.get()));
+        GEMB_TRY(cholqr_pass(W, W.G.get(), pool[0], V));
         GEMB_TRY(publish(W, V, b));
     }
     if (careful) {
@@ -671,8 +677,8 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         R.iters = it;
         // Rayleigh-Ritz on A: T = V^T A V, (l, Z) = eigh(T)
         GEMB_TRY(dist_spmm(W, false, b, 1.f, V, nullptr, AV, true));
-        GEMB_TRY(gram_full(W, V, AV, W.G2));
-        symmetrize_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, W.G2);
+        GEMB_TRY(gram_full(W, V, AV, W.G2.get()));
+        symmetrize_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, W.G2.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
         // (Measured: running the single-CTA Jacobi on a side stream while the filter starts with the PREVIOUS
@@ -681,9 +687,9 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         GEMB_TRY(c->t_dense.begin(c->stream));
         // Jacobi accuracy follows the requested tolerance (Z only pre-rotates the CholeskyQR and forms the Ritz vectors:
         // an off-diagonal remainder of 1e-2 tol is invisible at tol; one sweep less per round at the bench setting)
-        GEMB_TRY(eigh_launch(c, b, W.G2, W.w, W.Z, W.Zs, std::min(1e-5, std::max(1e-13, 1e-2 * (double)o.tol))));
+        GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)o.tol))));
         GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(lam.data(), W.w, sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(lam.data(), W.w.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         float *filtered = nullptr;
         if (ritz_bound) {
@@ -717,9 +723,9 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
             // residual of the Ritz pairs from the Rayleigh-Ritz products alone: with V orthonormal and (l, z) an
             // eigenpair of V^T A V,  ||A V z - l V z||^2 = z^T (AV)^T (AV) z - l^2.  Mapped to the Katz operator
             // through |f'(l)| = beta / (1 - beta l)^2 and measured against sigma_max, like compute_residual does.
-            GEMB_TRY(gram_full(W, AV, AV, W.G));
-            GEMB_CUDA(cudaMemcpyAsync(Wh.data(), W.G, sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
-            GEMB_CUDA(cudaMemcpyAsync(Zr.data(), W.Z, sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
+            GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
+            GEMB_CUDA(cudaMemcpyAsync(Wh.data(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
+            GEMB_CUDA(cudaMemcpyAsync(Zr.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
             GEMB_CUDA(cudaStreamSynchronize(c->stream));
             double worst = 0.0;
             for (int j = 0; j < k; j++) {
@@ -791,7 +797,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     if (mode) {
         // ---- largest algebraic eigenpairs, DESCENDING (= ascending eigenvalues of I - A_hat, the order lap.py:28-31 sorts into)
         std::vector<double> Zh((size_t)b * b);
-        GEMB_CUDA(cudaMemcpyAsync(Zh.data(), W.Z, sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         std::vector<float> M1((size_t)b * k), ev(k);
         for (int j = 0; j < k; j++) {
@@ -800,13 +806,13 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
             for (int i = 0; i < b; i++) M1[(size_t)i * k + j] = (float)Zh[(size_t)i * b + col];
         }
         R.sigma_max = gval[order[0]];
-        GEMB_CUDA(cudaMemcpyAsync(W.M1, M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
-        R.sig_dev = (float *)W.G2;
+        GEMB_CUDA(cudaMemcpyAsync(W.M1.get(), M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
+        R.sig_dev = (float *)W.G2.get();
         GEMB_CUDA(cudaMemcpyAsync(R.sig_dev, ev.data(), sizeof(float) * k, cudaMemcpyHostToDevice, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         R.Xd = pool[0];
         GEMB_TRY(c->t_dense.begin(c->stream));
-        GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1, k, k, R.Xd, k));
+        GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), k, k, R.Xd, k));
         GEMB_TRY(c->t_dense.end(c->stream));
         return GEMB_OK;
     }
@@ -814,7 +820,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     std::vector<int> sel(order.begin(), order.begin() + k);
     std::reverse(sel.begin(), sel.end());                             // ascending |f|
     std::vector<double> Zh((size_t)b * b);
-    GEMB_CUDA(cudaMemcpyAsync(Zh.data(), W.Z, sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     std::vector<float> M1((size_t)b * k), M2((size_t)b * k), sig(k);
     for (int j = 0; j < k; j++) {
@@ -829,19 +835,19 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         }
     }
     R.sigma_max = gval[order[0]];
-    GEMB_CUDA(cudaMemcpyAsync(W.M1, M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(W.M2, M2.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
-    R.sig_dev = (float *)W.G2;
+    GEMB_CUDA(cudaMemcpyAsync(W.M1.get(), M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(W.M2.get(), M2.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
+    R.sig_dev = (float *)W.G2.get();
     GEMB_CUDA(cudaMemcpyAsync(R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));                      // host staging vectors go out of scope
     R.Xd = pool[0];
     if ((size_t)d > (size_t)b) {
-        GEMB_CUDA(dmalloc(&R.Xalloc, sizeof(float) * (size_t)std::max<int64_t>(W.rows, 1) * d));
-        R.Xd = R.Xalloc;
+        GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(W.rows, 1) * d));
+        R.Xd = R.Xalloc.get();
     }
     GEMB_TRY(c->t_dense.begin(c->stream));
-    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1, k, k, R.Xd, d));
-    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2, k, k, R.Xd + k, d));
+    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), k, k, R.Xd, d));
+    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));
     GEMB_TRY(c->t_dense.end(c->stream));
 
     if (o.compute_residual) {
@@ -857,27 +863,29 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
                 MQ[(size_t)i * b + col] = (float)(z * fabs(f));       // v sigma
             }
         }
-        float *dMP = nullptr, *dMQ = nullptr, *Palloc = nullptr, *Q = nullptr, *STP = nullptr;
-        const size_t blk = sizeof(float) * (size_t)W.shard * b;
-        GEMB_CUDA(dmalloc(&dMP, sizeof(float) * b * b));
-        GEMB_CUDA(dmalloc(&dMQ, sizeof(float) * b * b));
+        DeviceBuffer<float> dMP, dMQ, Palloc, Q, STP;
+        const size_t blk = (size_t)W.shard * b;
+        GEMB_CUDA(dMP.alloc(b * b));
+        GEMB_CUDA(dMQ.alloc(b * b));
         // every SpMM INPUT must be a work block in halo mode (its rows travel to the peers): P lives in AV, the Horner
         // scratch in pool[1] / pool[2]; pool[0] may hold the result X and stays untouched
         float *P = AV;
-        if (!W.halo) { GEMB_CUDA(dmalloc(&Palloc, blk ? blk : 4)); GEMB_CUDA(cudaMemsetAsync(Palloc, 0, blk, c->stream)); P = Palloc; }
-        GEMB_CUDA(dmalloc(&Q, blk ? blk : 4));
-        GEMB_CUDA(dmalloc(&STP, blk ? blk : 4));
-        GEMB_CUDA(cudaMemsetAsync(Q, 0, blk, c->stream));
-        GEMB_CUDA(cudaMemsetAsync(STP, 0, blk, c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(dMP, MP.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(dMQ, MQ.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
-        int s = apply_launch(c, W.rows, V, b, dMP, b, b, P, b);
-        if (s == GEMB_OK) s = apply_launch(c, W.rows, V, b, dMQ, b, b, Q, b);
-        if (s == GEMB_OK) s = publish(W, P, b);
-        if (s == GEMB_OK) s = residual_check(W, beta, J, P, Q, STP, W.halo ? pool[1] : AV, W.halo ? pool[2] : pool[1], sel, R.sigma_max, &R.resid_max);
-        cudaStreamSynchronize(c->stream);
-        dfree(dMP); dfree(dMQ); dfree(Palloc); dfree(Q); dfree(STP);
-        if (s != GEMB_OK) return s;
+        if (!W.halo) {
+            GEMB_CUDA(Palloc.alloc(blk));
+            GEMB_CUDA(cudaMemsetAsync(Palloc.get(), 0, sizeof(float) * blk, c->stream));
+            P = Palloc.get();
+        }
+        GEMB_CUDA(Q.alloc(blk));
+        GEMB_CUDA(STP.alloc(blk));
+        GEMB_CUDA(cudaMemsetAsync(Q.get(), 0, sizeof(float) * blk, c->stream));
+        GEMB_CUDA(cudaMemsetAsync(STP.get(), 0, sizeof(float) * blk, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(dMP.get(), MP.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(dMQ.get(), MQ.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
+        GEMB_TRY(apply_launch(c, W.rows, V, b, dMP.get(), b, b, P, b));
+        GEMB_TRY(apply_launch(c, W.rows, V, b, dMQ.get(), b, b, Q.get(), b));
+        GEMB_TRY(publish(W, P, b));
+        GEMB_TRY(residual_check(W, beta, J, P, Q.get(), STP.get(), W.halo ? pool[1] : AV, W.halo ? pool[2] : pool[1], sel,
+                                R.sigma_max, &R.resid_max));
     }
     return GEMB_OK;
 }
@@ -935,26 +943,20 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
     const int nchunk = (m_max + cw - 1) / cw;
     const int mt = m_max + p;                                    // T carries the coupling block of the next q too
     const size_t chunk_bytes = sizeof(float) * (size_t)shard * cw;
-    std::vector<float *> Q(nchunk, nullptr), Qn((k_keep + cw - 1) / cw, nullptr);
-    struct Free { std::vector<float *> *a, *b; float *t[3]; double *g[3]; float *m32;
-                  ~Free() { for (auto x : *a) dfree(x); for (auto x : *b) dfree(x); for (auto x : t) dfree(x); for (auto x : g) dfree(x); dfree(m32); } }
-        guard{&Q, &Qn, {nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}, nullptr};
-    for (auto &q : Q) { GEMB_CUDA(dmalloc(&q, chunk_bytes ? chunk_bytes : 4)); GEMB_CUDA(cudaMemsetAsync(q, 0, chunk_bytes, c->stream)); }
-    for (auto &q : Qn) { GEMB_CUDA(dmalloc(&q, chunk_bytes ? chunk_bytes : 4)); }
+    std::vector<DeviceBuffer<float>> Q(nchunk), Qn((k_keep + cw - 1) / cw);
+    for (auto &q : Q) { GEMB_CUDA(q.alloc((size_t)shard * cw)); GEMB_CUDA(cudaMemsetAsync(q.get(), 0, chunk_bytes, c->stream)); }
+    for (auto &q : Qn) GEMB_CUDA(q.alloc((size_t)shard * cw));
     // narrow blocks: Vcur (SpMM input: a halo block on N GPUs), Wb, Tb
-    float *Vcur = W.buf[0], *Wb = W.buf[1], *Tb = W.buf[2], *Tmp64 = nullptr;
-    GEMB_CUDA(dmalloc(&guard.t[0], chunk_bytes ? chunk_bytes : 4));
-    Tmp64 = guard.t[0];
-    double *Gd = nullptr, *Td = nullptr, *Yd = nullptr;          // device: small Gram (cw x p), T (m x m), Y
-    GEMB_CUDA(dmalloc(&guard.g[0], sizeof(double) * (size_t)cw * cw)); Gd = guard.g[0];
-    GEMB_CUDA(dmalloc(&guard.g[1], sizeof(double) * (size_t)mt * mt)); Td = guard.g[1];
-    GEMB_CUDA(dmalloc(&guard.g[2], sizeof(double) * (size_t)mt * mt)); Yd = guard.g[2];
-    GEMB_CUDA(dmalloc(&guard.m32, sizeof(float) * (size_t)cw * cw));
-    float *M32 = guard.m32;
-    double *wd = nullptr, *Zs = nullptr;
-    GEMB_CUDA(dmalloc(&wd, sizeof(double) * mt));
-    GEMB_CUDA(dmalloc(&Zs, sizeof(double) * (size_t)mt * mt));
-    struct Free2 { double *a, *b; ~Free2() { dfree(a); dfree(b); } } guard2{wd, Zs};
+    float *Vcur = W.buf[0], *Wb = W.buf[1], *Tb = W.buf[2];
+    DeviceBuffer<float> Tmp64, M32;
+    DeviceBuffer<double> Gd, Td, Yd, wd, Zs;                     // device: small Gram (cw x p), T (m x m), Y, eigh's w and scratch
+    GEMB_CUDA(Tmp64.alloc((size_t)shard * cw));
+    GEMB_CUDA(Gd.alloc((size_t)cw * cw));
+    GEMB_CUDA(Td.alloc((size_t)mt * mt));
+    GEMB_CUDA(Yd.alloc((size_t)mt * mt));
+    GEMB_CUDA(M32.alloc((size_t)cw * cw));
+    GEMB_CUDA(wd.alloc(mt));
+    GEMB_CUDA(Zs.alloc((size_t)mt * mt));
 
     const int grid_el = c->sm_count * 8;
     auto gram_ar = [&](const float *P, int b1, const float *Qp, int b2, double *G) -> int {
@@ -967,13 +969,13 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
     std::vector<double> Rh((size_t)p * p), R1((size_t)p * p), R2((size_t)p * p), Ginv((size_t)p * p);
     auto cholqr_p = [&](float *src, float *scratch, double *Rout) -> int {
         for (int pass = 0; pass < 2; pass++) {
-            GEMB_TRY(gram_ar(src, p, src, p, W.G));
+            GEMB_TRY(gram_ar(src, p, src, p, W.G.get()));
             GEMB_TRY(c->t_dense.begin(c->stream));
-            GEMB_TRY(chol_inverse_launch(c, p, W.G, W.Minv, W.rank_dev, W.G2));     // G2 = R^-1 (fp64)
-            GEMB_TRY(apply_launch(c, rows, src, p, W.Minv, p, p, scratch, p));
+            GEMB_TRY(chol_inverse_launch(c, p, W.G.get(), W.Minv.get(), W.rank_dev.get(), W.G2.get()));     // G2 = R^-1 (fp64)
+            GEMB_TRY(apply_launch(c, rows, src, p, W.Minv.get(), p, p, scratch, p));
             GEMB_TRY(c->t_dense.end(c->stream));
             GEMB_CUDA(cudaMemcpyAsync(src, scratch, sizeof(float) * (size_t)rows * p, cudaMemcpyDeviceToDevice, c->stream));
-            GEMB_CUDA(cudaMemcpyAsync(Ginv.data(), W.G2, sizeof(double) * p * p, cudaMemcpyDeviceToHost, c->stream));
+            GEMB_CUDA(cudaMemcpyAsync(Ginv.data(), W.G2.get(), sizeof(double) * p * p, cudaMemcpyDeviceToHost, c->stream));
             GEMB_CUDA(cudaStreamSynchronize(c->stream));
             // invert the upper-triangular R^-1 on the host (p = 16): R = (R^-1)^-1; dropped columns (zero pivot) stay zero
             std::vector<double> &Rt = pass == 0 ? R1 : R2;
@@ -1009,7 +1011,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
     bool done = false;
     while (!done) {
         // ---- append q_j, expand
-        put_cols_kernel<<<grid_el, 256, 0, c->stream>>>(rows, p, Vcur, Q[m / cw], cw, m % cw);
+        put_cols_kernel<<<grid_el, 256, 0, c->stream>>>(rows, p, Vcur, Q[m / cw].get(), cw, m % cw);
         GEMB_CUDA(cudaGetLastError());
         count_launch();
         const int j0 = m;
@@ -1021,16 +1023,16 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
         const int nc_live = (m + cw - 1) / cw;
         for (int pass = 0; pass < 2; pass++) {
             for (int cc = 0; cc < nc_live; cc++) {
-                GEMB_TRY(gram_ar(Q[cc], cw, Wb, p, Gd));                               // H_c = Q_c^T W   (cw x p)
+                GEMB_TRY(gram_ar(Q[cc].get(), cw, Wb, p, Gd.get()));                               // H_c = Q_c^T W   (cw x p)
                 GEMB_TRY(c->t_dense.begin(c->stream));
-                f64_to_f32_kernel<<<(cw * p + 255) / 256, 256, 0, c->stream>>>(cw * p, Gd, M32);
+                f64_to_f32_kernel<<<(cw * p + 255) / 256, 256, 0, c->stream>>>(cw * p, Gd.get(), M32.get());
                 GEMB_CUDA(cudaGetLastError());
-                GEMB_TRY(apply_launch(c, rows, Q[cc], cw, M32, p, p, Tb, p));           // Q_c H_c
+                GEMB_TRY(apply_launch(c, rows, Q[cc].get(), cw, M32.get(), p, p, Tb, p));           // Q_c H_c
                 axpy_kernel<<<grid_el, 256, 0, c->stream>>>(rows * (int64_t)p, -1.f, Tb, Wb, 1);
                 GEMB_CUDA(cudaGetLastError());
                 count_launch(2);
                 GEMB_TRY(c->t_dense.end(c->stream));
-                GEMB_CUDA(cudaMemcpyAsync(Hc.data(), Gd, sizeof(double) * cw * p, cudaMemcpyDeviceToHost, c->stream));
+                GEMB_CUDA(cudaMemcpyAsync(Hc.data(), Gd.get(), sizeof(double) * cw * p, cudaMemcpyDeviceToHost, c->stream));
                 GEMB_CUDA(cudaStreamSynchronize(c->stream));
                 for (int r = 0; r < cw && cc * cw + r < m; r++)
                     for (int q = 0; q < p; q++) Hcol[(size_t)(cc * cw + r) * p + q] += Hc[(size_t)r * p + q];
@@ -1057,12 +1059,12 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
         // ---- Rayleigh-Ritz on T[0:m, 0:m]
         std::vector<double> Tm((size_t)m * m);
         for (int r = 0; r < m; r++) for (int q = 0; q < m; q++) Tm[(size_t)r * m + q] = T[(size_t)r * mt + q];
-        GEMB_CUDA(cudaMemcpyAsync(Td, Tm.data(), sizeof(double) * m * m, cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(Td.get(), Tm.data(), sizeof(double) * m * m, cudaMemcpyHostToDevice, c->stream));
         GEMB_TRY(c->t_dense.begin(c->stream));
-        GEMB_TRY(eigh_launch(c, m, Td, wd, Yd, Zs, 1e-9));      // Ritz values are needed to ~1e-6, the vectors feed fp32 GEMMs
+        GEMB_TRY(eigh_launch(c, m, Td.get(), wd.get(), Yd.get(), Zs.get(), 1e-9));      // Ritz values are needed to ~1e-6, the vectors feed fp32 GEMMs
         GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(theta.data(), wd, sizeof(double) * m, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(Y.data(), Yd, sizeof(double) * m * m, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(theta.data(), wd.get(), sizeof(double) * m, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(Y.data(), Yd.get(), sizeof(double) * m * m, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         double amax = 0.0;
         for (int i = 0; i < m; i++) amax = std::max(amax, fabs(theta[i]));
@@ -1103,12 +1105,12 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                 std::vector<float> Mh((size_t)cw * cw, 0.f);
                 for (int r = 0; r < cw && cc * cw + r < m; r++)
                     for (int q = 0; q < ow; q++) Mh[(size_t)r * cw + q] = (float)Y[(size_t)(cc * cw + r) * m + order[oc * cw + q]];
-                GEMB_CUDA(cudaMemcpyAsync(M32, Mh.data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice, c->stream));
+                GEMB_CUDA(cudaMemcpyAsync(M32.get(), Mh.data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice, c->stream));
                 GEMB_CUDA(cudaStreamSynchronize(c->stream));
                 GEMB_TRY(c->t_dense.begin(c->stream));
-                GEMB_TRY(apply_launch(c, rows, Q[cc], cw, M32, cw, cw, cc == 0 ? Qn[oc] : Tmp64, cw));
+                GEMB_TRY(apply_launch(c, rows, Q[cc].get(), cw, M32.get(), cw, cw, cc == 0 ? Qn[oc].get() : Tmp64.get(), cw));
                 if (cc > 0) {
-                    axpy_kernel<<<grid_el, 256, 0, c->stream>>>(rows * (int64_t)cw, 1.f, Tmp64, Qn[oc], 1);
+                    axpy_kernel<<<grid_el, 256, 0, c->stream>>>(rows * (int64_t)cw, 1.f, Tmp64.get(), Qn[oc].get(), 1);
                     GEMB_CUDA(cudaGetLastError());
                     count_launch();
                 }
@@ -1120,8 +1122,8 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
             std::vector<float> sig(k);
             R.sigma_max = smax;
             R.Xd = nullptr;
-            GEMB_CUDA(dmalloc(&R.Xalloc, sizeof(float) * (size_t)std::max<int64_t>(rows, 1) * d));
-            R.Xd = R.Xalloc;
+            GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(rows, 1) * d));
+            R.Xd = R.Xalloc.get();
             GEMB_ARG(k <= cw * (int)Qn.size(), "k");
             // per-column scaling on the host: column jj of Qn <-> order[jj] (descending |f|); output column k-1-jj
             std::vector<float> Ms((size_t)cw * cw), Mt((size_t)cw * cw);
@@ -1137,24 +1139,24 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                     Mt[(size_t)q * cw + q] = (float)rt;
                 }
                 for (int half = 0; half < 2; half++) {
-                    GEMB_CUDA(cudaMemcpyAsync(M32, (half == 0 ? Ms : Mt).data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice, c->stream));
+                    GEMB_CUDA(cudaMemcpyAsync(M32.get(), (half == 0 ? Ms : Mt).data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice, c->stream));
                     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-                    GEMB_TRY(apply_launch(c, rows, Qn[oc], cw, M32, cw, cw, Tmp64, cw));
+                    GEMB_TRY(apply_launch(c, rows, Qn[oc].get(), cw, M32.get(), cw, cw, Tmp64.get(), cw));
                     // reversed column order into X: source column q -> X column (half*k) + k-1-(oc*cw+q)
-                    reverse_put_kernel<<<grid_el, 256, 0, c->stream>>>(rows, ow, Tmp64, cw, R.Xd, d, half * k + k - 1 - oc * cw);
+                    reverse_put_kernel<<<grid_el, 256, 0, c->stream>>>(rows, ow, Tmp64.get(), cw, R.Xd, d, half * k + k - 1 - oc * cw);
                     GEMB_CUDA(cudaGetLastError());
                     count_launch();
                 }
             }
-            R.sig_dev = (float *)W.G2;
+            R.sig_dev = (float *)W.G2.get();
             GEMB_CUDA(cudaMemcpyAsync(R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice, c->stream));
             GEMB_CUDA(cudaStreamSynchronize(c->stream));
             break;
         }
         // ---- restart: new basis = Qn (nk columns), T = diag(theta_keep); q_{j+1} (= Vcur) is appended next
         for (int oc = 0; oc < nchunk; oc++) {
-            if (oc < ncn) GEMB_CUDA(cudaMemcpyAsync(Q[oc], Qn[oc], chunk_bytes, cudaMemcpyDeviceToDevice, c->stream));
-            else GEMB_CUDA(cudaMemsetAsync(Q[oc], 0, chunk_bytes, c->stream));
+            if (oc < ncn) GEMB_CUDA(cudaMemcpyAsync(Q[oc].get(), Qn[oc].get(), chunk_bytes, cudaMemcpyDeviceToDevice, c->stream));
+            else GEMB_CUDA(cudaMemsetAsync(Q[oc].get(), 0, chunk_bytes, c->stream));
         }
         std::fill(T.begin(), T.end(), 0.0);
         for (int q = 0; q < nk; q++) T[(size_t)q * mt + q] = theta[order[q]];
@@ -1205,17 +1207,16 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
     HopeWork W;
     W.g = g; W.c = c; W.b = w; W.rows = n; W.shard = n;
     const size_t blk = sizeof(float) * (size_t)n * w;
-    for (int i = 0; i < 5; i++) { GEMB_CUDA(dmalloc(&W.buf[i], blk)); GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, blk, c->stream)); }
-    GEMB_CUDA(dmalloc(&W.scal, sizeof(double) * (w + 8)));
-    GEMB_CUDA(dmalloc(&W.G, sizeof(double) * (size_t)k * w));
-    GEMB_CUDA(dmalloc(&W.M1, sizeof(float) * (size_t)k * w));
-    float *Xd = nullptr, *L = nullptr, *Rr = nullptr;
-    GEMB_CUDA(dmalloc(&Xd, sizeof(float) * (size_t)n * d));
-    GEMB_CUDA(dmalloc(&L, sizeof(float) * (size_t)n * k));
-    GEMB_CUDA(dmalloc(&Rr, sizeof(float) * (size_t)n * k));
-    struct Guard { float *a, *b, *c; ~Guard() { dfree(a); dfree(b); dfree(c); } } guard{Xd, L, Rr};
-    GEMB_CUDA(cudaMemcpyAsync(Xd, X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
-    split_halves_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n, d, Xd, L, Rr);
+    GEMB_TRY(W.alloc_blocks((size_t)n * w));
+    GEMB_CUDA(W.scal.alloc(w + 8));
+    GEMB_CUDA(W.G.alloc((size_t)k * w));
+    GEMB_CUDA(W.M1.alloc((size_t)k * w));
+    DeviceBuffer<float> Xd, L, Rr;
+    GEMB_CUDA(Xd.alloc((size_t)n * d));
+    GEMB_CUDA(L.alloc((size_t)n * k));
+    GEMB_CUDA(Rr.alloc((size_t)n * k));
+    GEMB_CUDA(cudaMemcpyAsync(Xd.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
+    split_halves_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n, d, Xd.get(), L.get(), Rr.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     c->t_spmm.reset(); c->t_dense.reset(); c->t_comm.reset();
@@ -1238,16 +1239,16 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
         GEMB_CUDA(cudaGetLastError());
         count_launch();
         GEMB_TRY(katz(W, false, beta, J, Z, SZ, W.buf[3], W.buf[4]));             // S Z
-        GEMB_TRY(gram_launch(c, n, Rr, k, Z, w, W.G));                            // X2^T Z   (k x w, fp64)
-        f64_to_f32_kernel<<<(k * w + 255) / 256, 256, 0, c->stream>>>(k * w, W.G, W.M1);
+        GEMB_TRY(gram_launch(c, n, Rr.get(), k, Z, w, W.G.get()));                            // X2^T Z   (k x w, fp64)
+        f64_to_f32_kernel<<<(k * w + 255) / 256, 256, 0, c->stream>>>(k * w, W.G.get(), W.M1.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-        GEMB_TRY(apply_launch(c, n, L, k, W.M1, w, w, LZ, w));                    // X1 (X2^T Z)
-        GEMB_CUDA(cudaMemsetAsync(W.scal, 0, sizeof(double) * w, c->stream));
-        coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(n, w, LZ, SZ, W.scal);
+        GEMB_TRY(apply_launch(c, n, L.get(), k, W.M1.get(), w, w, LZ, w));                    // X1 (X2^T Z)
+        GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, sizeof(double) * w, c->stream));
+        coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(n, w, LZ, SZ, W.scal.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-        GEMB_CUDA(cudaMemcpyAsync(rs.data(), W.scal, sizeof(double) * w, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(rs.data(), W.scal.get(), sizeof(double) * w, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
         for (int j = 0; j < live; j++) acc += rs[j];
     }
@@ -1317,13 +1318,13 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         if (hs == GEMB_OK) hs = halo_buffers(g, 5, b);
         NcclApi *api = nccl_api();
         if (!api) return GEMB_ERR_NCCL;
-        int *flag = nullptr, hflag = (hs == GEMB_OK) ? 1 : 0;
-        GEMB_CUDA(dmalloc(&flag, sizeof(int)));
-        GEMB_CUDA(cudaMemcpyAsync(flag, &hflag, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-        ncclResult_t r = api->AllReduce(flag, flag, 1, ncclInt, ncclMin, (ncclComm_t)c->comm, c->stream);
-        GEMB_CUDA(cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        int hflag = (hs == GEMB_OK) ? 1 : 0;
+        DeviceBuffer<int> flag;
+        GEMB_CUDA(flag.alloc(1));
+        GEMB_CUDA(cudaMemcpyAsync(flag.get(), &hflag, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+        ncclResult_t r = api->AllReduce(flag.get(), flag.get(), 1, ncclInt, ncclMin, (ncclComm_t)c->comm, c->stream);
+        GEMB_CUDA(cudaMemcpyAsync(&hflag, flag.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        dfree(flag);
         if (r != ncclSuccess) { set_error("ncclAllReduce(halo agreement): %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
         W.halo = hflag == 1;
         if (!W.halo && o.verbose) fprintf(stderr, "[gemb_hope] halo exchange unavailable (%s); all-gather per sweep\n", gemb_last_error());
@@ -1332,29 +1333,25 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         for (int i = 0; i < 5; i++) W.buf[i] = g->halo.buf[i];
         GEMB_TRY(halo_barrier(g));    // every rank's blocks are in place before the first push can arrive
     } else {
-        for (int i = 0; i < 5; i++) {
-            GEMB_CUDA(dmalloc(&W.buf[i], blk ? blk : 4));
-            GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, blk, c->stream));  // padded rows stay 0
-        }
-        if (c->nranks > 1) GEMB_CUDA(dmalloc(&W.full, sizeof(float) * (size_t)g->n_pad * b));
+        GEMB_TRY(W.alloc_blocks((size_t)W.shard * b));
+        if (c->nranks > 1) GEMB_CUDA(W.full.alloc((size_t)g->n_pad * b));
     }
-    GEMB_CUDA(dmalloc(&W.G, sizeof(double) * b * b));
-    GEMB_CUDA(dmalloc(&W.G2, sizeof(double) * b * b));
-    GEMB_CUDA(dmalloc(&W.Z, sizeof(double) * b * b));
-    GEMB_CUDA(dmalloc(&W.Zs, sizeof(double) * b * b));
-    GEMB_CUDA(dmalloc(&W.w, sizeof(double) * b));
-    GEMB_CUDA(dmalloc(&W.scal, sizeof(double) * (b + 8)));
-    GEMB_CUDA(dmalloc(&W.Minv, sizeof(float) * b * b));
-    GEMB_CUDA(dmalloc(&W.M1, sizeof(float) * b * b));
-    GEMB_CUDA(dmalloc(&W.M2, sizeof(float) * b * b));
-    GEMB_CUDA(dmalloc(&W.rank_dev, sizeof(int)));
+    GEMB_CUDA(W.G.alloc(b * b));
+    GEMB_CUDA(W.G2.alloc(b * b));
+    GEMB_CUDA(W.Z.alloc(b * b));
+    GEMB_CUDA(W.Zs.alloc(b * b));
+    GEMB_CUDA(W.w.alloc(b));
+    GEMB_CUDA(W.scal.alloc(b + 8));
+    GEMB_CUDA(W.Minv.alloc(b * b));
+    GEMB_CUDA(W.M1.alloc(b * b));
+    GEMB_CUDA(W.M2.alloc(b * b));
+    GEMB_CUDA(W.rank_dev.alloc(1));
 
     c->t_spmm.reset(); c->t_dense.reset(); c->t_comm.reset(); c->t_misc.reset();
     const double t_alloc = now();
-    cudaEvent_t ev0, ev1;
-    GEMB_CUDA(cudaEventCreate(&ev0));
-    GEMB_CUDA(cudaEventCreate(&ev1));
-    GEMB_CUDA(cudaEventRecord(ev0, c->stream));
+    CallEvents<2> ev;
+    GEMB_CUDA(ev.create());
+    GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
 
     double nrm = 0.0, hard_bound = 0.0;
     int J = o.katz_terms;
@@ -1363,7 +1360,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         // beta given relative to the spectral radius: beta = |beta| / ||A||_2 (= rho(A) for the symmetric graphs of
         // BASELINE.json configs[3]: "beta = 0.5 / rho_hat"), ||A||_2 by power iteration on a width-4 block
         GEMB_TRY(estimate_norm2(W, o.seed, W.buf[3], W.buf[4], W.buf[2], &nrm));
-        if (!(nrm > 0.0)) { set_error("beta < 0 asks for beta = |beta| / ||A||_2, but ||A||_2 = 0 (empty graph)"); cudaEventDestroy(ev0); cudaEventDestroy(ev1); return GEMB_ERR_ARG; }
+        if (!(nrm > 0.0)) { set_error("beta < 0 asks for beta = |beta| / ||A||_2, but ||A||_2 = 0 (empty graph)"); return GEMB_ERR_ARG; }
         beta = (float)(-(double)beta / nrm);
         have_nrm = true;
         for (int i = 2; i < 5; i++) GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, blk, c->stream));
@@ -1376,7 +1373,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         else need_power = !have_nrm;
     }
     if (have_nrm && nrm >= 0.0) {
-        if ((double)beta * nrm * 1.02 >= 1.0) { set_error("|beta| / ||A||_2 with |beta| >= 0.98: outside the Katz convergence radius"); cudaEventDestroy(ev0); cudaEventDestroy(ev1); return GEMB_ERR_DIVERGE; }
+        if ((double)beta * nrm * 1.02 >= 1.0) { set_error("|beta| / ||A||_2 with |beta| >= 0.98: outside the Katz convergence radius"); return GEMB_ERR_DIVERGE; }
         if (J <= 0) J = katz_terms_for(beta, nrm, o.katz_tol);
         if (hard_bound <= 0.0) hard_bound = nrm;
     }
@@ -1389,12 +1386,11 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
             int ps = GEMB_ERR_DIVERGE;
             if (algo == 1 && !W.halo) {
                 ps = probe_katz_terms(W, beta, o.katz_tol, o.seed, W.buf[3], W.buf[4], &Jp, &rho);
-                if (ps != GEMB_OK && ps != GEMB_ERR_DIVERGE) { cudaEventDestroy(ev0); cudaEventDestroy(ev1); return ps; }
+                if (ps != GEMB_OK && ps != GEMB_ERR_DIVERGE) return ps;
             }
             if (ps != GEMB_OK) {
                 set_error("beta * rho(A) ~ %.4g >= 1 (||A||_2 = %.4g): the Katz series (I - beta A)^-1 beta A does not "
                           "converge; choose beta < %.4g", (double)beta * rho, nrm, 1.0 / std::max(rho, 1e-300));
-                cudaEventDestroy(ev0); cudaEventDestroy(ev1);
                 return GEMB_ERR_DIVERGE;
             }
             if (J <= 0) J = Jp;
@@ -1413,29 +1409,26 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         s = hope_symmetric(W, o, d, beta, nrm, hard_bound, R);
         if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, beta, hard_bound > 0 ? hard_bound : nrm, R); }
     } else s = hope_general(W, o, d, beta, J, R);
-    if (s != GEMB_OK) { dfree(R.Xalloc); cudaEventDestroy(ev0); cudaEventDestroy(ev1); return s; }
+    if (s != GEMB_OK) return s;
 
-    GEMB_CUDA(cudaEventRecord(ev1, c->stream));
-    GEMB_CUDA(cudaEventSynchronize(ev1));
-    if (W.halo) { const int hs = halo_check_timeout(g); if (hs != GEMB_OK) { dfree(R.Xalloc); cudaEventDestroy(ev0); cudaEventDestroy(ev1); return hs; } }
+    GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
+    GEMB_CUDA(cudaEventSynchronize(ev[1]));
+    if (W.halo) GEMB_TRY(halo_check_timeout(g));
     float total_ms = 0.f;
-    GEMB_CUDA(cudaEventElapsedTime(&total_ms, ev0, ev1));
+    GEMB_CUDA(cudaEventElapsedTime(&total_ms, ev[0], ev[1]));
 
     const double t_solve = now();
     double d2h_ms = 0.0;
     if (X_out || sigma_out) {
-        cudaEvent_t e2, e3;
-        GEMB_CUDA(cudaEventCreate(&e2)); GEMB_CUDA(cudaEventCreate(&e3));
-        GEMB_CUDA(cudaEventRecord(e2, c->stream));
+        CallEvents<2> d2h;
+        GEMB_CUDA(d2h.create());
+        GEMB_CUDA(cudaEventRecord(d2h[0], c->stream));
         if (X_out) GEMB_CUDA(cudaMemcpyAsync(X_out, R.Xd, sizeof(float) * (size_t)W.rows * d, cudaMemcpyDeviceToHost, c->stream));
         if (sigma_out) GEMB_CUDA(cudaMemcpyAsync(sigma_out, R.sig_dev, sizeof(float) * k, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaEventRecord(e3, c->stream));
-        GEMB_CUDA(cudaEventSynchronize(e3));
-        float ms = 0.f; cudaEventElapsedTime(&ms, e2, e3); d2h_ms = ms;
-        cudaEventDestroy(e2); cudaEventDestroy(e3);
+        GEMB_CUDA(cudaEventRecord(d2h[1], c->stream));
+        GEMB_CUDA(cudaEventSynchronize(d2h[1]));
+        d2h_ms = d2h.ms(0, 1);
     }
-    dfree(R.Xalloc);
-    cudaEventDestroy(ev0); cudaEventDestroy(ev1);
     if (trace)
         fprintf(stderr, "[gemb_hope] host ms: alloc %.2f  solve %.2f (device %.2f)  d2h %.2f (device %.2f)\n",
                 t_alloc - t_enter, t_solve - t_alloc, total_ms, now() - t_solve, d2h_ms);

@@ -524,25 +524,19 @@ static void unigram_alias(const std::vector<int64_t> &vocab, std::vector<int32_t
 }
 
 struct N2VDev {
-    double *w = nullptr, *U = nullptr;
-    int32_t *K = nullptr, *scratch = nullptr, *order = nullptr, *walks = nullptr;
-    unsigned long long *first_pos = nullptr, *cnt = nullptr, *pairs = nullptr;
-    int32_t *KT = nullptr, *tok2node = nullptr;
-    uint4 *ent = nullptr;
-    double *UT = nullptr;
-    float *syn_pos = nullptr, *syn_neg = nullptr, *pos0 = nullptr, *delta = nullptr;
-    uint32_t *seq_state = nullptr;
+    DeviceBuffer<double> w, U;
+    DeviceBuffer<int32_t> K, scratch, order, walks;
+    DeviceBuffer<unsigned long long> first_pos, cnt, pairs;
+    DeviceBuffer<int32_t> KT, tok2node;
+    DeviceBuffer<uint4> ent;
+    DeviceBuffer<double> UT;
+    DeviceBuffer<float> syn_pos, syn_neg, pos0, delta;
+    DeviceBuffer<uint32_t> seq_state;
     bool second_order = false;
-    long long *off2 = nullptr;       // nnz + 1: table offset of every CSR edge
-    int32_t *K2 = nullptr;
-    double *U2 = nullptr;
+    DeviceBuffer<long long> off2;    // nnz + 1: table offset of every CSR edge
+    DeviceBuffer<int32_t> K2;
+    DeviceBuffer<double> U2;
     long long table_entries = 0;
-    ~N2VDev() {
-        dfree(off2); dfree(K2); dfree(U2);
-        dfree(w); dfree(U); dfree(K); dfree(scratch); dfree(order); dfree(walks);
-        dfree(first_pos); dfree(cnt); dfree(pairs); dfree(KT); dfree(tok2node); dfree(UT); dfree(ent);
-        dfree(syn_pos); dfree(syn_neg); dfree(pos0); dfree(delta); dfree(seq_state);
-    }
 };
 
 static int check_graph_for_n2v(gemb_graph *g) {
@@ -557,15 +551,16 @@ static int build_alias(gemb_graph *g, const double *weights64, N2VDev &D, double
     if (p != 1.0 || q != 1.0) return build_alias2(g, weights64, p, q, D);
     gemb_ctx *c = g->ctx;
     const int64_t nnz = g->A.nnz;
-    GEMB_CUDA(dmalloc(&D.K, sizeof(int32_t) * std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(dmalloc(&D.U, sizeof(double) * std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(dmalloc(&D.scratch, sizeof(int32_t) * std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(D.K.alloc(std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(D.U.alloc(std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(D.scratch.alloc(std::max<int64_t>(nnz, 1)));
     if (weights64 && nnz) {
-        GEMB_CUDA(dmalloc(&D.w, sizeof(double) * nnz));
-        GEMB_CUDA(cudaMemcpyAsync(D.w, weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(D.w.alloc(nnz));
+        GEMB_CUDA(cudaMemcpyAsync(D.w.get(), weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
     }
     const int64_t n = g->n;
-    alias_build_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->stream>>>(n, g->A.indptr, D.w, D.K, D.U, D.scratch);
+    alias_build_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->stream>>>(n, g->A.indptr, D.w.get(), D.K.get(), D.U.get(),
+                                                                            D.scratch.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     return GEMB_OK;
@@ -576,28 +571,29 @@ static int build_alias2(gemb_graph *g, const double *weights64, double p, double
     const int64_t nnz = g->A.nnz, n = g->n;
     D.second_order = true;
     if (weights64 && nnz) {
-        GEMB_CUDA(dmalloc(&D.w, sizeof(double) * nnz));
-        GEMB_CUDA(cudaMemcpyAsync(D.w, weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(D.w.alloc(nnz));
+        GEMB_CUDA(cudaMemcpyAsync(D.w.get(), weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
     }
-    GEMB_CUDA(dmalloc(&D.off2, sizeof(long long) * (nnz + 1)));
-    long long *deg = nullptr;
-    GEMB_CUDA(dmalloc(&deg, sizeof(long long) * (nnz + 1)));
-    GEMB_CUDA(cudaMemsetAsync(deg, 0, sizeof(long long) * (nnz + 1), c->stream));
-    if (nnz) {
-        edge_degree_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(nnz, g->A.indptr, g->A.indices, deg);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, deg, D.off2, nnz + 1, c->stream);
-    void *tmp = nullptr;
-    GEMB_CUDA(dmalloc(&tmp, tb ? tb : 4));
-    GEMB_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, deg, D.off2, nnz + 1, c->stream));
-    count_launch();
+    GEMB_CUDA(D.off2.alloc(nnz + 1));
     long long T = 0;
-    GEMB_CUDA(cudaMemcpyAsync(&T, D.off2 + nnz, sizeof T, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    dfree(deg); dfree(tmp);
+    {
+        DeviceBuffer<long long> deg;
+        GEMB_CUDA(deg.alloc(nnz + 1));
+        GEMB_CUDA(cudaMemsetAsync(deg.get(), 0, sizeof(long long) * (nnz + 1), c->stream));
+        if (nnz) {
+            edge_degree_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(nnz, g->A.indptr, g->A.indices, deg.get());
+            GEMB_CUDA(cudaGetLastError());
+            count_launch();
+        }
+        size_t tb = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, tb, deg.get(), D.off2.get(), nnz + 1, c->stream);
+        DeviceBuffer<char> tmp;
+        GEMB_CUDA(tmp.alloc(tb));
+        GEMB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.get(), tb, deg.get(), D.off2.get(), nnz + 1, c->stream));
+        count_launch();
+        GEMB_CUDA(cudaMemcpyAsync(&T, D.off2.get() + nnz, sizeof T, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    }
     D.table_entries = T;
     // the reference needs the same sum_(t->v) outdeg(v) entries in host hash maps; here they must fit in HBM
     size_t free_b = 0, total_b = 0;
@@ -608,18 +604,18 @@ static int build_alias2(gemb_graph *g, const double *weights64, double p, double
                   "outdeg(v)) and do not fit in the %.1f GB of free device memory", p, q, T, need / 1e9, (double)free_b / 1e9);
         return GEMB_ERR_NOMEM;
     }
-    GEMB_CUDA(dmalloc(&D.K2, sizeof(int32_t) * std::max<long long>(T, 1)));
-    GEMB_CUDA(dmalloc(&D.U2, sizeof(double) * std::max<long long>(T, 1)));
-    GEMB_CUDA(dmalloc(&D.scratch, sizeof(int32_t) * std::max<long long>(T, 1)));
+    GEMB_CUDA(D.K2.alloc(std::max<long long>(T, 1)));
+    GEMB_CUDA(D.U2.alloc(std::max<long long>(T, 1)));
+    GEMB_CUDA(D.scratch.alloc(std::max<long long>(T, 1)));
     if (nnz) {
-        alias2_build_kernel<<<(unsigned)((nnz + 127) / 128), 128, 0, c->stream>>>(n, nnz, g->A.indptr, g->A.indices, D.w, D.off2,
-                                                                                 p, q, D.K2, D.U2, D.scratch);
+        alias2_build_kernel<<<(unsigned)((nnz + 127) / 128), 128, 0, c->stream>>>(n, nnz, g->A.indptr, g->A.indices, D.w.get(),
+                                                                                 D.off2.get(), p, q, D.K2.get(), D.U2.get(),
+                                                                                 D.scratch.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
     }
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    dfree(D.scratch);
-    D.scratch = nullptr;
+    D.scratch.reset();
     return GEMB_OK;
 }
 
@@ -635,17 +631,19 @@ static int run_walks(gemb_graph *g, N2VDev &D, const int32_t *nids, int64_t N, i
     std::vector<int32_t> order((size_t)num_walks * N);
     shuffle_rounds(nids, N, num_walks, walk_len, seed, order.data());
     if (shuffle_ms) *shuffle_ms = ms_since(t0);
-    GEMB_CUDA(dmalloc(&D.order, sizeof(int32_t) * std::max<size_t>(order.size(), 1)));
-    GEMB_CUDA(cudaMemcpyAsync(D.order, order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(D.order.alloc(std::max<size_t>(order.size(), 1)));
+    GEMB_CUDA(cudaMemcpyAsync(D.order.get(), order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, c->stream));
     const int64_t cnt = w_end - w_begin;
-    GEMB_CUDA(dmalloc(&D.walks, sizeof(int32_t) * std::max<int64_t>(cnt * walk_len, 1)));
+    GEMB_CUDA(D.walks.alloc(std::max<int64_t>(cnt * walk_len, 1)));
     if (cnt > 0) {
         if (D.second_order)
-            walk2_kernel<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K2, D.U2, D.off2, D.order,
-                                                                              N, walk_len, seed, w_begin, w_end, D.walks);
+            walk2_kernel<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K2.get(), D.U2.get(),
+                                                                              D.off2.get(), D.order.get(), N, walk_len, seed,
+                                                                              w_begin, w_end, D.walks.get());
         else
-            walk_kernel<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K, D.U, D.order,
-                                                                             N, walk_len, seed, w_begin, w_end, D.walks);
+            walk_kernel<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K.get(), D.U.get(),
+                                                                             D.order.get(), N, walk_len, seed, w_begin, w_end,
+                                                                             D.walks.get());
         GEMB_CUDA(cudaGetLastError());
     count_launch();
     }
@@ -696,8 +694,8 @@ int gemb_n2v_alias(gemb_graph *g, const double *weights64, int32_t *K_out, doubl
     N2VDev D;
     GEMB_TRY(build_alias(g, weights64, D));
     const int64_t nnz = g->A.nnz;
-    GEMB_CUDA(cudaMemcpyAsync(K_out, D.K, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(U_out, D.U, sizeof(double) * nnz, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(K_out, D.K.get(), sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(U_out, D.U.get(), sizeof(double) * nnz, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     return GEMB_OK;
 }
@@ -721,22 +719,20 @@ int gemb_n2v_walks(gemb_graph *g, const double *weights64, const int32_t *nids, 
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     N2VDev D;
-    cudaEvent_t e0, e1, e2;
-    GEMB_CUDA(cudaEventCreate(&e0)); GEMB_CUDA(cudaEventCreate(&e1)); GEMB_CUDA(cudaEventCreate(&e2));
-    GEMB_CUDA(cudaEventRecord(e0, c->stream));
+    CallEvents<3> ev;
+    GEMB_CUDA(ev.create());
+    GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
     GEMB_TRY(build_alias(g, weights64, D, p, q));
-    GEMB_CUDA(cudaEventRecord(e1, c->stream));
+    GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
     double sh_ms = 0;
     GEMB_TRY(run_walks(g, D, nids, N, walk_len, num_walks, (uint32_t)seed, w_begin, w_end, &sh_ms));
-    GEMB_CUDA(cudaEventRecord(e2, c->stream));
+    GEMB_CUDA(cudaEventRecord(ev[2], c->stream));
     if (walks_out && w_end > w_begin)
-        GEMB_CUDA(cudaMemcpyAsync(walks_out, D.walks, sizeof(int32_t) * (size_t)(w_end - w_begin) * walk_len,
+        GEMB_CUDA(cudaMemcpyAsync(walks_out, D.walks.get(), sizeof(int32_t) * (size_t)(w_end - w_begin) * walk_len,
                                   cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     if (stats) {
-        float a = 0, b = 0;
-        cudaEventElapsedTime(&a, e0, e1);
-        cudaEventElapsedTime(&b, e1, e2);
+        const float a = ev.ms(0, 1), b = ev.ms(1, 2);
         memset((char *)stats + sizeof(uint32_t), 0, sizeof(*stats) - sizeof(uint32_t));
         stats->alias_ms = a;
         stats->shuffle_ms = sh_ms;
@@ -744,7 +740,6 @@ int gemb_n2v_walks(gemb_graph *g, const double *weights64, const int32_t *nids, 
         stats->n_walks = w_end - w_begin;
         stats->walk_bytes = 24.0 * (double)(w_end - w_begin) * (double)std::max(walk_len - 1, 0);
     }
-    cudaEventDestroy(e0); cudaEventDestroy(e1); cudaEventDestroy(e2);
     return GEMB_OK;
 }
 
@@ -761,8 +756,8 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     GEMB_CUDA(cudaSetDevice(c->device));
     GEMB_ARG(!(sequential && c->nranks > 1), "sequential parity mode is single-GPU");
     N2VDev D;
-    cudaEvent_t ev[6];
-    for (auto &e : ev) GEMB_CUDA(cudaEventCreate(&e));
+    CallEvents<6> ev;
+    GEMB_CUDA(ev.create());
     GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
     GEMB_TRY(build_alias(g, weights64, D, p, q));
     GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
@@ -776,30 +771,31 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     double sh_ms = 0;
     GEMB_TRY(run_walks(g, D, nids, N, walk_len, num_walks, (uint32_t)seed, w_begin, w_end, &sh_ms));
     GEMB_CUDA(cudaEventRecord(ev[2], c->stream));
-    if (D.second_order) { dfree(D.K2); dfree(D.U2); dfree(D.off2); D.K2 = nullptr; D.U2 = nullptr; D.off2 = nullptr; }   // tables are walk-only
+    if (D.second_order) { D.K2.reset(); D.U2.reset(); D.off2.reset(); }   // tables are walk-only
 
     // ---- vocabulary: first appearance + counts (all ranks combined), host renumbering + Vose
     auto tv0 = std::chrono::steady_clock::now();
     const int64_t n_ids = g->n;
-    GEMB_CUDA(dmalloc(&D.first_pos, sizeof(unsigned long long) * n_ids));
-    GEMB_CUDA(dmalloc(&D.cnt, sizeof(unsigned long long) * n_ids));
-    GEMB_CUDA(cudaMemsetAsync(D.first_pos, 0xff, sizeof(unsigned long long) * n_ids, c->stream));
-    GEMB_CUDA(cudaMemsetAsync(D.cnt, 0, sizeof(unsigned long long) * n_ids, c->stream));
+    GEMB_CUDA(D.first_pos.alloc(n_ids));
+    GEMB_CUDA(D.cnt.alloc(n_ids));
+    GEMB_CUDA(cudaMemsetAsync(D.first_pos.get(), 0xff, sizeof(unsigned long long) * n_ids, c->stream));
+    GEMB_CUDA(cudaMemsetAsync(D.cnt.get(), 0, sizeof(unsigned long long) * n_ids, c->stream));
     if (n_local > 0) {
-        vocab_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(D.walks, n_local * walk_len, w_begin * walk_len, D.first_pos, D.cnt);
+        vocab_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(D.walks.get(), n_local * walk_len, w_begin * walk_len,
+                                                             D.first_pos.get(), D.cnt.get());
         GEMB_CUDA(cudaGetLastError());
     count_launch();
     }
     if (c->nranks > 1) {
         NcclApi *api = nccl_api();
         if (!api) return GEMB_ERR_NCCL;
-        ncclResult_t r = api->AllReduce(D.first_pos, D.first_pos, n_ids, ncclUint64, ncclMin, (ncclComm_t)c->comm, c->stream);
-        if (r == ncclSuccess) r = api->AllReduce(D.cnt, D.cnt, n_ids, ncclUint64, ncclSum, (ncclComm_t)c->comm, c->stream);
+        ncclResult_t r = api->AllReduce(D.first_pos.get(), D.first_pos.get(), n_ids, ncclUint64, ncclMin, (ncclComm_t)c->comm, c->stream);
+        if (r == ncclSuccess) r = api->AllReduce(D.cnt.get(), D.cnt.get(), n_ids, ncclUint64, ncclSum, (ncclComm_t)c->comm, c->stream);
         if (r != ncclSuccess) { set_error("nccl vocab allreduce: %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
     }
     std::vector<unsigned long long> h_first(n_ids), h_cnt(n_ids);
-    GEMB_CUDA(cudaMemcpyAsync(h_first.data(), D.first_pos, sizeof(unsigned long long) * n_ids, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(h_cnt.data(), D.cnt, sizeof(unsigned long long) * n_ids, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(h_first.data(), D.first_pos.get(), sizeof(unsigned long long) * n_ids, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(h_cnt.data(), D.cnt.get(), sizeof(unsigned long long) * n_ids, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     std::vector<int32_t> tok2node;
     tok2node.reserve(n_ids);
@@ -824,46 +820,47 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
         while (t < 2147483647LL && (double)t / 2147483647.0 < u) t++;
         ent[i] = make_uint4((uint32_t)t, (uint32_t)tok2node[i], (uint32_t)tok2node[KT[i]], 0u);
     }
-    GEMB_CUDA(dmalloc(&D.ent, sizeof(uint4) * V));
-    GEMB_CUDA(cudaMemcpyAsync(D.ent, ent.data(), sizeof(uint4) * V, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(dmalloc(&D.KT, sizeof(int32_t) * V));
-    GEMB_CUDA(dmalloc(&D.UT, sizeof(double) * V));
-    GEMB_CUDA(dmalloc(&D.tok2node, sizeof(int32_t) * V));
-    GEMB_CUDA(cudaMemcpyAsync(D.KT, KT.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(D.UT, UT.data(), sizeof(double) * V, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(D.tok2node, tok2node.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(D.ent.alloc(V));
+    GEMB_CUDA(cudaMemcpyAsync(D.ent.get(), ent.data(), sizeof(uint4) * V, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(D.KT.alloc(V));
+    GEMB_CUDA(D.UT.alloc(V));
+    GEMB_CUDA(D.tok2node.alloc(V));
+    GEMB_CUDA(cudaMemcpyAsync(D.KT.get(), KT.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(D.UT.get(), UT.data(), sizeof(double) * V, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(D.tok2node.get(), tok2node.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     const double vocab_ms = ms_since(tv0);
     GEMB_CUDA(cudaEventRecord(ev[3], c->stream));
 
     // ---- embeddings
     const size_t tab = (size_t)n_rows * d;
-    GEMB_CUDA(dmalloc(&D.syn_pos, sizeof(float) * tab));
-    GEMB_CUDA(dmalloc(&D.syn_neg, sizeof(float) * tab));
-    GEMB_CUDA(cudaMemsetAsync(D.syn_pos, 0, sizeof(float) * tab, c->stream));
-    GEMB_CUDA(cudaMemsetAsync(D.syn_neg, 0, sizeof(float) * tab, c->stream));
-    init_pos_kernel<<<(unsigned)((V + 127) / 128), 128, 0, c->stream>>>(V, d, (uint32_t)seed, D.tok2node, D.syn_pos);
+    GEMB_CUDA(D.syn_pos.alloc(tab));
+    GEMB_CUDA(D.syn_neg.alloc(tab));
+    GEMB_CUDA(cudaMemsetAsync(D.syn_pos.get(), 0, sizeof(float) * tab, c->stream));
+    GEMB_CUDA(cudaMemsetAsync(D.syn_neg.get(), 0, sizeof(float) * tab, c->stream));
+    init_pos_kernel<<<(unsigned)((V + 127) / 128), 128, 0, c->stream>>>(V, d, (uint32_t)seed, D.tok2node.get(), D.syn_pos.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    GEMB_CUDA(dmalloc(&D.pairs, sizeof(unsigned long long)));
-    GEMB_CUDA(cudaMemsetAsync(D.pairs, 0, sizeof(unsigned long long), c->stream));
-    GEMB_CUDA(dmalloc(&D.seq_state, sizeof(uint32_t)));
+    GEMB_CUDA(D.pairs.alloc(1));
+    GEMB_CUDA(cudaMemsetAsync(D.pairs.get(), 0, sizeof(unsigned long long), c->stream));
+    GEMB_CUDA(D.seq_state.alloc(1));
     {
         const uint32_t st0 = lcg_skip((uint32_t)seed, (uint64_t)V * (uint64_t)d);  // after InitPosEmb's V*d draws
-        GEMB_CUDA(cudaMemcpyAsync(D.seq_state, &st0, sizeof st0, cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(D.seq_state.get(), &st0, sizeof st0, cudaMemcpyHostToDevice, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
     }
     if (c->nranks > 1) {
-        GEMB_CUDA(dmalloc(&D.pos0, sizeof(float) * tab));
-        GEMB_CUDA(dmalloc(&D.delta, sizeof(float) * tab));
+        GEMB_CUDA(D.pos0.alloc(tab));
+        GEMB_CUDA(D.delta.alloc(tab));
     }
 
     SgnsParams P;
-    P.walks = D.walks; P.n_walks_local = n_local; P.walk_offset = w_begin; P.n_walks_total = total_walks;
+    P.walks = D.walks.get(); P.n_walks_local = n_local; P.walk_offset = w_begin; P.n_walks_total = total_walks;
     P.walk_len = walk_len; P.d = d; P.win = con_size; P.iters = max_iter; P.epoch = 0;
-    P.syn_pos = D.syn_pos; P.syn_neg = D.syn_neg; P.KT = D.KT; P.UT = D.UT; P.tok2node = D.tok2node; P.ent = D.ent; P.V = V;
+    P.syn_pos = D.syn_pos.get(); P.syn_neg = D.syn_neg.get(); P.KT = D.KT.get(); P.UT = D.UT.get();
+    P.tok2node = D.tok2node.get(); P.ent = D.ent.get(); P.V = V;
     P.seed = (uint32_t)seed; P.seq_start = (uint64_t)V * d; P.sequential = sequential ? 1 : 0;
-    P.seq_state = D.seq_state; P.pair_counter = D.pairs;
+    P.seq_state = D.seq_state.get(); P.pair_counter = D.pairs.get();
     const int threads = 128;
     // Hogwild: concurrent walks race on embedding rows exactly as SNAP's OpenMP threads do.  Keep the
     // number of in-flight walks far below the vocabulary size so that lost updates stay as rare as in
@@ -875,12 +872,13 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     }
     const int threads_used = sequential ? 32 : threads;
     double comm_ms = 0;
+    float *syn_pos = D.syn_pos.get(), *syn_neg = D.syn_neg.get(), *pos0 = D.pos0.get(), *delta = D.delta.get();
     for (int it = 0; it < max_iter; it++) {
         P.epoch = it;
         const int64_t tabn = (int64_t)tab;
         if (c->nranks > 1) {
-            GEMB_CUDA(cudaMemcpyAsync(D.pos0, D.syn_pos, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
-            GEMB_CUDA(cudaMemcpyAsync(D.delta, D.syn_neg, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
+            GEMB_CUDA(cudaMemcpyAsync(pos0, syn_pos, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
+            GEMB_CUDA(cudaMemcpyAsync(delta, syn_neg, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
         }
         if (n_local > 0) GEMB_TRY(dispatch_sgns(c, P, blocks, threads_used));
         if (c->nranks > 1) {
@@ -890,12 +888,12 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
             GEMB_TRY(c->t_comm.begin(c->stream));
             const int gs = c->sm_count * 8;
             // syn_neg: delta held the pre-epoch copy
-            sub_kernel<<<gs, 256, 0, c->stream>>>(tabn, D.syn_neg, D.delta, D.syn_neg);       // syn_neg := d_neg
-            ncclResult_t r = api->AllReduce(D.syn_neg, D.syn_neg, tab, ncclFloat, ncclSum, (ncclComm_t)c->comm, c->stream);
-            axpy1_kernel<<<gs, 256, 0, c->stream>>>(tabn, D.delta, D.syn_neg, 1.f);           // + neg0
-            sub_kernel<<<gs, 256, 0, c->stream>>>(tabn, D.syn_pos, D.pos0, D.syn_pos);        // syn_pos := d_pos
-            if (r == ncclSuccess) r = api->AllReduce(D.syn_pos, D.syn_pos, tab, ncclFloat, ncclSum, (ncclComm_t)c->comm, c->stream);
-            axpy1_kernel<<<gs, 256, 0, c->stream>>>(tabn, D.pos0, D.syn_pos, 1.f);            // + pos0
+            sub_kernel<<<gs, 256, 0, c->stream>>>(tabn, syn_neg, delta, syn_neg);       // syn_neg := d_neg
+            ncclResult_t r = api->AllReduce(syn_neg, syn_neg, tab, ncclFloat, ncclSum, (ncclComm_t)c->comm, c->stream);
+            axpy1_kernel<<<gs, 256, 0, c->stream>>>(tabn, delta, syn_neg, 1.f);         // + neg0
+            sub_kernel<<<gs, 256, 0, c->stream>>>(tabn, syn_pos, pos0, syn_pos);        // syn_pos := d_pos
+            if (r == ncclSuccess) r = api->AllReduce(syn_pos, syn_pos, tab, ncclFloat, ncclSum, (ncclComm_t)c->comm, c->stream);
+            axpy1_kernel<<<gs, 256, 0, c->stream>>>(tabn, pos0, syn_pos, 1.f);          // + pos0
             if (r != ncclSuccess) { set_error("nccl embedding allreduce: %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
             GEMB_CUDA(cudaGetLastError());
     count_launch();
@@ -903,25 +901,21 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
         }
     }
     GEMB_CUDA(cudaEventRecord(ev[4], c->stream));
-    if (X_out) GEMB_CUDA(cudaMemcpyAsync(X_out, D.syn_pos, sizeof(float) * tab, cudaMemcpyDeviceToHost, c->stream));
+    if (X_out) GEMB_CUDA(cudaMemcpyAsync(X_out, syn_pos, sizeof(float) * tab, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaEventRecord(ev[5], c->stream));
     unsigned long long h_pairs = 0;
-    GEMB_CUDA(cudaMemcpyAsync(&h_pairs, D.pairs, sizeof h_pairs, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(&h_pairs, D.pairs.get(), sizeof h_pairs, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     if (c->nranks > 1) { comm_ms = c->t_comm.total_ms(); c->t_comm.reset(); }
     if (stats) {
-        float t01, t12, t23, t34, t45, t05;
-        cudaEventElapsedTime(&t01, ev[0], ev[1]); cudaEventElapsedTime(&t12, ev[1], ev[2]);
-        cudaEventElapsedTime(&t23, ev[2], ev[3]); cudaEventElapsedTime(&t34, ev[3], ev[4]);
-        cudaEventElapsedTime(&t45, ev[4], ev[5]); cudaEventElapsedTime(&t05, ev[0], ev[4]);
         memset((char *)stats + sizeof(uint32_t), 0, sizeof(*stats) - sizeof(uint32_t));
-        stats->alias_ms = t01;
+        stats->alias_ms = ev.ms(0, 1);
         stats->shuffle_ms = sh_ms;
-        stats->walk_ms = std::max(0.0, (double)t12 - sh_ms);
+        stats->walk_ms = std::max(0.0, (double)ev.ms(1, 2) - sh_ms);
         stats->vocab_ms = vocab_ms;
-        stats->sgns_ms = t34;
-        stats->total_ms = t05;
-        stats->d2h_ms = t45;
+        stats->sgns_ms = ev.ms(3, 4);
+        stats->total_ms = ev.ms(0, 4);
+        stats->d2h_ms = ev.ms(4, 5);
         stats->comm_ms = comm_ms;
         stats->n_tokens = V;
         stats->n_walks = n_local;
@@ -929,7 +923,6 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
         stats->sgns_bytes = (double)h_pairs * 14.0 * 4.0 * (double)d;
         stats->walk_bytes = 24.0 * (double)n_local * (double)std::max(walk_len - 1, 0);
     }
-    for (auto &e : ev) cudaEventDestroy(e);
     return GEMB_OK;
 }
 

@@ -246,41 +246,34 @@ int gemb_recon_create(gemb_ctx *c, const float *X, int64_t n, int d, int split, 
                   (long long)n, (long long)n, need / 1e9, (double)free_b / 1e9);
         return GEMB_ERR_NOMEM;
     }
-    gemb_recon *r = new gemb_recon();
-    r->ctx = c; r->n = n; r->n_pad = n_pad; r->k = k;
-    float *dX = nullptr, *L = nullptr, *Rt = nullptr;
-    int s = GEMB_OK;
-    auto fail = [&](int code) { dfree(dX); if (L != dX) dfree(L); dfree(Rt); dfree(r->adj); delete r; return code; };
-#define RC(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { set_error("%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(_e)); (void)cudaGetLastError(); return fail(GEMB_ERR_CUDA); } } while (0)
-    RC(dmalloc(&dX, sizeof(float) * (size_t)n * d));
-    RC(dmalloc(&Rt, sizeof(float) * (size_t)n_pad * k));
-    RC(dmalloc(&r->adj, sizeof(float) * (size_t)n * n_pad));
-    RC(cudaMemcpyAsync(dX, X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
+    DeviceBuffer<float> dX, L, Rt, adj;
+    GEMB_CUDA(dX.alloc((size_t)n * d));
+    GEMB_CUDA(Rt.alloc((size_t)n_pad * k));
+    GEMB_CUDA(adj.alloc((size_t)n * n_pad));
+    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
+    const float *Lp = dX.get();
     if (split) {
-        RC(dmalloc(&L, sizeof(float) * (size_t)n * k));
-        recon_left_kernel<<<grid_for(c, n * k, 256), 256, 0, c->stream>>>(n, d, k, dX, L);
-        RC(cudaGetLastError());
+        GEMB_CUDA(L.alloc((size_t)n * k));
+        recon_left_kernel<<<grid_for(c, n * k, 256), 256, 0, c->stream>>>(n, d, k, dX.get(), L.get());
+        GEMB_CUDA(cudaGetLastError());
         count_launch();
-    } else {
-        L = dX;
+        Lp = L.get();
     }
     {
         dim3 grid((unsigned)((n_pad + 31) / 32), (unsigned)((k + 31) / 32)), block(32, 8);
-        recon_right_t_kernel<<<grid, block, 0, c->stream>>>(n, n_pad, d, k, split ? k : 0, dX, Rt);
-        RC(cudaGetLastError());
+        recon_right_t_kernel<<<grid, block, 0, c->stream>>>(n, n_pad, d, k, split ? k : 0, dX.get(), Rt.get());
+        GEMB_CUDA(cudaGetLastError());
         count_launch();
     }
-    for (int64_t p = 0; p < n_pad / PW && s == GEMB_OK; p++)
-        s = apply_launch(c, n, L, k, Rt + p * PW, (int)n_pad, PW, r->adj + (size_t)p * n * PW, PW);
-    if (s != GEMB_OK) return fail(s);
-    recon_zero_diag_kernel<<<grid_for(c, n, 256), 256, 0, c->stream>>>(n, r->adj);
-    RC(cudaGetLastError());
+    for (int64_t p = 0; p < n_pad / PW; p++)
+        GEMB_TRY(apply_launch(c, n, Lp, k, Rt.get() + p * PW, (int)n_pad, PW, adj.get() + (size_t)p * n * PW, PW));
+    recon_zero_diag_kernel<<<grid_for(c, n, 256), 256, 0, c->stream>>>(n, adj.get());
+    GEMB_CUDA(cudaGetLastError());
     count_launch();
-    RC(cudaStreamSynchronize(c->stream));
-#undef RC
-    dfree(dX);
-    if (L != dX) dfree(L);
-    dfree(Rt);
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    gemb_recon *r = new gemb_recon();
+    r->ctx = c; r->n = n; r->n_pad = n_pad; r->k = k;
+    r->adj = adj.release();
     *out = r;
     return GEMB_OK;
 }
@@ -299,18 +292,16 @@ int gemb_recon_dense(gemb_recon *r, float *adj_out) {
     GEMB_CUDA(cudaSetDevice(c->device));
     const int64_t n = r->n;
     int64_t rows = std::max<int64_t>(1, std::min<int64_t>(n, ((int64_t)256 << 20) / (4 * n)));   // <= 256 MB chunks
-    float *buf = nullptr;
-    GEMB_CUDA(dmalloc(&buf, sizeof(float) * (size_t)rows * n));
+    DeviceBuffer<float> buf;
+    GEMB_CUDA(buf.alloc((size_t)rows * n));
     for (int64_t r0 = 0; r0 < n; r0 += rows) {
         const int64_t nr = std::min(rows, n - r0);
-        recon_rowmajor_kernel<<<grid_for(c, nr * n, 256), 256, 0, c->stream>>>(n, r0, nr, r->adj, buf);
-        cudaError_t e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaMemcpyAsync(adj_out + (size_t)r0 * n, buf, sizeof(float) * (size_t)nr * n, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        recon_rowmajor_kernel<<<grid_for(c, nr * n, 256), 256, 0, c->stream>>>(n, r0, nr, r->adj, buf.get());
+        GEMB_CUDA(cudaGetLastError());
         count_launch();
-        if (e != cudaSuccess) { set_error("gemb_recon_dense: %s", cudaGetErrorString(e)); dfree(buf); return GEMB_ERR_CUDA; }
+        GEMB_CUDA(cudaMemcpyAsync(adj_out + (size_t)r0 * n, buf.get(), sizeof(float) * (size_t)nr * n, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaStreamSynchronize(c->stream));
     }
-    dfree(buf);
     return GEMB_OK;
 }
 
@@ -321,24 +312,19 @@ int gemb_recon_pairs(gemb_recon *r, const int32_t *pi, const int32_t *pj, int64_
     GEMB_CUDA(cudaSetDevice(c->device));
     for (int64_t t = 0; t < m; t++)
         GEMB_ARG(pi[t] >= 0 && pi[t] < r->n && pj[t] >= 0 && pj[t] < r->n, "pair index out of range");
-    int32_t *di = nullptr, *dj = nullptr;
-    float *dout = nullptr;
-    int s = GEMB_OK;
-    cudaError_t e = dmalloc(&di, sizeof(int32_t) * (size_t)m);
-    if (e == cudaSuccess) e = dmalloc(&dj, sizeof(int32_t) * (size_t)m);
-    if (e == cudaSuccess) e = dmalloc(&dout, sizeof(float) * (size_t)m);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(di, pi, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dj, pj, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        recon_pairs_kernel<<<grid_for(c, m, 256), 256, 0, c->stream>>>(r->n, m, di, dj, r->adj, dout);
-        e = cudaGetLastError();
-        count_launch();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, dout, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("gemb_recon_pairs: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); s = GEMB_ERR_CUDA; }
-    dfree(di); dfree(dj); dfree(dout);
-    return s;
+    DeviceBuffer<int32_t> di, dj;
+    DeviceBuffer<float> dout;
+    GEMB_CUDA(di.alloc((size_t)m));
+    GEMB_CUDA(dj.alloc((size_t)m));
+    GEMB_CUDA(dout.alloc((size_t)m));
+    GEMB_CUDA(cudaMemcpyAsync(di.get(), pi, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(dj.get(), pj, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->stream));
+    recon_pairs_kernel<<<grid_for(c, m, 256), 256, 0, c->stream>>>(r->n, m, di.get(), dj.get(), r->adj, dout.get());
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    GEMB_CUDA(cudaMemcpyAsync(out, dout.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }
 
 int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indices, int is_undirected,
@@ -350,25 +336,21 @@ int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indice
     const int64_t nnz = indptr[n];
     GEMB_ARG(indptr[0] == 0 && nnz >= 0 && (nnz == 0 || (indices && rank_out)), "CSR");
     for (int64_t t = 0; t < nnz; t++) GEMB_ARG(indices[t] >= 0 && indices[t] < n, "column id out of range");
-    int32_t *dp = nullptr, *dix = nullptr, *drank = nullptr, *dnp = nullptr;
-    int s = GEMB_OK;
-    cudaError_t e = dmalloc(&dp, sizeof(int32_t) * (size_t)(n + 1));
-    if (e == cudaSuccess) e = dmalloc(&dix, sizeof(int32_t) * (size_t)std::max<int64_t>(nnz, 1));
-    if (e == cudaSuccess) e = dmalloc(&drank, sizeof(int32_t) * (size_t)std::max<int64_t>(nnz, 1));
-    if (e == cudaSuccess) e = dmalloc(&dnp, sizeof(int32_t) * (size_t)n);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dp, indptr, sizeof(int32_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess && nnz) e = cudaMemcpyAsync(dix, indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        recon_rank_kernel<<<grid_for(c, n * 32, 256), 256, 0, c->stream>>>(n, dp, dix, is_undirected ? 1 : 0, r->adj, drank, dnp);
-        e = cudaGetLastError();
-        count_launch();
-    }
-    if (e == cudaSuccess && nnz) e = cudaMemcpyAsync(rank_out, drank, sizeof(int32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(n_pred_row, dnp, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("gemb_recon_ranks: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); s = GEMB_ERR_CUDA; }
-    dfree(dp); dfree(dix); dfree(drank); dfree(dnp);
-    return s;
+    DeviceBuffer<int32_t> dp, dix, drank, dnp;
+    GEMB_CUDA(dp.alloc((size_t)(n + 1)));
+    GEMB_CUDA(dix.alloc((size_t)std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(drank.alloc((size_t)std::max<int64_t>(nnz, 1)));
+    GEMB_CUDA(dnp.alloc((size_t)n));
+    GEMB_CUDA(cudaMemcpyAsync(dp.get(), indptr, sizeof(int32_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, c->stream));
+    if (nnz) GEMB_CUDA(cudaMemcpyAsync(dix.get(), indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, c->stream));
+    recon_rank_kernel<<<grid_for(c, n * 32, 256), 256, 0, c->stream>>>(n, dp.get(), dix.get(), is_undirected ? 1 : 0, r->adj,
+                                                                       drank.get(), dnp.get());
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    if (nnz) GEMB_CUDA(cudaMemcpyAsync(rank_out, drank.get(), sizeof(int32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(n_pred_row, dnp.get(), sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }
 
 int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap, int32_t *i_out, int32_t *j_out,
@@ -378,60 +360,50 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
     gemb_ctx *c = r->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     const int und = is_undirected ? 1 : 0;
-    unsigned long long *dcounter = nullptr;
-    GEMB_CUDA(dmalloc(&dcounter, sizeof(unsigned long long)));
-    int s = GEMB_OK;
+    DeviceBuffer<unsigned long long> dcounter;
+    GEMB_CUDA(dcounter.alloc(1));
     if (!(r->top_valid && r->top_und == und && r->top_k == max_k)) {
         int64_t total = 0;
-        s = count_ge(r, und, 1u, dcounter, &total);
+        GEMB_TRY(count_ge(r, und, 1u, dcounter.get(), &total));
         uint32_t bits = 1u;
         int64_t count = total;
-        if (s == GEMB_OK && max_k >= 0 && total > max_k) {
+        if (max_k >= 0 && total > max_k) {
             // largest bit pattern T with count(>= T) >= max_k:  count(>= lo) >= K  and  count(>= hi) < K
             uint32_t lo = 1u, hi = 0x7f800001u;
-            while (s == GEMB_OK && hi - lo > 1u) {
+            while (hi - lo > 1u) {
                 const uint32_t mid = lo + (hi - lo) / 2u;
                 int64_t cm = 0;
-                s = count_ge(r, und, mid, dcounter, &cm);
+                GEMB_TRY(count_ge(r, und, mid, dcounter.get(), &cm));
                 if (cm >= std::max<int64_t>(max_k, 1)) { lo = mid; count = cm; } else { hi = mid; }
             }
             bits = lo;
             if (max_k == 0) count = 0;
         }
-        if (s == GEMB_OK) { r->top_valid = 1; r->top_und = und; r->top_k = max_k; r->top_bits = bits; r->top_count = count; }
+        r->top_valid = 1; r->top_und = und; r->top_k = max_k; r->top_bits = bits; r->top_count = count;
     }
-    if (s == GEMB_OK) {
-        *m_out = r->top_count;
-        if (cap > 0 && r->top_count > 0) {
-            if (cap < r->top_count) {
-                set_error("gemb_recon_top: %lld entries reach the threshold, cap is %lld", (long long)r->top_count, (long long)cap);
-                s = GEMB_ERR_ARG;
-            } else {
-                const int64_t m = r->top_count;
-                int32_t *di = nullptr, *dj = nullptr;
-                float *dw = nullptr;
-                cudaError_t e = dmalloc(&di, sizeof(int32_t) * (size_t)m);
-                if (e == cudaSuccess) e = dmalloc(&dj, sizeof(int32_t) * (size_t)m);
-                if (e == cudaSuccess) e = dmalloc(&dw, sizeof(float) * (size_t)m);
-                if (e == cudaSuccess) e = cudaMemsetAsync(dcounter, 0, sizeof(unsigned long long), c->stream);
-                if (e == cudaSuccess) {
-                    const int64_t n_panels = r->n_pad / PW;
-                    recon_select_kernel<true><<<grid_for(c, n_panels * r->n * 32, 256), 256, 0, c->stream>>>(
-                        r->n, n_panels, und, r->top_bits, r->adj, dcounter, m, di, dj, dw);
-                    e = cudaGetLastError();
-                    count_launch();
-                }
-                if (e == cudaSuccess) e = cudaMemcpyAsync(i_out, di, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream);
-                if (e == cudaSuccess) e = cudaMemcpyAsync(j_out, dj, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream);
-                if (e == cudaSuccess) e = cudaMemcpyAsync(w_out, dw, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream);
-                if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-                if (e != cudaSuccess) { set_error("gemb_recon_top: %s", cudaGetErrorString(e)); (void)cudaGetLastError(); s = GEMB_ERR_CUDA; }
-                dfree(di); dfree(dj); dfree(dw);
-            }
-        }
+    *m_out = r->top_count;
+    if (cap <= 0 || r->top_count <= 0) return GEMB_OK;
+    if (cap < r->top_count) {
+        set_error("gemb_recon_top: %lld entries reach the threshold, cap is %lld", (long long)r->top_count, (long long)cap);
+        return GEMB_ERR_ARG;
     }
-    dfree(dcounter);
-    return s;
+    const int64_t m = r->top_count;
+    DeviceBuffer<int32_t> di, dj;
+    DeviceBuffer<float> dw;
+    GEMB_CUDA(di.alloc((size_t)m));
+    GEMB_CUDA(dj.alloc((size_t)m));
+    GEMB_CUDA(dw.alloc((size_t)m));
+    GEMB_CUDA(cudaMemsetAsync(dcounter.get(), 0, sizeof(unsigned long long), c->stream));
+    const int64_t n_panels = r->n_pad / PW;
+    recon_select_kernel<true><<<grid_for(c, n_panels * r->n * 32, 256), 256, 0, c->stream>>>(
+        r->n, n_panels, und, r->top_bits, r->adj, dcounter.get(), m, di.get(), dj.get(), dw.get());
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    GEMB_CUDA(cudaMemcpyAsync(i_out, di.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(j_out, dj.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(w_out, dw.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }
 
 }  // extern "C"

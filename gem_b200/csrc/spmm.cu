@@ -296,27 +296,18 @@ extern "C" int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const
     GEMB_ARG(b > 0 && b % 4 == 0, "b must be a positive multiple of 4");
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
-    float *dX = nullptr, *dXs = nullptr, *dX0 = nullptr, *dY = nullptr;
-    const size_t full = sizeof(float) * (size_t)g->n * b, shard = sizeof(float) * (size_t)g->n_local * b;
-    GEMB_CUDA(dmalloc(&dX, full ? full : 4));
-    GEMB_CUDA(dmalloc(&dY, shard ? shard : 4));
-    if (Xself) GEMB_CUDA(dmalloc(&dXs, shard ? shard : 4));
-    if (X0) GEMB_CUDA(dmalloc(&dX0, shard ? shard : 4));
-    GEMB_CUDA(cudaMemcpyAsync(dX, X, full, cudaMemcpyHostToDevice, c->stream));
-    if (Xself) GEMB_CUDA(cudaMemcpyAsync(dXs, Xself, shard, cudaMemcpyHostToDevice, c->stream));
-    if (X0) GEMB_CUDA(cudaMemcpyAsync(dX0, X0, shard, cudaMemcpyHostToDevice, c->stream));
-    int s = spmm3_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX, gamma, dXs, delta, dX0, dY);
-    if (s == GEMB_OK) {
-        cudaError_t e = cudaMemcpyAsync(Y, dY, shard, cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) {
-            set_error("gemb_spmm: %s", cudaGetErrorString(e));
-            s = GEMB_ERR_CUDA;
-        }
-    }
-    dfree(dX);
-    dfree(dY);
-    dfree(dXs);
-    dfree(dX0);
-    return s;
+    DeviceBuffer<float> dX, dY, dXs, dX0;
+    const size_t full = (size_t)g->n * b, shard = (size_t)g->n_local * b;
+    GEMB_CUDA(dX.alloc(full));
+    GEMB_CUDA(dY.alloc(shard));
+    if (Xself) GEMB_CUDA(dXs.alloc(shard));
+    if (X0) GEMB_CUDA(dX0.alloc(shard));
+    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * full, cudaMemcpyHostToDevice, c->stream));
+    if (Xself) GEMB_CUDA(cudaMemcpyAsync(dXs.get(), Xself, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
+    if (X0) GEMB_CUDA(cudaMemcpyAsync(dX0.get(), X0, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
+    GEMB_TRY(spmm3_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX.get(), gamma, dXs.get(), delta, dX0.get(),
+                          dY.get()));
+    GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * shard, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
 }

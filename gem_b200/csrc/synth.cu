@@ -74,6 +74,76 @@ __global__ void rmat_cols_kernel(int64_t cnt, const uint64_t *__restrict__ keys,
         cols[i] = (int32_t)(uint32_t)keys[i];
 }
 
+// gemb_synth_rmat without the argument checks and the final trim: its scratch is released when it returns
+static int rmat_generate(gemb_ctx *ctx, int scale, int edge_factor, double a, double b, double c, uint64_t seed, int permute,
+                         int64_t row0, int64_t n_rows, int64_t *nnz_out, int64_t *nnz_total_out, int64_t *indptr_out,
+                         int32_t *indices_out, int64_t cap) {
+    const int64_t n = (int64_t)1 << scale, m = n * edge_factor, nk = 2 * m;
+    cudaStream_t st = ctx->stream;
+    const int grid = ctx->sm_count * 8;
+    DeviceBuffer<uint64_t> pk, pk2, keys, keys2;
+    DeviceBuffer<int32_t> pv, perm, cols;
+    DeviceBuffer<int64_t> d_ip, d_cnt;
+    DeviceBuffer<char> tmp;
+    size_t tb = 0, need = 0;
+    if (permute) {
+        GEMB_CUDA(pk.alloc(n)); GEMB_CUDA(pk2.alloc(n));
+        GEMB_CUDA(pv.alloc(n)); GEMB_CUDA(perm.alloc(n));
+        cub::DeviceRadixSort::SortPairs(nullptr, need, pk.get(), pk2.get(), pv.get(), perm.get(), n, 0, 64, st); tb = std::max(tb, need);
+    }
+    GEMB_CUDA(keys.alloc(nk)); GEMB_CUDA(keys2.alloc(nk));
+    GEMB_CUDA(d_cnt.alloc(2));
+    cub::DeviceRadixSort::SortKeys(nullptr, need, keys.get(), keys2.get(), nk, 0, 64, st); tb = std::max(tb, need);
+    cub::DeviceSelect::Unique(nullptr, need, keys2.get(), keys.get(), d_cnt.get(), nk, st); tb = std::max(tb, need);
+    GEMB_CUDA(tmp.alloc(tb));
+    if (permute) {
+        rmat_perm_keys_kernel<<<grid, 256, 0, st>>>(n, seed, pk.get(), pv.get());
+        GEMB_CUDA(cudaGetLastError());
+        GEMB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tb, pk.get(), pk2.get(), pv.get(), perm.get(), n, 0, 64, st));
+        count_launch(2);
+    }
+    const uint32_t ta = (uint32_t)std::min(4294967295.0, a * 4294967296.0);
+    const uint32_t tab = (uint32_t)std::min(4294967295.0, (a + b) * 4294967296.0);
+    const uint32_t tabc = (uint32_t)std::min(4294967295.0, (a + b + c) * 4294967296.0);
+    rmat_pairs_kernel<<<grid, 256, 0, st>>>(m, scale, ta, tab, tabc, seed, permute ? perm.get() : nullptr, keys.get());
+    GEMB_CUDA(cudaGetLastError());
+    GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.get(), tb, keys.get(), keys2.get(), nk, 0, 64, st));
+    GEMB_CUDA(cub::DeviceSelect::Unique(tmp.get(), tb, keys2.get(), keys.get(), d_cnt.get(), nk, st));
+    count_launch(3);
+    int64_t nu = 0;
+    GEMB_CUDA(cudaMemcpyAsync(&nu, d_cnt.get(), 8, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaStreamSynchronize(st));
+    uint64_t last = 0;
+    if (nu > 0) {
+        GEMB_CUDA(cudaMemcpyAsync(&last, keys.get() + (nu - 1), 8, cudaMemcpyDeviceToHost, st));
+        GEMB_CUDA(cudaStreamSynchronize(st));
+        if (last == ~0ull) nu--;                                   // the self-loop sentinel
+    }
+    if (nnz_total_out) *nnz_total_out = nu;
+    GEMB_CUDA(d_ip.alloc(n_rows + 1));
+    rmat_rowptr_kernel<<<grid, 256, 0, st>>>(n_rows, row0, keys.get(), nu, d_ip.get(), d_cnt.get() + 1);
+    GEMB_CUDA(cudaGetLastError());
+    int64_t ends[2] = {0, 0};
+    GEMB_CUDA(cudaMemcpyAsync(&ends[0], d_ip.get(), 8, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaMemcpyAsync(&ends[1], d_ip.get() + n_rows, 8, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaStreamSynchronize(st));
+    const int64_t cnt = ends[1] - ends[0];
+    if (nnz_out) *nnz_out = cnt;
+    count_launch();
+    if (!indices_out) return GEMB_OK;
+    GEMB_ARG(indptr_out && cap >= cnt, "indptr_out / cap");
+    rmat_rebase_kernel<<<grid, 256, 0, st>>>(n_rows, d_ip.get(), d_cnt.get() + 1);
+    GEMB_CUDA(cudaGetLastError());
+    GEMB_CUDA(cols.alloc(std::max<int64_t>(cnt, 1)));
+    rmat_cols_kernel<<<grid, 256, 0, st>>>(cnt, keys.get() + ends[0], cols.get());
+    GEMB_CUDA(cudaGetLastError());
+    count_launch(2);
+    GEMB_CUDA(cudaMemcpyAsync(indptr_out, d_ip.get(), 8 * (size_t)(n_rows + 1), cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaMemcpyAsync(indices_out, cols.get(), 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
+    GEMB_CUDA(cudaStreamSynchronize(st));
+    return GEMB_OK;
+}
+
 }  // namespace gemb
 
 using namespace gemb;
@@ -87,79 +157,12 @@ extern "C" int gemb_synth_rmat(gemb_ctx *ctx, int scale, int edge_factor, double
     GEMB_ARG(ctx, "ctx");
     GEMB_ARG(scale >= 1 && scale <= 30 && edge_factor >= 1, "scale / edge_factor");
     GEMB_ARG(a > 0 && b >= 0 && c >= 0 && a + b + c < 1.0, "quadrant probabilities");
-    const int64_t n = (int64_t)1 << scale, m = n * edge_factor, nk = 2 * m;
+    const int64_t n = (int64_t)1 << scale;
     if (n_rows < 0) { row0 = 0; n_rows = n; }
     GEMB_ARG(row0 >= 0 && row0 + n_rows <= n, "row range");
     GEMB_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    const int grid = ctx->sm_count * 8;
-    uint64_t *pk = nullptr, *pk2 = nullptr, *keys = nullptr, *keys2 = nullptr;
-    int32_t *pv = nullptr, *perm = nullptr, *cols = nullptr;
-    int64_t *d_ip = nullptr, *d_cnt = nullptr;
-    void *tmp = nullptr;
-    int status = GEMB_OK;
-    auto body = [&]() -> int {
-        size_t tb = 0, need = 0;
-        if (permute) {
-            GEMB_CUDA(dmalloc(&pk, 8 * (size_t)n)); GEMB_CUDA(dmalloc(&pk2, 8 * (size_t)n));
-            GEMB_CUDA(dmalloc(&pv, 4 * (size_t)n)); GEMB_CUDA(dmalloc(&perm, 4 * (size_t)n));
-            cub::DeviceRadixSort::SortPairs(nullptr, need, pk, pk2, pv, perm, n, 0, 64, st); tb = std::max(tb, need);
-        }
-        GEMB_CUDA(dmalloc(&keys, 8 * (size_t)nk)); GEMB_CUDA(dmalloc(&keys2, 8 * (size_t)nk));
-        GEMB_CUDA(dmalloc(&d_cnt, 16));
-        cub::DeviceRadixSort::SortKeys(nullptr, need, keys, keys2, nk, 0, 64, st); tb = std::max(tb, need);
-        cub::DeviceSelect::Unique(nullptr, need, keys2, keys, d_cnt, nk, st); tb = std::max(tb, need);
-        GEMB_CUDA(dmalloc(&tmp, tb ? tb : 4));
-        if (permute) {
-            rmat_perm_keys_kernel<<<grid, 256, 0, st>>>(n, seed, pk, pv);
-            GEMB_CUDA(cudaGetLastError());
-            GEMB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, pk, pk2, pv, perm, n, 0, 64, st));
-            count_launch(2);
-        }
-        const uint32_t ta = (uint32_t)std::min(4294967295.0, a * 4294967296.0);
-        const uint32_t tab = (uint32_t)std::min(4294967295.0, (a + b) * 4294967296.0);
-        const uint32_t tabc = (uint32_t)std::min(4294967295.0, (a + b + c) * 4294967296.0);
-        rmat_pairs_kernel<<<grid, 256, 0, st>>>(m, scale, ta, tab, tabc, seed, permute ? perm : nullptr, keys);
-        GEMB_CUDA(cudaGetLastError());
-        GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, keys, keys2, nk, 0, 64, st));
-        GEMB_CUDA(cub::DeviceSelect::Unique(tmp, tb, keys2, keys, d_cnt, nk, st));
-        count_launch(3);
-        int64_t nu = 0;
-        GEMB_CUDA(cudaMemcpyAsync(&nu, d_cnt, 8, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
-        uint64_t last = 0;
-        if (nu > 0) {
-            GEMB_CUDA(cudaMemcpyAsync(&last, keys + (nu - 1), 8, cudaMemcpyDeviceToHost, st));
-            GEMB_CUDA(cudaStreamSynchronize(st));
-            if (last == ~0ull) nu--;                                   // the self-loop sentinel
-        }
-        if (nnz_total_out) *nnz_total_out = nu;
-        GEMB_CUDA(dmalloc(&d_ip, 8 * (size_t)(n_rows + 1)));
-        rmat_rowptr_kernel<<<grid, 256, 0, st>>>(n_rows, row0, keys, nu, d_ip, d_cnt + 1);
-        GEMB_CUDA(cudaGetLastError());
-        int64_t ends[2] = {0, 0};
-        GEMB_CUDA(cudaMemcpyAsync(&ends[0], d_ip, 8, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaMemcpyAsync(&ends[1], d_ip + n_rows, 8, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
-        const int64_t cnt = ends[1] - ends[0];
-        if (nnz_out) *nnz_out = cnt;
-        count_launch();
-        if (!indices_out) return GEMB_OK;
-        GEMB_ARG(indptr_out && cap >= cnt, "indptr_out / cap");
-        rmat_rebase_kernel<<<grid, 256, 0, st>>>(n_rows, d_ip, d_cnt + 1);
-        GEMB_CUDA(cudaGetLastError());
-        GEMB_CUDA(dmalloc(&cols, 4 * (size_t)std::max<int64_t>(cnt, 1)));
-        rmat_cols_kernel<<<grid, 256, 0, st>>>(cnt, keys + ends[0], cols);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch(2);
-        GEMB_CUDA(cudaMemcpyAsync(indptr_out, d_ip, 8 * (size_t)(n_rows + 1), cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaMemcpyAsync(indices_out, cols, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
-        return GEMB_OK;
-    };
-    status = body();
-    cudaStreamSynchronize(st);
-    dfree(pk); dfree(pk2); dfree(pv); dfree(perm); dfree(keys); dfree(keys2); dfree(d_cnt); dfree(tmp); dfree(d_ip); dfree(cols);
+    const int status = rmat_generate(ctx, scale, edge_factor, a, b, c, seed, permute, row0, n_rows, nnz_out, nnz_total_out,
+                                     indptr_out, indices_out, cap);
     gemb_mem_trim();            // ~7 GB of generator scratch at scale 24: give it back before the solver allocates
     return status;
 }

@@ -57,9 +57,12 @@ int gemb_host_free(void *p);
  * list when the call returns, so that the next learn_embedding on the same problem shape makes no driver
  * allocation (the reference re-allocates everything per call, hope.py:26-34; at 2.5 GB per call the
  * driver's page mapping costs more than the solve).  GEMB_CACHE_MB caps the list (0 = off).
- * gemb_mem_trim returns every cached block to the driver; gemb_mem_cached_bytes reports the list. */
+ * gemb_mem_trim returns every cached block to the driver; gemb_mem_cached_bytes reports the list.
+ * gemb_mem_live_blocks counts the blocks handed out and not yet released (graphs, reconstructions, context scratch,
+ * and the work buffers of calls in flight); 0 when the cache is off.  A call that returns leaves it as it found it. */
 int gemb_mem_trim(void);
 size_t gemb_mem_cached_bytes(void);
+size_t gemb_mem_live_blocks(void);
 
 /* ---- Graph Factorization (SURVEY 8(f) rank 4).  Replaces the edge SGD of gem/embedding/gf.py:94-104 (its C++ twin:
  * gem/c_src/gf.cpp:143-164; the reference shells out to gem/c_exe/gf when it exists and then runs the Python loop anyway):
