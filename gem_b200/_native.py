@@ -381,17 +381,33 @@ class DeviceGraph:
             pass
 
 
-class Reconstruction:
-    """A_hat = L R^T (zero diagonal) resident on the device: gemb_recon_* (include/gemb200.h)."""
+RECON_DOT, RECON_SPLIT, RECON_GAUSS = 0, 1, 2
 
-    def __init__(self, ctx, X, split):
+
+class Reconstruction:
+    """The reconstruction of an embedding X resident on the device: gemb_recon_* (include/gemb200.h).
+
+    kind 0 (or False): A_hat = X X^T; kind 1 (or True, or any other value but 2): A_hat = L R^T with L, R the two
+    halves of the columns.  For both, dense / pairs / the w of top return A_hat (0 on the diagonal).
+    kind 2: score exp(-delta) with delta = |x_i - x_j|^2 (fp32).  dense / pairs / the w of top return delta itself,
+    +inf on the diagonal and where the fp64 score underflows to 0 (delta > 745.1332), so exp(-out) is the score
+    everywhere; ranks / top order by delta ascending.  A non-finite X raises.
+    `split=` is the keyword of the earlier signature and means the same as `kind`."""
+
+    def __init__(self, ctx, X, kind=None, *, split=None):
+        if (kind is None) == (split is None):
+            raise TypeError('Reconstruction: give kind (or split) once')
+        if kind is None:
+            kind = split
         X = np.ascontiguousarray(X, dtype=np.float32)
         assert X.ndim == 2
         self.ctx = ctx
         self.n, self.d = int(X.shape[0]), int(X.shape[1])
-        self.split = bool(split)
+        kind = int(kind)
+        self.kind = kind if kind in (RECON_DOT, RECON_GAUSS) else RECON_SPLIT
+        self.split = self.kind == RECON_SPLIT
         self._h = ctypes.c_void_p()
-        check(lib().gemb_recon_create(ctx._h, _ptr(X), self.n, self.d, int(self.split), ctypes.byref(self._h)))
+        check(lib().gemb_recon_create(ctx._h, _ptr(X), self.n, self.d, self.kind, ctypes.byref(self._h)))
 
     def dense(self, out=None):
         A = out if out is not None else np.empty((self.n, self.n), dtype=np.float32)

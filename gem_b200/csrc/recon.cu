@@ -20,13 +20,21 @@
 // (ldo = 64: the rows of one panel are adjacent).  Padded columns hold 0.
 // Roofline: HBM writes of 4 n^2 bytes for the product (k = 64: 32 flop per byte written, far below the tensor
 // pipe), HBM reads of 4 n^2 bytes per counting pass.
+//
+// Gaussian kind (LaplacianEigenmaps / LocallyLinearEmbedding, lap.py:39-42, lle.py:37-40: exp(-|x_i - x_j|^2)):
+// the panels hold an ORDER KEY instead of the score, key = bits 0x7f800000 - bits(delta) with delta = |x_i - x_j|^2
+// (0 when delta > 745.1332f, the last fp32 delta whose fp64 exp(-delta) is > 0).  The key is a positive float that
+// orders exactly as the score does, so the counting kernels below run on it unchanged; fp32 exp(-delta) would merge
+// distinct distances.  delta is summed in the difference form (recon_sqdist_kernel): exact 0 for equal rows.
 #include "common.cuh"
 #include <algorithm>
+#include <cmath>
 
 struct gemb_recon {
     gemb_ctx *ctx = nullptr;
     int64_t n = 0, n_pad = 0;
     int k = 0;
+    int kind = 0;             // GEMB_RECON_DOT, _SPLIT or _GAUSS
     float *adj = nullptr;     // n x n_pad, panel-major
     // gemb_recon_top cache (the bisection is 31 passes; the caller asks for the count first, then the entries)
     int top_valid = 0, top_und = 0;
@@ -201,6 +209,86 @@ recon_select_kernel(int64_t n, int64_t n_panels, int undirected, uint32_t bits, 
     }
 }
 
+// ---- Gaussian kind
+constexpr uint32_t GAUSS_KEY_ONE = 0x7f800000u;      // key of delta = 0: +inf
+constexpr uint32_t GAUSS_DELTA_MAX = 0x443a4886u;    // 745.1332f: fp64 exp(-delta) > 0 up to here, 0.0 above
+
+__device__ __forceinline__ float gauss_key(float delta) {
+    const uint32_t b = __float_as_uint(delta);       // delta >= 0 (or +inf), so its bits order like the value
+    return b <= GAUSS_DELTA_MAX ? __uint_as_float(GAUSS_KEY_ONE - b) : 0.f;
+}
+
+constexpr int SQD_ROWS = 128, SQD_KC = 16, SQD_THREADS = 256;   // 16 x 16 threads, 8 rows x 4 columns each
+
+// One launch over every (128-row x 64-column) tile, tile t = panel (t / row_tiles), row tile (t % row_tiles): the row
+// tiles of one panel run next to each other and share its 64 column vectors in L2.  The rows and the panel's
+// columns are staged k-major in shared memory, SQD_KC coordinates at a time; each thread keeps an 8 x 4 tile of
+// sum_k (x_ik - x_jk)^2 (FADD + FFMA per term, fp32) and its 16 threads of a row write the whole 256-byte panel row.
+// Diagonal and padded columns get key 0.
+__global__ void __launch_bounds__(SQD_THREADS)
+recon_sqdist_kernel(int64_t n, int d, int64_t row_tiles, const float *__restrict__ X, float *__restrict__ adj) {
+    __shared__ __align__(16) float xr[SQD_KC][SQD_ROWS + 4];
+    __shared__ __align__(16) float xc[SQD_KC][PW + 4];
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int64_t p = (int64_t)blockIdx.x / row_tiles;
+    const int64_t i0 = ((int64_t)blockIdx.x - p * row_tiles) * SQD_ROWS, j0 = p * PW;
+    float acc[8][4];
+#pragma unroll
+    for (int r = 0; r < 8; r++)
+#pragma unroll
+        for (int c = 0; c < 4; c++) acc[r][c] = 0.f;
+    for (int k0 = 0; k0 < d; k0 += SQD_KC) {
+        const int kc = min(SQD_KC, d - k0);
+        for (int idx = tid; idx < SQD_ROWS * SQD_KC; idx += SQD_THREADS) {
+            const int kk = idx % SQD_KC, r = idx / SQD_KC;
+            const int64_t i = i0 + r;
+            xr[kk][r] = (i < n && kk < kc) ? X[i * d + k0 + kk] : 0.f;
+        }
+        for (int idx = tid; idx < PW * SQD_KC; idx += SQD_THREADS) {
+            const int kk = idx % SQD_KC, c = idx / SQD_KC;
+            const int64_t j = j0 + c;
+            xc[kk][c] = (j < n && kk < kc) ? X[j * d + k0 + kk] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int kk = 0; kk < kc; kk++) {
+            const float4 a0 = *reinterpret_cast<const float4 *>(&xr[kk][ty * 8]);
+            const float4 a1 = *reinterpret_cast<const float4 *>(&xr[kk][ty * 8 + 4]);
+            const float4 b4 = *reinterpret_cast<const float4 *>(&xc[kk][tx * 4]);
+            const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            const float b[4] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+            for (int r = 0; r < 8; r++)
+#pragma unroll
+                for (int c = 0; c < 4; c++) {
+                    const float t = a[r] - b[c];
+                    acc[r][c] = fmaf(t, t, acc[r][c]);
+                }
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const int64_t i = i0 + ty * 8 + r;
+        if (i >= n) break;
+        float v[4];
+#pragma unroll
+        for (int c = 0; c < 4; c++) {
+            const int64_t j = j0 + tx * 4 + c;
+            v[c] = (j < n && j != i) ? gauss_key(acc[r][c]) : 0.f;
+        }
+        *reinterpret_cast<float4 *>(adj + ((size_t)p * (size_t)n + (size_t)i) * PW + tx * 4) = make_float4(v[0], v[1], v[2], v[3]);
+    }
+}
+
+// key -> delta in place (key 0: the diagonal, padding or an underflowed score -> +inf, so exp(-delta) = 0 there too)
+__global__ void recon_key_to_delta_kernel(int64_t m, float *__restrict__ w) {
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t b = __float_as_uint(w[t]);
+        w[t] = b ? __uint_as_float(GAUSS_KEY_ONE - b) : __uint_as_float(GAUSS_KEY_ONE);
+    }
+}
+
 static int grid_for(gemb_ctx *c, int64_t items, int per_block) {
     int64_t g = (items + per_block - 1) / per_block;
     const int64_t cap = (int64_t)c->sm_count * 16;
@@ -224,27 +312,66 @@ static int count_ge(gemb_recon *r, int undirected, uint32_t bits, unsigned long 
     return GEMB_OK;
 }
 
+// Gaussian kind: turn the m keys at w (device) into delta before they are copied out; a no-op for the other kinds
+static int decode_out(const gemb_recon *r, int64_t m, float *w) {
+    if (r->kind != GEMB_RECON_GAUSS || m == 0) return GEMB_OK;
+    recon_key_to_delta_kernel<<<grid_for(r->ctx, m, 256), 256, 0, r->ctx->stream>>>(m, w);
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    return GEMB_OK;
+}
+
 }  // namespace gemb
 
 using namespace gemb;
 
 extern "C" {
 
-int gemb_recon_create(gemb_ctx *c, const float *X, int64_t n, int d, int split, gemb_recon **out) {
+static int recon_create_gauss(gemb_ctx *c, const float *X, int64_t n, int d, int64_t n_pad, float *adj) {
+    DeviceBuffer<float> dX;
+    GEMB_CUDA(dX.alloc((size_t)n * d));
+    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
+    const int64_t row_tiles = (n + SQD_ROWS - 1) / SQD_ROWS;
+    recon_sqdist_kernel<<<(unsigned)(row_tiles * (n_pad / PW)), SQD_THREADS, 0, c->stream>>>(n, d, row_tiles, dX.get(), adj);
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
+}
+
+int gemb_recon_create(gemb_ctx *c, const float *X, int64_t n, int d, int kind, gemb_recon **out) {
     GEMB_ARG(c && X && out, "ctx/X/out");
     GEMB_ARG(n > 0 && n < ((int64_t)1 << 31), "n");
+    if (kind != GEMB_RECON_DOT && kind != GEMB_RECON_GAUSS) kind = GEMB_RECON_SPLIT;
+    const bool split = kind == GEMB_RECON_SPLIT;
     GEMB_ARG(d > 0 && (!split || d % 2 == 0), "d (even when split)");
+    if (kind == GEMB_RECON_GAUSS) {
+        const size_t total = (size_t)n * (size_t)d;
+        for (size_t t = 0; t < total; t++)
+            GEMB_ARG(std::isfinite(X[t]), "X finite (a NaN or infinite distance has no place in the order)");
+    }
     GEMB_CUDA(cudaSetDevice(c->device));
     const int k = split ? d / 2 : d;
     const int64_t n_pad = (n + PW - 1) / PW * PW;
     size_t free_b = 0, total_b = 0;
     GEMB_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    const double need = 4.0 * (double)n * (double)n_pad + 4.0 * (double)n * d + 8.0 * (double)n_pad * k;
+    const double factors = kind == GEMB_RECON_GAUSS ? 0.0 : 8.0 * (double)n_pad * k;   // L and Rt
+    const double need = 4.0 * (double)n * (double)n_pad + 4.0 * (double)n * d + factors;
     if (need > 0.9 * ((double)free_b + (double)gemb_mem_cached_bytes())) {
         set_error("gemb_recon_create: the %lld x %lld reconstruction needs %.1f GB of device memory, %.1f GB free "
                   "(evaluate a node sample instead, as evaluate_graph_reconstruction.py does at scale)",
                   (long long)n, (long long)n, need / 1e9, (double)free_b / 1e9);
         return GEMB_ERR_NOMEM;
+    }
+    if (kind == GEMB_RECON_GAUSS) {
+        DeviceBuffer<float> adj;
+        GEMB_CUDA(adj.alloc((size_t)n * n_pad));
+        GEMB_TRY(recon_create_gauss(c, X, n, d, n_pad, adj.get()));
+        gemb_recon *r = new gemb_recon();
+        r->ctx = c; r->n = n; r->n_pad = n_pad; r->k = d; r->kind = kind;
+        r->adj = adj.release();
+        *out = r;
+        return GEMB_OK;
     }
     DeviceBuffer<float> dX, L, Rt, adj;
     GEMB_CUDA(dX.alloc((size_t)n * d));
@@ -272,7 +399,7 @@ int gemb_recon_create(gemb_ctx *c, const float *X, int64_t n, int d, int split, 
     count_launch();
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     gemb_recon *r = new gemb_recon();
-    r->ctx = c; r->n = n; r->n_pad = n_pad; r->k = k;
+    r->ctx = c; r->n = n; r->n_pad = n_pad; r->k = k; r->kind = kind;
     r->adj = adj.release();
     *out = r;
     return GEMB_OK;
@@ -299,6 +426,7 @@ int gemb_recon_dense(gemb_recon *r, float *adj_out) {
         recon_rowmajor_kernel<<<grid_for(c, nr * n, 256), 256, 0, c->stream>>>(n, r0, nr, r->adj, buf.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
+        GEMB_TRY(decode_out(r, nr * n, buf.get()));
         GEMB_CUDA(cudaMemcpyAsync(adj_out + (size_t)r0 * n, buf.get(), sizeof(float) * (size_t)nr * n, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
     }
@@ -322,6 +450,7 @@ int gemb_recon_pairs(gemb_recon *r, const int32_t *pi, const int32_t *pj, int64_
     recon_pairs_kernel<<<grid_for(c, m, 256), 256, 0, c->stream>>>(r->n, m, di.get(), dj.get(), r->adj, dout.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
+    GEMB_TRY(decode_out(r, m, dout.get()));
     GEMB_CUDA(cudaMemcpyAsync(out, dout.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     return GEMB_OK;
@@ -399,6 +528,7 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
         r->n, n_panels, und, r->top_bits, r->adj, dcounter.get(), m, di.get(), dj.get(), dw.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
+    GEMB_TRY(decode_out(r, m, dw.get()));
     GEMB_CUDA(cudaMemcpyAsync(i_out, di.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(j_out, dj.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(w_out, dw.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));

@@ -71,7 +71,7 @@ def undirected_normalised(csr):
 
 class LaplacianEigenmaps(StaticGraphEmbedding):
 
-    _recon_split = None      # get_edge_weight is exp(-|x_i - x_j|^2): the base class evaluates it entry by entry, like the reference
+    _recon_score = 'gaussian'      # get_edge_weight is exp(-|x_i - x_j|^2): reconstructed and evaluated on the GPU
 
     hyper_params = {
         'method_name': 'lap_eigmap_svd'

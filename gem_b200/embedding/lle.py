@@ -46,7 +46,7 @@ def lle_operator(csr):
 
 class LocallyLinearEmbedding(StaticGraphEmbedding):
 
-    _recon_split = None      # get_edge_weight is exp(-|x_i - x_j|^2): evaluated entry by entry, like the reference
+    _recon_score = 'gaussian'      # get_edge_weight is exp(-|x_i - x_j|^2): reconstructed and evaluated on the GPU
 
     hyper_params = {
         'method_name': 'lle_svd'

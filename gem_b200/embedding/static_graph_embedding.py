@@ -2,18 +2,30 @@
 same constructor plumbing (class-level hyper_params dict updated by kwargs, then mirrored into
 self._<key>: SURVEY F13), same getters, same error strings.  get_reconstructed_adj is the one method
 whose n^2 Python loop (reference :59-64) is replaced: a subclass that declares `_recon_split` (True: split
-halves, hope.py:43-44; False: dot product, node2vec.py:56-57) gets the product from the GPU
-(gemb_recon_create / gemb_recon_dense, fp32 arithmetic, returned as fp64 with a zero diagonal); there is no
-CPU path for it -- without a GPU it raises RuntimeError."""
+halves, hope.py:43-44; False: dot product, node2vec.py:56-57) or `_recon_score = 'gaussian'`
+(exp(-|x_i - x_j|^2), lap.py:39-42 / lle.py:37-40) gets the matrix from the GPU (gemb_recon_create /
+gemb_recon_dense, fp32 arithmetic, returned as fp64 with a zero diagonal); there is no CPU path for it -- without a
+GPU it raises RuntimeError."""
 from abc import ABC, abstractmethod
 
 import numpy as np
 
 
+def recon_kind(model):
+    """The gemb_recon_create kind of a model's get_edge_weight: 2 for `_recon_score = 'gaussian'`, 1 / 0 for
+    `_recon_split` True / False, None when it declares neither (its score is evaluated entry by entry)."""
+    if getattr(model, '_recon_score', None) == 'gaussian':
+        return 2
+    split = getattr(model, '_recon_split', None)
+    if split is None:
+        return None
+    return 1 if split else 0
+
+
 class StaticGraphEmbedding(ABC):
     """Base of the drop-in embedding classes.  Subclasses provide a class-level `hyper_params` dict (at least
-    'method_name'), `learn_embedding` and `get_edge_weight`; a subclass whose score is one of the two reference forms
-    declares `_recon_split` so that reconstruction and evaluation run on the GPU."""
+    'method_name'), `learn_embedding` and `get_edge_weight`; a subclass whose score is one of the three reference
+    forms declares `_recon_split` or `_recon_score` so that reconstruction and evaluation run on the GPU."""
 
     def __init__(self, *param_dicts, **params):
         self._method_name = self._d = self._X = None
@@ -48,8 +60,8 @@ class StaticGraphEmbedding(ABC):
         else:
             self._X = X
             rows = X.shape[0]
-        split = getattr(self, '_recon_split', None)
-        if split is None:
+        kind = recon_kind(self)
+        if kind is None:
             # a subclass with a score function of its own: evaluate it entry by entry, like the reference
             score = self.get_edge_weight
             return np.array([[0.0 if i == j else score(i, j) for j in range(rows)] for i in range(rows)],
@@ -57,8 +69,10 @@ class StaticGraphEmbedding(ABC):
         from gem_b200 import _native
         ctx = _native.Context(getattr(self, '_device', 0))
         try:
-            rec = _native.Reconstruction(ctx, np.asarray(self._X)[:rows], split)
+            rec = _native.Reconstruction(ctx, np.asarray(self._X)[:rows], kind)
             try:
+                if kind == _native.RECON_GAUSS:
+                    return np.exp(-rec.dense().astype(np.float64))     # delta is +inf on the diagonal: exp gives 0
                 return rec.dense().astype(np.float64)
             finally:
                 rec.free()

@@ -8,13 +8,17 @@ kernel (gemb_recon_ranks), the global precision curve a threshold selection (gem
 a gather of the true edges (gemb_recon_pairs).  No CPU fallback: without a GPU this raises RuntimeError.
 
 The score function is the model's get_edge_weight: split halves for HOPE (hope.py:43-44), plain dot product for
-node2vec (node2vec.py:56-57); a model must say which through its `_recon_split` attribute.
+node2vec (node2vec.py:56-57), exp(-|x_i - x_j|^2) for LaplacianEigenmaps and LocallyLinearEmbedding (lap.py:39-42,
+lle.py:37-40); a model says which through its `_recon_split` or `_recon_score` attribute.  For the Gaussian score the
+device returns delta = |x_i - x_j|^2 and the order is delta ascending (stable), which is the reference's descending
+score order; the weighted error uses exp(-delta) in fp64.
 `max_k` (extra, optional): length of the precision curve to return; the reference always returns all
 n_pred entries (max_k = -1, default here too).
 """
 import numpy as np
 
 from gem_b200 import _native
+from gem_b200.embedding.static_graph_embedding import recon_kind
 from gem_b200.evaluation import metrics
 
 
@@ -45,10 +49,11 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
                                       device=None):
     from gem_b200.graph import HostCSR
     node_num = digraph.n if isinstance(digraph, HostCSR) else len(digraph.nodes)
-    split = getattr(graph_embedding, '_recon_split', None)
-    if split is None:
-        raise TypeError('%s does not declare _recon_split (True: hope.py:43-44, False: node2vec.py:56-57)'
-                        % type(graph_embedding).__name__)
+    kind = recon_kind(graph_embedding)
+    if kind is None:
+        raise TypeError("%s declares neither _recon_split (True: hope.py:43-44, False: node2vec.py:56-57) nor "
+                        "_recon_score ('gaussian': lap.py:39-42)" % type(graph_embedding).__name__)
+    gauss = kind == _native.RECON_GAUSS
     if X_stat is not None:
         graph_embedding._X = X_stat                   # get_reconstructed_adj(X) does this (static_graph_embedding.py:56)
     X = graph_embedding.get_embedding()
@@ -67,7 +72,7 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
     dev = device if device is not None else getattr(graph_embedding, '_device', 0)
     ctx = _native.Context(dev)
     try:
-        rec = _native.Reconstruction(ctx, X, split)
+        rec = _native.Reconstruction(ctx, X, kind)
         try:
             if sample_ratio_e:
                 # evaluation_util.py:5-18 + :25-28: random pairs, kept when A_hat >= 0
@@ -75,7 +80,12 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
                 pairs = np.array(evaluation_util.get_random_edge_pairs(node_num, sample_ratio_e, is_undirected),
                                  dtype=np.int64).reshape(-1, 2)
                 w = rec.pairs(pairs[:, 0], pairs[:, 1])
-                keep = w >= 0.0
+                if gauss:
+                    # exp(-delta) >= 0 keeps every pair; ordering by -delta (exact) is ordering by the score
+                    keep = np.ones(w.shape, dtype=bool)
+                    w = -w
+                else:
+                    keep = w >= 0.0
                 pi, pj, pw = pairs[keep, 0], pairs[keep, 1], w[keep]
                 MAP, _, _ = _map_of_list(node_num, pi, pj, pw, indptr, has_edge, is_undirected)
                 order = np.argsort(-pw.astype(np.float64), kind='stable')
@@ -85,6 +95,8 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
                 ranks, _ = rec.ranks(indptr, indices, is_undirected)
                 MAP, _, _ = metrics.map_from_ranks(node_num, indptr, ranks, is_undirected)
                 ti, tj, tw = rec.top(is_undirected, max_k)
+                if gauss:
+                    tw = -tw                              # delta ascending = -delta descending
                 prec_curv, _ = metrics.precision_curve_from_top(ti, tj, tw, has_edge, max_k)
             if is_weighted:
                 # :37-40 -- nx.to_numpy_matrix(digraph) has rows/columns in list(digraph.nodes) order while the
@@ -104,6 +116,8 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
                     ev = np.array([t[1] for t in ed], dtype=np.int64)
                     a = np.array([t[2] for t in ed], dtype=np.float64)
                 est = rec.pairs(pos[eu], pos[ev]).astype(np.float64)
+                if gauss:
+                    est = np.exp(-est)
                 nz = a != 0
                 err = float(np.sqrt(np.sum((a[nz] - est[nz]) ** 2)))
                 err_baseline = float(np.sqrt(np.sum(a ** 2)))

@@ -265,18 +265,30 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
 /* ---- reconstruction and its evaluation (SURVEY 8(f) rank 1; the step after learn_embedding in tests/fit_model.py:10).
  * gemb_recon_create replaces the n^2 get_edge_weight calls of static_graph_embedding.py:48-65: A_hat = L R^T with a
  * zero diagonal, kept ON THE DEVICE (n x n fp32; GEMB_ERR_NOMEM with a message when it does not fit).
- *   split = 1: L = X[:, :d/2], R = X[:, d/2:]   (HOPE.get_edge_weight, hope.py:43-44)
- *   split = 0: L = R = X                        (node2vec.get_edge_weight, node2vec.py:56-57)
+ *   kind = 1 (or any value other than 0 and 2): L = X[:, :d/2], R = X[:, d/2:]
+ *                                                 (HOPE.get_edge_weight, hope.py:43-44)
+ *   kind = 0: L = R = X                          (node2vec.get_edge_weight, node2vec.py:56-57)
+ *   kind = 2: score exp(-delta_ij), delta_ij = |x_i - x_j|^2 summed as sum_k (x_ik - x_jk)^2 in fp32 (exactly 0 for
+ *             equal rows)   (LaplacianEigenmaps / LocallyLinearEmbedding.get_edge_weight, lap.py:39-42, lle.py:37-40).
+ *             The ranking, n_pred and top-k below order by delta ascending (= score descending) and count a pair as
+ *             predicted when delta <= 745.1332f, where the fp64 score is still > 0.  dense, pairs and the w_out of
+ *             top return delta, not the score: +inf on the diagonal and where delta > 745.1332f, so that
+ *             score = exp(-out) holds for every entry.  A non-finite X is GEMB_ERR_ARG.
  * X: host, n x d row-major fp32. */
+#define GEMB_RECON_DOT 0
+#define GEMB_RECON_SPLIT 1
+#define GEMB_RECON_GAUSS 2
 typedef struct gemb_recon gemb_recon;
-int gemb_recon_create(gemb_ctx *ctx, const float *X, int64_t n, int d, int split, gemb_recon **out);
+int gemb_recon_create(gemb_ctx *ctx, const float *X, int64_t n, int d, int kind, gemb_recon **out);
 int gemb_recon_free(gemb_recon *r);
 
-/* The dense matrix get_reconstructed_adj returns (static_graph_embedding.py:48-65): adj_out host, n x n row-major. */
+/* The dense matrix get_reconstructed_adj returns (static_graph_embedding.py:48-65): adj_out host, n x n row-major
+ * (kind 2: delta, see above). */
 int gemb_recon_dense(gemb_recon *r, float *adj_out);
 
-/* A_hat[i[t]][j[t]] for m pairs (0 on the diagonal): the sampled-pairs branch of get_edge_list_from_adj_mtrx
- * (evaluation_util.py:25-28) and the weighted reconstruction error (evaluate_graph_reconstruction.py:37-40). */
+/* A_hat[i[t]][j[t]] for m pairs (0 on the diagonal; kind 2: delta, +inf on the diagonal): the sampled-pairs branch
+ * of get_edge_list_from_adj_mtrx (evaluation_util.py:25-28) and the weighted reconstruction error
+ * (evaluate_graph_reconstruction.py:37-40). */
 int gemb_recon_pairs(gemb_recon *r, const int32_t *i, const int32_t *j, int64_t m, float *out);
 
 /* computeMAP (metrics.py:28-46) without sorting.  The true graph is a CSR by node id (host, int32).  For every
@@ -290,7 +302,8 @@ int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indice
 /* computePrecisionCurve (metrics.py:6-25): the predicted edges that can be among the max_k heaviest (max_k < 0: all
  * of them), i.e. every valid entry >= the max_k-th largest value; UNORDERED.  *m_out = their number.  Call with
  * cap = 0 to get the count, then with cap >= count and three arrays of that length; the caller orders them
- * (weight descending, then i, then j ascending = the reference's stable sort of the row-major list). */
+ * (weight descending, then i, then j ascending = the reference's stable sort of the row-major list; kind 2: w_out
+ * is delta, ordered ascending). */
 int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap, int32_t *i_out, int32_t *j_out,
                    float *w_out, int64_t *m_out);
 
