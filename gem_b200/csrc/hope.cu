@@ -78,6 +78,32 @@ struct HopeResult {
     double sigma_max = 0.0;
 };
 
+// host <-> device staging: the copy, then a stream synchronise (the host reads the result, or its buffer goes out of scope)
+static int copy_sync(gemb_ctx *c, void *dst, const void *src, size_t bytes, cudaMemcpyKind kind) {
+    GEMB_CUDA(cudaMemcpyAsync(dst, src, bytes, kind, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
+}
+
+// the width-4 probes (norm estimate, Katz series probe) leave their vectors in work blocks 2..4: zero them again, as
+// alloc_blocks left them
+static int clear_scratch(HopeWork &W) {
+    for (int i = 2; i < 5; i++) GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, sizeof(float) * (size_t)W.shard * W.b, W.c->stream));
+    return GEMB_OK;
+}
+
+// X goes into work block `blk` when it fits (d <= b; blk = nullptr: never), else into its own n_local x d allocation;
+// sigma goes into G2, free once the solver's iterations end
+static int place_output(HopeWork &W, HopeResult &R, float *blk, int d) {
+    R.Xd = blk;
+    if (!blk || (size_t)d > (size_t)W.b) {
+        GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(W.rows, 1) * d));
+        R.Xd = R.Xalloc.get();
+    }
+    R.sig_dev = (float *)W.G2.get();
+    return GEMB_OK;
+}
+
 static int comm_allgather(HopeWork &W, const float *shard_src, int width) {
     NcclApi *api = nccl_api();
     if (!api) return GEMB_ERR_NCCL;
@@ -335,8 +361,7 @@ static int rowsum_bound(HopeWork &W, double *norm_inf, bool *nonneg) {
     }
     GEMB_TRY(comm_allreduce_max_f64(W, W.scal.get(), 2));
     double h[2];
-    GEMB_CUDA(cudaMemcpyAsync(h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
     *norm_inf = h[0];
     *nonneg = (h[1] == 0.0);
     return GEMB_OK;
@@ -357,8 +382,7 @@ static int estimate_norm2(HopeWork &W, uint64_t seed, float *x, float *y, float 
         GEMB_TRY(dist_spmm(W, true, pw, 1.f, y, nullptr, z, false));
         GEMB_TRY(sumsq_launch(c, W.rows * pw, z, W.scal.get() + 1));
         GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 2));
-        GEMB_CUDA(cudaMemcpyAsync(h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
         if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }  // A^T A x = 0 (empty graph)
         est = sqrt(sqrt(h[1] / h[0]));   // ||A^T A x|| / ||x|| -> sigma_max^2
         GEMB_TRY(scale_launch(c, W.rows * pw, (float)(1.0 / sqrt(h[1])), z));
@@ -390,8 +414,7 @@ static int probe_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t s
             GEMB_TRY(dist_spmm(W, tr == 1, pw, beta, x, nullptr, y, false));
             GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get()));
             GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 1));
-            GEMB_CUDA(cudaMemcpyAsync(&h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost, c->stream));
-            GEMB_CUDA(cudaStreamSynchronize(c->stream));
+            GEMB_TRY(copy_sync(c, &h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
             const double nt = sqrt(h);
             if (prev > 0.0) *rho_est = std::max(*rho_est * (j > 8 ? 0.0 : 1.0), nt / prev / (double)beta);
             if (!(nt < 1e30)) break;
@@ -436,12 +459,35 @@ static int residual_check(HopeWork &W, float beta, int J, const float *P, const 
     count_launch();
     GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), b));
     std::vector<double> rs(b);
-    GEMB_CUDA(cudaMemcpyAsync(rs.data(), W.scal.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, rs.data(), W.scal.get(), sizeof(double) * b, cudaMemcpyDeviceToHost));
     double rm = 0.0;
     for (int j : cols) rm = std::max(rm, sqrt(rs[j]) / std::max(smax, 1e-300));
     *out = (float)rm;
     return GEMB_OK;
+}
+
+// Rayleigh-Ritz eigen step: (W.w, W.Z) = eigh(W.G2) (G2 destroyed), the eigenvalues (ascending) read back into lam.
+// Jacobi accuracy follows the requested tolerance (Z only pre-rotates the CholeskyQR and forms the Ritz vectors:
+// an off-diagonal remainder of 1e-2 tol is invisible at tol; one sweep less per round at the bench setting)
+static int ritz_eigh(HopeWork &W, float tol, std::vector<double> &lam) {
+    gemb_ctx *c = W.c;
+    const int b = W.b;
+    GEMB_TRY(c->t_dense.begin(c->stream));
+    GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)tol))));
+    GEMB_TRY(c->t_dense.end(c->stream));
+    return copy_sync(c, lam.data(), W.w.get(), sizeof(double) * b, cudaMemcpyDeviceToHost);
+}
+
+// stop measure: per-value relative change of the k SINGULAR values (theta = sigma^2) since the last round, floored at
+// 1e-3 sigma_max (tmax = sigma_max^2): a change measured against sigma_max alone never resolves the small end of a skewed
+// spectrum (R-MAT: sigma_k ~ 1e-2 sigma_max)
+static double sigma_change(const double *theta, const double *theta_prev, int k, double tmax) {
+    double change = 0.0;
+    for (int j = 0; j < k; j++) {
+        const double sj = sqrt(std::max(theta[j], 0.0)), sp = sqrt(std::max(theta_prev[j], 0.0));
+        change = std::max(change, fabs(sj - sp) / std::max(sj, 1e-3 * sqrt(tmax)));
+    }
+    return change;
 }
 
 // ------------------------------------------------------------------------------------ general solver
@@ -460,21 +506,9 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         GEMB_TRY(katz(W, false, beta, J, V, U, T1, T2));              // U = S V
         GEMB_TRY(gram_full(W, U, U, W.G.get()));                            // T = U^T U
         GEMB_CUDA(cudaMemcpyAsync(W.G2.get(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToDevice, c->stream));
-        GEMB_TRY(c->t_dense.begin(c->stream));
-        // Jacobi accuracy follows the requested tolerance (Z only pre-rotates the CholeskyQR and forms the Ritz vectors:
-        // an off-diagonal remainder of 1e-2 tol is invisible at tol; one sweep less per round at the bench setting)
-        GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)o.tol))));
-        GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(theta.data(), W.w.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(ritz_eigh(W, o.tol, theta));
         const double tmax = std::max(theta[b - 1], 1e-300);
-        double change = 0.0;
-        // per-value relative change of the SINGULAR values (theta = sigma^2), floored at 1e-3 sigma_max: a change
-        // measured against sigma_max alone never resolves the small end of a skewed spectrum (R-MAT: sigma_k ~ 1e-2 sigma_max)
-        for (int j = b - k; j < b; j++) {
-            const double sj = sqrt(std::max(theta[j], 0.0)), sp = sqrt(std::max(theta_prev[j], 0.0));
-            change = std::max(change, fabs(sj - sp) / std::max(sj, 1e-3 * sqrt(tmax)));
-        }
+        const double change = sigma_change(&theta[b - k], &theta_prev[b - k], k, tmax);
         R.change = change;
         theta_prev = theta;
         if (o.verbose)
@@ -496,18 +530,13 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
     R.sigma_max = sqrt(std::max(theta[b - 1], 0.0));
 
     // extraction: X = [U Z_k theta^-1/4 | V Z_k theta^1/4]; U = S V (un-normalised), V orthonormal
-    R.Xd = T1;
-    if ((size_t)d > (size_t)b) {
-        GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(W.rows, 1) * d));
-        R.Xd = R.Xalloc.get();
-    }
+    GEMB_TRY(place_output(W, R, T1, d));
     GEMB_TRY(c->t_dense.begin(c->stream));
     ritz_maps_kernel<<<(b * k + 255) / 256, 256, 0, c->stream>>>(b, k, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.25, 0.25);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), k, k, R.Xd, d));
     GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));
-    R.sig_dev = (float *)W.G2.get();  // G2 is free after eigh
     sqrt_top_kernel<<<(k + 127) / 128, 128, 0, c->stream>>>(b, k, W.w.get(), R.sig_dev);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
@@ -574,8 +603,7 @@ static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t 
     gemb_ctx *c = W.c;
     const int b = W.b;
     int rank = b;
-    GEMB_CUDA(cudaMemcpyAsync(&rank, W.rank_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, &rank, W.rank_dev.get(), sizeof(int), cudaMemcpyDeviceToHost));
     if (rank >= b) return GEMB_OK;      // the Gram is all-reduced: every rank takes the same branch
     GEMB_TRY(randn_launch(c, W.rows, b, seed, (uint64_t)W.g->row0, s1));
     GEMB_TRY(gram_full(W, V, V, W.G.get()));
@@ -593,14 +621,60 @@ static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t 
     return GEMB_OK;
 }
 
-// ------------------------------------------------------------------------------------ symmetric solver
-static inline double katz_f(double beta, double l) { return beta * l / (1.0 - beta * l); }
+// ------------------------------------------------------------------------------------ symmetric solvers
+// The spectral map of the symmetric solvers.  Katz (spectral_mode 0): S = f(A), f(l) = beta l / (1 - beta l), so the
+// wanted values are the largest |f(l)| over A's eigenvalues l; spectral_mode 1: the largest algebraic l themselves.
+// Every Ritz value is clamped to [-bound, bound] (Ritz values lie inside the spectrum) before it is mapped.
+struct SpecMap {
+    double beta;
+    bool katz;
+    double norm;    // a priori bound on |l|: ||A||_inf, or the power-iteration ||A||_2
+    double bound;   // current bound on |l|
+    SpecMap(double beta, bool katz, double norm) : beta(beta), katz(katz), norm(norm), bound(norm * 1.02 + 1e-30) {}
+    // bound from the Ritz values l[0..n): growth * max |l|, never above the a priori one
+    void tighten(const double *l, int n, double growth) {
+        double amax = 0.0;
+        for (int i = 0; i < n; i++) amax = std::max(amax, fabs(l[i]));
+        bound = std::min(norm * 1.02, growth * amax) + 1e-30;
+    }
+    double clamp(double l) const { return std::max(-bound, std::min(bound, l)); }
+    double f(double l) const { return beta * l / (1.0 - beta * l); }
+    // rank key, largest wanted first: |f(l)| (= sigma), or l + bound
+    double key(double l) const { l = clamp(l); return katz ? fabs(f(l)) : l + bound; }
+    // |d key / dl|: maps an eigen-residual of A to the residual of the key's triplet (|f'(l)| = beta / (1 - beta l)^2)
+    double slope(double l) const { l = clamp(l); return katz ? beta / ((1.0 - beta * l) * (1.0 - beta * l)) : 1.0; }
+    // Chebyshev filter interval [c0 - e, c0 + e] over the damped set {l : key(l) < key(l_min)}, l_min the block's Ritz
+    // value of smallest key, and the end aL (+-bound) the filter is normalised at: the dominant end, the side of l_top
+    struct Interval { double e, c0, aL; };
+    Interval damped(double l_top, double l_min) const {
+        const double tau = key(l_min);
+        double hi = katz ? tau / (beta * (1.0 + tau)) : clamp(l_min);
+        double lo = katz && tau < 1.0 ? -tau / (beta * (1.0 - tau)) : -bound;
+        lo = std::max(lo, -bound);
+        hi = std::min(hi, bound);
+        if (hi - lo < 2e-3 * bound) { const double mid = 0.5 * (hi + lo); lo = mid - 1e-3 * bound; hi = mid + 1e-3 * bound; }
+        const double e = 0.5 * (hi - lo), c0 = 0.5 * (hi + lo);
+        return {e, c0, (!katz || l_top >= c0) ? bound : -bound};
+    }
+    // the output of Ritz value l: sigma (|f(l)|, or l), the scale of its vector in X (sqrt(sigma), or 1), and whether
+    // the left half of X takes the vector negated (f(l) < 0)
+    struct Column { double sigma, scale; bool neg; };
+    Column column(double l) const {
+        l = clamp(l);
+        if (!katz) return {l, 1.0, false};
+        const double fl = f(l);
+        return {fabs(fl), sqrt(fabs(fl)), fl < 0};
+    }
+    // X column of the j-th best of k: HOPE lists sigma ascending (as svds does), LE / LLE eigenvalues descending
+    int out_col(int j, int k) const { return katz ? k - 1 - j : j; }
+};
+
 constexpr int GEMB_SWITCH_TO_LANCZOS = 1000;   // internal status of hope_symmetric (algorithm = 0 on a skewed spectrum)
 
-// nrm: tight estimate of ||A||_2 (power iteration), or < 0 when A is symmetric with non-negative weights: then
-// lambda_max = rho(A) >= |lambda_min| (Perron-Frobenius), so 1.05 * (largest Ritz value) bounds the spectrum on
-// both sides and the 2 x 16 narrow SpMM sweeps of the power iteration are not needed; hard_bound = ||A||_inf.
-static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double nrm, double hard_bound, HopeResult &R) {
+// ritz_bound: A is symmetric with non-negative weights and map.norm = ||A||_inf; then lambda_max = rho(A) >= |lambda_min|
+// (Perron-Frobenius), so 1.05 * (largest Ritz value) bounds the spectrum on both sides and the 2 x 16 narrow SpMM sweeps
+// of the power iteration are not needed.  Otherwise map.norm is a tight estimate of ||A||_2 (power iteration).
+static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool ritz_bound, HopeResult &R) {
     gemb_ctx *c = W.c;
     const int mode = o.spectral_mode;
     const int b = W.b, k = mode ? d : d / 2;
@@ -608,8 +682,6 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     R.katz_terms = 0;
     float *V = W.buf[0], *AV = W.buf[1];
     float *pool[3] = {W.buf[2], W.buf[3], W.buf[4]};
-    const bool ritz_bound = nrm < 0.0;
-    double bound = ritz_bound ? hard_bound * 1.02 + 1e-30 : nrm * 1.02 + 1e-30;
 
     // warm-up: V = orth(A^3 R), R Gaussian.  The three power steps run on the raw block and ONE CholeskyQR2 closes them
     // (round 1 orthonormalised after every step: 4 x CholeskyQR2 = 3.5 ms of the 58 ms solve at S, for nothing -- the
@@ -623,15 +695,12 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
     GEMB_TRY(cholqr_pass(W, W.G.get(), AV, pool[0]));
     int rank1 = b;
-    GEMB_CUDA(cudaMemcpyAsync(&rank1, W.rank_dev.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    const bool careful = rank1 < b;
-    if (!careful) {
+    GEMB_TRY(copy_sync(c, &rank1, W.rank_dev.get(), sizeof(int), cudaMemcpyDeviceToHost));
+    if (rank1 >= b) {
         GEMB_TRY(gram_full(W, pool[0], pool[0], W.G.get()));
         GEMB_TRY(cholqr_pass(W, W.G.get(), pool[0], V));
         GEMB_TRY(publish(W, V, b));
-    }
-    if (careful) {
+    } else {
         GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, pool[0]));
         GEMB_TRY(cholqr2(W, pool[0], pool[1], V));
         GEMB_TRY(publish(W, V, b));
@@ -645,22 +714,21 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
     std::vector<double> lam(b), gval(b), th_sorted(b), th_prev(b, 0.0);
     std::vector<double> Wh(o.stop_rule == 1 ? (size_t)b * b : 0), Zr(o.stop_rule == 1 ? (size_t)b * b : 0);
     std::vector<int> order(b);
-    struct Plan { bool valid = false; int deg = 0; double e = 0, c0 = 0, sigma1 = 0; } plan;
 
-    // scaled three-term Chebyshev recurrence on [c0 - e, c0 + e], normalised at the dominant end; returns the
-    // filtered block (one of the pool buffers); A V must be current
-    auto run_filter = [&](const Plan &pl, float **out) -> int {
-        double sigma = pl.sigma1;
-        const double e = pl.e, c0 = pl.c0, tau2 = 2.0 / pl.sigma1;
+    // scaled three-term Chebyshev recurrence of degree deg on [c0 - e, c0 + e], normalised at the dominant end by
+    // sigma1 = e / (aL - c0); returns the filtered block (one of the pool buffers); A V must be current
+    auto run_filter = [&](int deg, double e, double c0, double sigma1, float **out) -> int {
+        double sigma = sigma1;
+        const double tau2 = 2.0 / sigma1;
         float *prev = V, *cur = pool[0];
         float *free_a = pool[1], *free_b = pool[2];
         // Y1 = (sigma/e) (A V - c0 V)  -- A V is the Rayleigh-Ritz product, no extra SpMM
         GEMB_TRY(axpby_launch(W, (float)(sigma / e), AV, (float)(-sigma * c0 / e), V, cur));
-        for (int i = 2; i <= pl.deg; i++) {
+        for (int i = 2; i <= deg; i++) {
             const double sn = 1.0 / (tau2 - sigma);
             float *nxt = free_a;
             GEMB_TRY(dist_spmm3(W, false, b, (float)(2.0 * sn / e), cur, (float)(-2.0 * sn * c0 / e), true,
-                                (float)(-sigma * sn), prev, nxt, true, /*push_out=*/i < pl.deg));
+                                (float)(-sigma * sn), prev, nxt, true, /*push_out=*/i < deg));
             sigma = sn;
             // rotate: the old `prev` becomes free unless it is V (V must survive until the new basis exists)
             float *old_prev = prev;
@@ -684,32 +752,14 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         // (Measured: running the single-CTA Jacobi on a side stream while the filter starts with the PREVIOUS
         // round's interval costs two extra rounds -- 75 instead of 56 SpMM sweeps -- and is slower overall;
         // the eigen-decomposition therefore stays on the critical path.)
-        GEMB_TRY(c->t_dense.begin(c->stream));
-        // Jacobi accuracy follows the requested tolerance (Z only pre-rotates the CholeskyQR and forms the Ritz vectors:
-        // an off-diagonal remainder of 1e-2 tol is invisible at tol; one sweep less per round at the bench setting)
-        GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)o.tol))));
-        GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(lam.data(), W.w.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        float *filtered = nullptr;
-        if (ritz_bound) {
-            double amax = 0.0;
-            for (int i = 0; i < b; i++) amax = std::max(amax, fabs(lam[i]));
-            bound = std::min(hard_bound * 1.02, 1.05 * amax) + 1e-30;
-        }
-        for (int i = 0; i < b; i++) {
-            const double l = std::max(-bound, std::min(bound, lam[i]));  // Ritz values lie inside the spectrum
-            gval[i] = mode ? (l + bound) : fabs(katz_f(beta, l));        // rank key: largest algebraic / largest |f|
-        }
+        GEMB_TRY(ritz_eigh(W, o.tol, lam));
+        if (ritz_bound) map.tighten(lam.data(), b, 1.05);
+        for (int i = 0; i < b; i++) gval[i] = map.key(lam[i]);
         std::iota(order.begin(), order.end(), 0);
-        std::sort(order.begin(), order.end(), [&](int a, int c2) { return gval[a] > gval[c2]; });   // descending |f|
+        std::sort(order.begin(), order.end(), [&](int a, int c2) { return gval[a] > gval[c2]; });   // descending key
         for (int i = 0; i < b; i++) th_sorted[i] = gval[order[i]] * gval[order[i]];
         const double tmax = std::max(th_sorted[0], 1e-300);
-        double change = 0.0;
-        for (int j = 0; j < k; j++) {   // per-value relative change of sigma_j, floored at 1e-3 sigma_max (see hope_general)
-            const double sj = sqrt(th_sorted[j]), sp = sqrt(th_prev[j]);
-            change = std::max(change, fabs(sj - sp) / std::max(sj, 1e-3 * sqrt(tmax)));
-        }
+        const double change = sigma_change(th_sorted.data(), th_prev.data(), k, tmax);
         R.change = change;
         th_prev = th_sorted;
         // algorithm = 0 (auto): a first Rayleigh-Ritz round whose wanted values already span more than 3x -- a
@@ -725,8 +775,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
             // through |f'(l)| = beta / (1 - beta l)^2 and measured against sigma_max, like compute_residual does.
             GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
             GEMB_CUDA(cudaMemcpyAsync(Wh.data(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
-            GEMB_CUDA(cudaMemcpyAsync(Zr.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
-            GEMB_CUDA(cudaStreamSynchronize(c->stream));
+            GEMB_TRY(copy_sync(c, Zr.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost));
             double worst = 0.0;
             for (int j = 0; j < k; j++) {
                 const int col = order[j];
@@ -736,10 +785,8 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
                     for (int s2 = 0; s2 < b; s2++) t += Wh[(size_t)r * b + s2] * Zr[(size_t)s2 * b + col];
                     q += Zr[(size_t)r * b + col] * t;
                 }
-                const double l = std::max(-bound, std::min(bound, lam[col]));
                 const double r2 = std::max(q - lam[col] * lam[col], 0.0);
-                const double fp = mode ? 1.0 : (double)beta / ((1.0 - beta * l) * (1.0 - beta * l));
-                worst = std::max(worst, fp * sqrt(r2) / std::max(gval[order[0]], 1e-300));
+                worst = std::max(worst, map.slope(lam[col]) * sqrt(r2) / std::max(gval[order[0]], 1e-300));
             }
             stop_measure = worst;
             R.resid_est = (float)worst;
@@ -750,41 +797,28 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         if (it >= o.min_iters && stop_measure <= (double)o.tol) { R.converged = 1; break; }
         if (it == o.max_iters) break;
 
-        // damped set {l : |f(l)| < tau}, tau = smallest |f| in the block
-        const double tau = gval[order[b - 1]];
-        double hi = mode ? std::max(-bound, std::min(bound, lam[order[b - 1]])) : tau / ((double)beta * (1.0 + tau));
-        double lo = mode ? -bound : (tau < 1.0 ? -tau / ((double)beta * (1.0 - tau)) : -bound);
-        lo = std::max(lo, -bound);
-        hi = std::min(hi, bound);
-        if (hi - lo < 2e-3 * bound) { const double mid = 0.5 * (hi + lo); lo = mid - 1e-3 * bound; hi = mid + 1e-3 * bound; }
-        Plan np;
-        np.valid = true;
-        np.e = 0.5 * (hi - lo);
-        np.c0 = 0.5 * (hi + lo);
-        const double aL = (mode || lam[order[0]] >= np.c0) ? bound : -bound;    // normalise p(aL) = 1 at the dominant end
-        np.sigma1 = np.e / (aL - np.c0);
+        // filter interval over the damped set: every key below the smallest one in the block
+        const SpecMap::Interval iv = map.damped(lam[order[0]], lam[order[b - 1]]);
+        const double sigma1 = iv.e / (iv.aL - iv.c0);
         // fp32 guard: the filter spreads the block's columns over a dynamic range T_m(x_L) ~ g^m / 2; the
         // Gram-based orthonormalisation squares it, so keep it below ~2^8 (degree m), else take a power step
-        const double xL = fabs(aL - np.c0) / np.e;
+        const double xL = fabs(iv.aL - iv.c0) / iv.e;
         const double growth = xL + sqrt(std::max(xL * xL - 1.0, 0.0));
-        np.deg = o.cheb_degree;
+        int deg = o.cheb_degree;
         // opts.cheb_range_log2 (default 8): the column scaling inside the
         // Ritz-rotated CholeskyQR tolerates far more than 2^8 on the SBM spectrum (scripts/exp_solver.py sweeps the settings):
         // 2^14 with degree 16 reaches a residual of 3.0e-3 in 4 rounds / 42 sweeps (the bench setting) where 2^8 with degree 8
         // needed 8 rounds / 56 sweeps for 4.0e-3.  The library default stays conservative (tight-tolerance solves).
-        if (growth > 1.0 + 1e-9) np.deg = std::min(np.deg, (int)floor(log(2.0 * exp2((double)o.range_log2)) / log(growth)));
+        if (growth > 1.0 + 1e-9) deg = std::min(deg, (int)floor(log(2.0 * exp2((double)o.range_log2)) / log(growth)));
 
-        if (!filtered) {
-            if (np.deg < 2) {                                          // A V is already there: one power step
-                GEMB_TRY(orth_rotated(W, AV, pool[0], V));
-                GEMB_TRY(refill_dropped(W, V, pool[0], pool[1], o.seed + 7919ull * (uint64_t)it));
-                GEMB_TRY(publish(W, V, b));
-                plan = np;
-                continue;
-            }
-            GEMB_TRY(run_filter(np, &filtered));
+        if (deg < 2) {                                          // A V is already there: one power step
+            GEMB_TRY(orth_rotated(W, AV, pool[0], V));
+            GEMB_TRY(refill_dropped(W, V, pool[0], pool[1], o.seed + 7919ull * (uint64_t)it));
+            GEMB_TRY(publish(W, V, b));
+            continue;
         }
-        plan = np;
+        float *filtered = nullptr;
+        GEMB_TRY(run_filter(deg, iv.e, iv.c0, sigma1, &filtered));
         // orthonormalise the filtered block into V; scratch = any block that is neither `filtered` nor V
         float *tmp = nullptr;
         for (float *cand : {pool[0], pool[1], pool[2], AV})
@@ -794,100 +828,69 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, float beta, double 
         GEMB_TRY(publish(W, V, b));
     }
 
-    if (mode) {
-        // ---- largest algebraic eigenpairs, DESCENDING (= ascending eigenvalues of I - A_hat, the order lap.py:28-31 sorts into)
-        std::vector<double> Zh((size_t)b * b);
-        GEMB_CUDA(cudaMemcpyAsync(Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        std::vector<float> M1((size_t)b * k), ev(k);
-        for (int j = 0; j < k; j++) {
-            const int col = order[j];
-            ev[j] = (float)std::max(-bound, std::min(bound, lam[col]));
-            for (int i = 0; i < b; i++) M1[(size_t)i * k + j] = (float)Zh[(size_t)i * b + col];
-        }
-        R.sigma_max = gval[order[0]];
-        GEMB_CUDA(cudaMemcpyAsync(W.M1.get(), M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
-        R.sig_dev = (float *)W.G2.get();
-        GEMB_CUDA(cudaMemcpyAsync(R.sig_dev, ev.data(), sizeof(float) * k, cudaMemcpyHostToDevice, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        R.Xd = pool[0];
-        GEMB_TRY(c->t_dense.begin(c->stream));
-        GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), k, k, R.Xd, k));
-        GEMB_TRY(c->t_dense.end(c->stream));
-        return GEMB_OK;
-    }
-    // ---- extraction: top k by |f|, ascending sigma
-    std::vector<int> sel(order.begin(), order.begin() + k);
-    std::reverse(sel.begin(), sel.end());                             // ascending |f|
+    // ---- extraction: the k wanted columns, in output order (map.out_col).  Katz: X = [ V Z_k sign(f) sqrt(sigma) |
+    // V Z_k sqrt(sigma) ]; LE / LLE: X = V Z_k, the largest algebraic eigenpairs DESCENDING (= ascending eigenvalues of
+    // I - A_hat, the order lap.py:28-31 sorts into)
     std::vector<double> Zh((size_t)b * b);
-    GEMB_CUDA(cudaMemcpyAsync(Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost));
     std::vector<float> M1((size_t)b * k), M2((size_t)b * k), sig(k);
+    std::vector<int> sel(k);
     for (int j = 0; j < k; j++) {
-        const int col = sel[j];
-        const double l = std::max(-bound, std::min(bound, lam[col]));
-        const double f = katz_f(beta, l), sg = fabs(f), rt = sqrt(sg);
-        sig[j] = (float)sg;
+        const int col = order[j], q = map.out_col(j, k);
+        const SpecMap::Column t = map.column(lam[col]);
+        sel[q] = col;
+        sig[q] = (float)t.sigma;
         for (int i = 0; i < b; i++) {
             const double z = Zh[(size_t)i * b + col];
-            M2[(size_t)i * k + j] = (float)(z * rt);
-            M1[(size_t)i * k + j] = (float)((f < 0 ? -z : z) * rt);
+            M2[(size_t)i * k + q] = (float)(z * t.scale);
+            M1[(size_t)i * k + q] = (float)((t.neg ? -z : z) * t.scale);
         }
     }
     R.sigma_max = gval[order[0]];
+    GEMB_TRY(place_output(W, R, pool[0], d));
     GEMB_CUDA(cudaMemcpyAsync(W.M1.get(), M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(W.M2.get(), M2.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
-    R.sig_dev = (float *)W.G2.get();
-    GEMB_CUDA(cudaMemcpyAsync(R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));                      // host staging vectors go out of scope
-    R.Xd = pool[0];
-    if ((size_t)d > (size_t)b) {
-        GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(W.rows, 1) * d));
-        R.Xd = R.Xalloc.get();
-    }
+    GEMB_TRY(copy_sync(c, R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice));   // host staging goes out of scope
     GEMB_TRY(c->t_dense.begin(c->stream));
     GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), k, k, R.Xd, d));
-    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));
+    if (!mode) GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));   // LE / LLE: no right half
     GEMB_TRY(c->t_dense.end(c->stream));
+    if (mode || !o.compute_residual) return GEMB_OK;
 
-    if (o.compute_residual) {
-        // check the triplets against the Katz operator itself: || S^T u - sigma v || / sigma_max
-        const int J = katz_terms_for(beta, ritz_bound ? bound / 1.02 : nrm, o.katz_tol);
-        std::vector<float> MP((size_t)b * b, 0.f), MQ((size_t)b * b, 0.f);
-        for (int col = 0; col < b; col++) {
-            const double l = std::max(-bound, std::min(bound, lam[col]));
-            const double f = katz_f(beta, l);
-            for (int i = 0; i < b; i++) {
-                const double z = Zh[(size_t)i * b + col];
-                MP[(size_t)i * b + col] = (float)(f < 0 ? -z : z);    // u = sign(f) v
-                MQ[(size_t)i * b + col] = (float)(z * fabs(f));       // v sigma
-            }
+    // check the triplets against the Katz operator itself: || S^T u - sigma v || / sigma_max
+    const int J = katz_terms_for(map.beta, ritz_bound ? map.bound / 1.02 : map.norm, o.katz_tol);
+    std::vector<float> MP((size_t)b * b, 0.f), MQ((size_t)b * b, 0.f);
+    for (int col = 0; col < b; col++) {
+        const SpecMap::Column t = map.column(lam[col]);
+        for (int i = 0; i < b; i++) {
+            const double z = Zh[(size_t)i * b + col];
+            MP[(size_t)i * b + col] = (float)(t.neg ? -z : z);    // u = sign(f) v
+            MQ[(size_t)i * b + col] = (float)(z * t.sigma);       // v sigma
         }
-        DeviceBuffer<float> dMP, dMQ, Palloc, Q, STP;
-        const size_t blk = (size_t)W.shard * b;
-        GEMB_CUDA(dMP.alloc(b * b));
-        GEMB_CUDA(dMQ.alloc(b * b));
-        // every SpMM INPUT must be a work block in halo mode (its rows travel to the peers): P lives in AV, the Horner
-        // scratch in pool[1] / pool[2]; pool[0] may hold the result X and stays untouched
-        float *P = AV;
-        if (!W.halo) {
-            GEMB_CUDA(Palloc.alloc(blk));
-            GEMB_CUDA(cudaMemsetAsync(Palloc.get(), 0, sizeof(float) * blk, c->stream));
-            P = Palloc.get();
-        }
-        GEMB_CUDA(Q.alloc(blk));
-        GEMB_CUDA(STP.alloc(blk));
-        GEMB_CUDA(cudaMemsetAsync(Q.get(), 0, sizeof(float) * blk, c->stream));
-        GEMB_CUDA(cudaMemsetAsync(STP.get(), 0, sizeof(float) * blk, c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(dMP.get(), MP.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(dMQ.get(), MQ.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
-        GEMB_TRY(apply_launch(c, W.rows, V, b, dMP.get(), b, b, P, b));
-        GEMB_TRY(apply_launch(c, W.rows, V, b, dMQ.get(), b, b, Q.get(), b));
-        GEMB_TRY(publish(W, P, b));
-        GEMB_TRY(residual_check(W, beta, J, P, Q.get(), STP.get(), W.halo ? pool[1] : AV, W.halo ? pool[2] : pool[1], sel,
-                                R.sigma_max, &R.resid_max));
     }
-    return GEMB_OK;
+    DeviceBuffer<float> dMP, dMQ, Palloc, Q, STP;
+    const size_t blk = (size_t)W.shard * b;
+    GEMB_CUDA(dMP.alloc(b * b));
+    GEMB_CUDA(dMQ.alloc(b * b));
+    // every SpMM INPUT must be a work block in halo mode (its rows travel to the peers): P lives in AV, the Horner
+    // scratch in pool[1] / pool[2]; pool[0] may hold the result X and stays untouched
+    float *P = AV;
+    if (!W.halo) {
+        GEMB_CUDA(Palloc.alloc(blk));
+        GEMB_CUDA(cudaMemsetAsync(Palloc.get(), 0, sizeof(float) * blk, c->stream));
+        P = Palloc.get();
+    }
+    GEMB_CUDA(Q.alloc(blk));
+    GEMB_CUDA(STP.alloc(blk));
+    GEMB_CUDA(cudaMemsetAsync(Q.get(), 0, sizeof(float) * blk, c->stream));
+    GEMB_CUDA(cudaMemsetAsync(STP.get(), 0, sizeof(float) * blk, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(dMP.get(), MP.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(dMQ.get(), MQ.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
+    GEMB_TRY(apply_launch(c, W.rows, V, b, dMP.get(), b, b, P, b));
+    GEMB_TRY(apply_launch(c, W.rows, V, b, dMQ.get(), b, b, Q.get(), b));
+    GEMB_TRY(publish(W, P, b));
+    return residual_check(W, (float)map.beta, J, P, Q.get(), STP.get(), W.halo ? pool[1] : AV, W.halo ? pool[2] : pool[1], sel,
+                          R.sigma_max, &R.resid_max);
 }
 
 // ------------------------------------------------------------------------------------ Lanczos solver
@@ -930,7 +933,7 @@ __global__ void axpy_kernel(int64_t count, float a, const float *__restrict__ X,
 //   full:   (theta, Y) = eigh(T); residual of Ritz pair i = || R Y[last block, i] || (no extra sweep);
 //           stop when |f'(theta_i)| res_i <= tol * sigma_max for the k wanted pairs;
 //           else keep the k + 16 best by |f|: Q <- Q Y_keep, T <- diag(theta_keep), continue with q_{j+1}
-static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double hard_bound, HopeResult &R) {
+static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResult &R) {
     gemb_ctx *c = W.c;
     const int k = d / 2, p = 16, cw = 64;
     const int64_t rows = W.rows, shard = W.shard;
@@ -975,8 +978,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
             GEMB_TRY(apply_launch(c, rows, src, p, W.Minv.get(), p, p, scratch, p));
             GEMB_TRY(c->t_dense.end(c->stream));
             GEMB_CUDA(cudaMemcpyAsync(src, scratch, sizeof(float) * (size_t)rows * p, cudaMemcpyDeviceToDevice, c->stream));
-            GEMB_CUDA(cudaMemcpyAsync(Ginv.data(), W.G2.get(), sizeof(double) * p * p, cudaMemcpyDeviceToHost, c->stream));
-            GEMB_CUDA(cudaStreamSynchronize(c->stream));
+            GEMB_TRY(copy_sync(c, Ginv.data(), W.G2.get(), sizeof(double) * p * p, cudaMemcpyDeviceToHost));
             // invert the upper-triangular R^-1 on the host (p = 16): R = (R^-1)^-1; dropped columns (zero pivot) stay zero
             std::vector<double> &Rt = pass == 0 ? R1 : R2;
             std::fill(Rt.begin(), Rt.end(), 0.0);
@@ -1006,7 +1008,6 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
     GEMB_TRY(randn_launch(c, rows, p, o.seed, (uint64_t)W.g->row0, Vcur));
     GEMB_TRY(cholqr_p(Vcur, Tb, Rh.data()));
     int m = 0, restarts = 0, steps = 0;
-    double bound = hard_bound * 1.02 + 1e-30;
     const int max_steps = std::max(o.max_iters, 1) * (m_max / p);
     bool done = false;
     while (!done) {
@@ -1032,8 +1033,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                 GEMB_CUDA(cudaGetLastError());
                 count_launch(2);
                 GEMB_TRY(c->t_dense.end(c->stream));
-                GEMB_CUDA(cudaMemcpyAsync(Hc.data(), Gd.get(), sizeof(double) * cw * p, cudaMemcpyDeviceToHost, c->stream));
-                GEMB_CUDA(cudaStreamSynchronize(c->stream));
+                GEMB_TRY(copy_sync(c, Hc.data(), Gd.get(), sizeof(double) * cw * p, cudaMemcpyDeviceToHost));
                 for (int r = 0; r < cw && cc * cw + r < m; r++)
                     for (int q = 0; q < p; q++) Hcol[(size_t)(cc * cw + r) * p + q] += Hc[(size_t)r * p + q];
             }
@@ -1064,12 +1064,9 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
         GEMB_TRY(eigh_launch(c, m, Td.get(), wd.get(), Yd.get(), Zs.get(), 1e-9));      // Ritz values are needed to ~1e-6, the vectors feed fp32 GEMMs
         GEMB_TRY(c->t_dense.end(c->stream));
         GEMB_CUDA(cudaMemcpyAsync(theta.data(), wd.get(), sizeof(double) * m, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaMemcpyAsync(Y.data(), Yd.get(), sizeof(double) * m * m, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
-        double amax = 0.0;
-        for (int i = 0; i < m; i++) amax = std::max(amax, fabs(theta[i]));
-        bound = std::min(hard_bound * 1.02, 1.02 * amax) + 1e-30;
-        for (int i = 0; i < m; i++) fabsv[i] = fabs(katz_f(beta, std::max(-bound, std::min(bound, theta[i]))));
+        GEMB_TRY(copy_sync(c, Y.data(), Yd.get(), sizeof(double) * m * m, cudaMemcpyDeviceToHost));
+        map.tighten(theta.data(), m, 1.02);
+        for (int i = 0; i < m; i++) fabsv[i] = map.key(theta[i]);
         std::iota(order.begin(), order.begin() + m, 0);
         std::sort(order.begin(), order.begin() + m, [&](int a2, int b2) { return fabsv[a2] > fabsv[b2]; });
         const double smax = std::max(fabsv[order[0]], 1e-300);
@@ -1082,9 +1079,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                 for (int b2 = 0; b2 < p; b2++) t += Rh[(size_t)a2 * p + b2] * Y[(size_t)(m - p + b2) * m + col];
                 r2 += t * t;
             }
-            const double l = std::max(-bound, std::min(bound, theta[col]));
-            const double fp = (double)beta / ((1.0 - beta * l) * (1.0 - beta * l));
-            worst = std::max(worst, fp * sqrt(r2) / smax);
+            worst = std::max(worst, map.slope(theta[col]) * sqrt(r2) / smax);
         }
         R.change = worst;
         R.resid_est = (float)worst;
@@ -1105,8 +1100,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                 std::vector<float> Mh((size_t)cw * cw, 0.f);
                 for (int r = 0; r < cw && cc * cw + r < m; r++)
                     for (int q = 0; q < ow; q++) Mh[(size_t)r * cw + q] = (float)Y[(size_t)(cc * cw + r) * m + order[oc * cw + q]];
-                GEMB_CUDA(cudaMemcpyAsync(M32.get(), Mh.data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice, c->stream));
-                GEMB_CUDA(cudaStreamSynchronize(c->stream));
+                GEMB_TRY(copy_sync(c, M32.get(), Mh.data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice));
                 GEMB_TRY(c->t_dense.begin(c->stream));
                 GEMB_TRY(apply_launch(c, rows, Q[cc].get(), cw, M32.get(), cw, cw, cc == 0 ? Qn[oc].get() : Tmp64.get(), cw));
                 if (cc > 0) {
@@ -1121,9 +1115,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
             // X = [ v sign(f) sqrt(sigma) | v sqrt(sigma) ], sigma ascending
             std::vector<float> sig(k);
             R.sigma_max = smax;
-            R.Xd = nullptr;
-            GEMB_CUDA(R.Xalloc.alloc((size_t)std::max<int64_t>(rows, 1) * d));
-            R.Xd = R.Xalloc.get();
+            GEMB_TRY(place_output(W, R, nullptr, d));
             GEMB_ARG(k <= cw * (int)Qn.size(), "k");
             // per-column scaling on the host: column jj of Qn <-> order[jj] (descending |f|); output column k-1-jj
             std::vector<float> Ms((size_t)cw * cw), Mt((size_t)cw * cw);
@@ -1132,15 +1124,13 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                 std::fill(Ms.begin(), Ms.end(), 0.f); std::fill(Mt.begin(), Mt.end(), 0.f);
                 for (int q = 0; q < ow; q++) {
                     const int jj = oc * cw + q, col = order[jj];
-                    const double l = std::max(-bound, std::min(bound, theta[col]));
-                    const double f = katz_f(beta, l), sg = fabs(f), rt = sqrt(sg);
-                    sig[k - 1 - jj] = (float)sg;
-                    Ms[(size_t)q * cw + q] = (float)(f < 0 ? -rt : rt);
-                    Mt[(size_t)q * cw + q] = (float)rt;
+                    const SpecMap::Column t = map.column(theta[col]);
+                    sig[k - 1 - jj] = (float)t.sigma;
+                    Ms[(size_t)q * cw + q] = (float)(t.neg ? -t.scale : t.scale);
+                    Mt[(size_t)q * cw + q] = (float)t.scale;
                 }
                 for (int half = 0; half < 2; half++) {
-                    GEMB_CUDA(cudaMemcpyAsync(M32.get(), (half == 0 ? Ms : Mt).data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice, c->stream));
-                    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+                    GEMB_TRY(copy_sync(c, M32.get(), (half == 0 ? Ms : Mt).data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice));
                     GEMB_TRY(apply_launch(c, rows, Qn[oc].get(), cw, M32.get(), cw, cw, Tmp64.get(), cw));
                     // reversed column order into X: source column q -> X column (half*k) + k-1-(oc*cw+q)
                     reverse_put_kernel<<<grid_el, 256, 0, c->stream>>>(rows, ow, Tmp64.get(), cw, R.Xd, d, half * k + k - 1 - oc * cw);
@@ -1148,9 +1138,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, float beta, double ha
                     count_launch();
                 }
             }
-            R.sig_dev = (float *)W.G2.get();
-            GEMB_CUDA(cudaMemcpyAsync(R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice, c->stream));
-            GEMB_CUDA(cudaStreamSynchronize(c->stream));
+            GEMB_TRY(copy_sync(c, R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice));
             break;
         }
         // ---- restart: new basis = Qn (nk columns), T = diag(theta_keep); q_{j+1} (= Vcur) is appended next
@@ -1206,7 +1194,6 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
     const int w = (int)std::min<int64_t>(64, probe ? ((n_probe + 3) / 4 * 4) : ((n + 3) / 4 * 4));   // panel width
     HopeWork W;
     W.g = g; W.c = c; W.b = w; W.rows = n; W.shard = n;
-    const size_t blk = sizeof(float) * (size_t)n * w;
     GEMB_TRY(W.alloc_blocks((size_t)n * w));
     GEMB_CUDA(W.scal.alloc(w + 8));
     GEMB_CUDA(W.G.alloc((size_t)k * w));
@@ -1227,7 +1214,7 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
         return GEMB_ERR_DIVERGE;
     }
     const int J = katz_terms_for(beta, nrm, 1e-9);
-    for (int i = 2; i < 5; i++) GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, blk, c->stream));
+    GEMB_TRY(clear_scratch(W));
     float *Z = W.buf[0], *SZ = W.buf[1], *LZ = W.buf[2];
     const int64_t total_cols = probe ? n_probe : n;
     double acc = 0.0;
@@ -1248,8 +1235,7 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
         coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(n, w, LZ, SZ, W.scal.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-        GEMB_CUDA(cudaMemcpyAsync(rs.data(), W.scal.get(), sizeof(double) * w, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(copy_sync(c, rs.data(), W.scal.get(), sizeof(double) * w, cudaMemcpyDeviceToHost));
         for (int j = 0; j < live; j++) acc += rs[j];
     }
     *err_out = sqrt(probe ? acc / (double)n_probe : acc);
@@ -1309,7 +1295,6 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     const double t_enter = now();
     HopeWork W;
     W.g = g; W.c = c; W.b = b; W.rows = g->n_local; W.shard = g->n_shard;
-    const size_t blk = sizeof(float) * (size_t)W.shard * b;
     // multi-GPU, symmetric shard: needed-rows-only exchange over peer memory (halo.cu) unless GEMB_MG=allgather or
     // CUDA IPC is not available on this box (then every rank falls back to the all-gather form together)
     static const bool mg_allgather = getenv("GEMB_MG") && !strcmp(getenv("GEMB_MG"), "allgather");
@@ -1323,8 +1308,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         GEMB_CUDA(flag.alloc(1));
         GEMB_CUDA(cudaMemcpyAsync(flag.get(), &hflag, sizeof(int), cudaMemcpyHostToDevice, c->stream));
         ncclResult_t r = api->AllReduce(flag.get(), flag.get(), 1, ncclInt, ncclMin, (ncclComm_t)c->comm, c->stream);
-        GEMB_CUDA(cudaMemcpyAsync(&hflag, flag.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(copy_sync(c, &hflag, flag.get(), sizeof(int), cudaMemcpyDeviceToHost));
         if (r != ncclSuccess) { set_error("ncclAllReduce(halo agreement): %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
         W.halo = hflag == 1;
         if (!W.halo && o.verbose) fprintf(stderr, "[gemb_hope] halo exchange unavailable (%s); all-gather per sweep\n", gemb_last_error());
@@ -1355,7 +1339,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
 
     double nrm = 0.0, hard_bound = 0.0;
     int J = o.katz_terms;
-    bool have_nrm = false;
+    bool have_nrm = false, ritz_bound = false;
     if (beta < 0.f) {
         // beta given relative to the spectral radius: beta = |beta| / ||A||_2 (= rho(A) for the symmetric graphs of
         // BASELINE.json configs[3]: "beta = 0.5 / rho_hat"), ||A||_2 by power iteration on a width-4 block
@@ -1363,16 +1347,16 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         if (!(nrm > 0.0)) { set_error("beta < 0 asks for beta = |beta| / ||A||_2, but ||A||_2 = 0 (empty graph)"); return GEMB_ERR_ARG; }
         beta = (float)(-(double)beta / nrm);
         have_nrm = true;
-        for (int i = 2; i < 5; i++) GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, blk, c->stream));
+        GEMB_TRY(clear_scratch(W));
     }
     bool need_power = (J <= 0 && algo == 1) && !have_nrm;
     if (algo >= 2) {
         bool nonneg = false;
         GEMB_TRY(rowsum_bound(W, &hard_bound, &nonneg));
-        if (nonneg && (double)beta * hard_bound * 1.02 < 1.0) nrm = -1.0;   // spectrum bounds from Ritz values
+        if (nonneg && (double)beta * hard_bound * 1.02 < 1.0) ritz_bound = true;   // spectrum bounds from Ritz values
         else need_power = !have_nrm;
     }
-    if (have_nrm && nrm >= 0.0) {
+    if (have_nrm && !ritz_bound) {
         if ((double)beta * nrm * 1.02 >= 1.0) { set_error("|beta| / ||A||_2 with |beta| >= 0.98: outside the Katz convergence radius"); return GEMB_ERR_DIVERGE; }
         if (J <= 0) J = katz_terms_for(beta, nrm, o.katz_tol);
         if (hard_bound <= 0.0) hard_bound = nrm;
@@ -1397,17 +1381,19 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         }
         if (J <= 0) J = katz_terms_for(beta, nrm, o.katz_tol);
         if (hard_bound <= 0.0) hard_bound = nrm;
-        for (int i = 2; i < 5; i++) GEMB_CUDA(cudaMemsetAsync(W.buf[i], 0, blk, c->stream));  // width-4 scratch (local rows)
+        GEMB_TRY(clear_scratch(W));
     }
 
     HopeResult R;
     int s;
     // thick-restart Lanczos needs room for its basis (k + 16 kept + expansions); tiny graphs take the subspace solver
     const bool lanczos_fits = g->n >= 2048;
-    if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, beta, hard_bound > 0 ? hard_bound : nrm, R);
+    // a priori spectrum bound: ||A||_inf for Lanczos; for Chebyshev see hope_symmetric
+    const SpecMap lanczos_map(beta, true, hard_bound);
+    if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, lanczos_map, R);
     else if (algo >= 2) {
-        s = hope_symmetric(W, o, d, beta, nrm, hard_bound, R);
-        if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, beta, hard_bound > 0 ? hard_bound : nrm, R); }
+        s = hope_symmetric(W, o, d, SpecMap(beta, o.spectral_mode == 0, ritz_bound ? hard_bound : nrm), ritz_bound, R);
+        if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, lanczos_map, R); }
     } else s = hope_general(W, o, d, beta, J, R);
     if (s != GEMB_OK) return s;
 
@@ -1461,7 +1447,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         stats->total_ms = total_ms;
         stats->h2d_ms = 0.0;
         stats->d2h_ms = d2h_ms;
-        stats->norm2_A = (float)(nrm >= 0.0 ? nrm : hard_bound);   /* ||A||_inf when no power iteration ran */
+        stats->norm2_A = (float)(ritz_bound ? hard_bound : nrm);   /* ||A||_inf when no power iteration ran */
         stats->beta_used = beta;
         stats->ritz_change = (float)R.change;
         stats->resid_max = R.resid_max;
