@@ -242,6 +242,8 @@ int randn_launch(gemb_ctx *ctx, int64_t n, int b, uint64_t seed, uint64_t row_of
 // sum of squares of all entries (fp64 accumulate) -> out_dev[0]
 int sumsq_launch(gemb_ctx *ctx, int64_t count, const float *X, double *out_dev);
 int scale_launch(gemb_ctx *ctx, int64_t count, float s, float *X);
+// Y += a * X over count floats (one rounding per element: a = -1 gives exactly Y - X)
+int axpy_launch(gemb_ctx *ctx, int64_t count, float a, const float *X, float *Y);
 
 
 #ifdef __CUDACC__

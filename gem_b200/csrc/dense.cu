@@ -850,6 +850,19 @@ int scale_launch(gemb_ctx *ctx, int64_t count, float s, float *X) {
     return GEMB_OK;
 }
 
+// Y += a * X over count floats
+__global__ void axpy_kernel(int64_t count, float a, const float *__restrict__ X, float *__restrict__ Y) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
+        Y[i] = fmaf(a, X[i], Y[i]);
+}
+
+int axpy_launch(gemb_ctx *ctx, int64_t count, float a, const float *X, float *Y) {
+    axpy_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(count, a, X, Y);
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    return GEMB_OK;
+}
+
 }  // namespace gemb
 
 extern "C" int gemb_gram(gemb_ctx *c, int64_t n, const float *P, int b1, const float *Q, int b2,

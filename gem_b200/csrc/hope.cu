@@ -914,11 +914,6 @@ __global__ void f64_to_f32_kernel(int count, const double *__restrict__ a, float
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count) o[i] = (float)a[i];
 }
-// Y (+)= a * X over count floats
-__global__ void axpy_kernel(int64_t count, float a, const float *__restrict__ X, float *__restrict__ Y, int accumulate) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-        Y[i] = accumulate ? fmaf(a, X[i], Y[i]) : a * X[i];
-}
 
 // Thick-restart block Lanczos (block Krylov-Schur) on the symmetric A; S = f(A) shares its eigenvectors, so the
 // singular triplets of S are (|f(l)|, sign(f(l)) v, v) for the k eigenpairs with the largest |f(l)|.  This is the
@@ -1028,10 +1023,9 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
                 GEMB_TRY(c->t_dense.begin(c->stream));
                 f64_to_f32_kernel<<<(cw * p + 255) / 256, 256, 0, c->stream>>>(cw * p, Gd.get(), M32.get());
                 GEMB_CUDA(cudaGetLastError());
+                count_launch();
                 GEMB_TRY(apply_launch(c, rows, Q[cc].get(), cw, M32.get(), p, p, Tb, p));           // Q_c H_c
-                axpy_kernel<<<grid_el, 256, 0, c->stream>>>(rows * (int64_t)p, -1.f, Tb, Wb, 1);
-                GEMB_CUDA(cudaGetLastError());
-                count_launch(2);
+                GEMB_TRY(axpy_launch(c, rows * (int64_t)p, -1.f, Tb, Wb));
                 GEMB_TRY(c->t_dense.end(c->stream));
                 GEMB_TRY(copy_sync(c, Hc.data(), Gd.get(), sizeof(double) * cw * p, cudaMemcpyDeviceToHost));
                 for (int r = 0; r < cw && cc * cw + r < m; r++)
@@ -1103,11 +1097,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
                 GEMB_TRY(copy_sync(c, M32.get(), Mh.data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice));
                 GEMB_TRY(c->t_dense.begin(c->stream));
                 GEMB_TRY(apply_launch(c, rows, Q[cc].get(), cw, M32.get(), cw, cw, cc == 0 ? Qn[oc].get() : Tmp64.get(), cw));
-                if (cc > 0) {
-                    axpy_kernel<<<grid_el, 256, 0, c->stream>>>(rows * (int64_t)cw, 1.f, Tmp64.get(), Qn[oc].get(), 1);
-                    GEMB_CUDA(cudaGetLastError());
-                    count_launch();
-                }
+                if (cc > 0) GEMB_TRY(axpy_launch(c, rows * (int64_t)cw, 1.f, Tmp64.get(), Qn[oc].get()));
                 GEMB_TRY(c->t_dense.end(c->stream));
             }
         }

@@ -2,9 +2,11 @@
 //
 // Replaces the prebuilt SNAP executable GEM shells out to (gem/embedding/node2vec.py:31-48;
 // function addresses `bin@...` refer to gem/c_exe/node2vec, see SURVEY Appendix A):
-//   PreprocessTransitionProbs/GetNodeAlias (bin@0x4127f0 / 0x4115f0) -> alias_build_kernel
+//   PreprocessTransitionProbs/GetNodeAlias (bin@0x4127f0 / 0x4115f0) -> alias_build_kernel  (first order, thread per node)
+//   PreprocessNode (bin@0x411f40)                                    -> alias2_build_kernel (p, q != 1, thread per edge)
+//                                                                       both through one Vose routine, vose()
 //   TVec::Shuffle (bin@0x40d1a0)                                     -> shuffle_rounds (host, LCG skip-ahead)
-//   SimulateWalk / AliasDrawInt (bin@0x411a00 / 0x411360)            -> walk_kernel   (thread per walk)
+//   SimulateWalk / AliasDrawInt (bin@0x411a00 / 0x411360)            -> walk_kernel<SECOND> (thread per walk, both orders)
 //   LearnVocab / InitUnigramTable (bin@0x40d560 / 0x40e520)          -> vocab_kernel + host Vose
 //   InitPosEmb / TrainModel (bin@0x40e270 / 0x40d6a0)                -> init_pos_kernel, sgns_kernel (warp per walk)
 //
@@ -47,8 +49,32 @@ __host__ __device__ __forceinline__ uint32_t lcg_skip(uint32_t seed, uint64_t k)
 __device__ __forceinline__ double lcg_uni(uint32_t s) { return __ddiv_rn((double)s, 2147483647.0); }
 
 // ------------------------------------------------------------------------------ alias tables
-// Thread per node, sequential Vose exactly as GetNodeAlias (LIFO Under/Over stacks; the two stacks
-// share the node's `scratch` segment growing from both ends).  fp64, no FMA contraction.
+// Vose's alias method exactly as GetNodeAlias: the d unnormalised weights weight(i), whose sequential sum is psum,
+// become the thresholds U and the aliases K of one table.  LIFO Under/Over stacks share the table's `st` segment,
+// growing from both ends.  fp64 in the oracle's operation order, no FMA contraction.  weight(i) may read U[i] (the
+// second-order tables keep their weights there): it is read before U[i] is written.
+template <class Weight>
+__device__ __forceinline__ void vose(int d, Weight weight, double psum, int32_t *K, double *U, int32_t *st) {
+    int nu = 0, no = 0;
+    for (int i = 0; i < d; i++) {
+        const double u = __dmul_rn(__ddiv_rn(weight(i), psum), (double)d);
+        K[i] = 0;
+        U[i] = u;
+        if (u < 1.0) st[nu++] = i; else st[d - 1 - (no++)] = i;
+    }
+    while (nu > 0 && no > 0) {
+        const int small = st[--nu];
+        const int large = st[d - 1 - (--no)];
+        K[small] = large;
+        const double ul = __dadd_rn(__dadd_rn(U[large], U[small]), -1.0);
+        U[large] = ul;
+        if (ul < 1.0) st[nu++] = large; else st[d - 1 - (no++)] = large;
+    }
+    while (nu > 0) U[st[--nu]] = 1.0;
+    while (no > 0) U[st[d - 1 - (--no)]] = 1.0;
+}
+
+// first order: thread per node, the node's table at its CSR rows
 __global__ void alias_build_kernel(int64_t n, const int32_t *__restrict__ indptr, const double *__restrict__ w,
                                    int32_t *__restrict__ K, double *__restrict__ U, int32_t *__restrict__ scratch) {
     const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -57,73 +83,16 @@ __global__ void alias_build_kernel(int64_t n, const int32_t *__restrict__ indptr
     const int d = indptr[v + 1] - indptr[v];
     if (d == 0) return;
     double psum = 0.0;
-    for (int j = 0; j < d; j++) psum = __dadd_rn(psum, w ? w[s + j] : 1.0);
-    int32_t *st = scratch + s;
-    int nu = 0, no = 0;
-    for (int i = 0; i < d; i++) {
-        const double p = __ddiv_rn(w ? w[s + i] : 1.0, psum);
-        const double u = __dmul_rn(p, (double)d);
-        K[s + i] = 0;
-        U[s + i] = u;
-        if (u < 1.0) st[nu++] = i; else st[d - 1 - (no++)] = i;
-    }
-    while (nu > 0 && no > 0) {
-        const int small = st[--nu];
-        const int large = st[d - 1 - (--no)];
-        K[s + small] = large;
-        const double ul = __dadd_rn(__dadd_rn(U[s + large], U[s + small]), -1.0);
-        U[s + large] = ul;
-        if (ul < 1.0) st[nu++] = large; else st[d - 1 - (no++)] = large;
-    }
-    while (nu > 0) U[s + st[--nu]] = 1.0;
-    while (no > 0) U[s + st[d - 1 - (--no)]] = 1.0;
+    const auto weight = [=](int j) { return w ? w[s + j] : 1.0; };
+    for (int j = 0; j < d; j++) psum = __dadd_rn(psum, weight(j));
+    vose(d, weight, psum, K + s, U + s, scratch + s);
 }
 
-// ------------------------------------------------------------------------------ walks
-// Thread per walk w = i*N + j (round i, shuffled position j).  Stream offset (oracle mode 1):
-//   (i+1)*(N-1) + w*(2*walk_len-3).
-__global__ void walk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__ idx,
-                            const int32_t *__restrict__ K, const double *__restrict__ U,
-                            const int32_t *__restrict__ order, int64_t N, int walk_len, uint32_t seed,
-                            int64_t w_begin, int64_t w_end, int32_t *__restrict__ out) {
-    const int64_t w = w_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= w_end) return;
-    int32_t *row = out + (w - w_begin) * walk_len;
-    const int64_t i = w / N;
-    const uint64_t per_walk = walk_len >= 2 ? (uint64_t)(2 * walk_len - 3) : 0;
-    uint32_t st = lcg_skip(seed, (uint64_t)(i + 1) * (uint64_t)(N - 1) + (uint64_t)w * per_walk);
-    int cur = order[w];
-    int len = 0;
-    row[len++] = cur;
-    if (walk_len > 1) {
-        int s = indptr[cur], d = indptr[cur + 1] - s;
-        if (d > 0) {
-            st = lcg_next(st);
-            cur = idx[s + (int)(st % (uint32_t)d)];   // step 1: uniform, ignores weights (bin@0x411b31)
-            row[len++] = cur;
-            while (len < walk_len) {
-                s = indptr[cur];
-                d = indptr[cur + 1] - s;
-                if (d == 0) break;
-                st = lcg_next(st);
-                const int x = (int)(int64_t)__dmul_rn(lcg_uni(st), (double)d);
-                st = lcg_next(st);
-                const double y = lcg_uni(st);
-                const int nx = y < U[s + x] ? x : K[s + x];
-                cur = idx[s + nx];
-                row[len++] = cur;
-            }
-        }
-    }
-    for (; len < walk_len; len++) row[len] = 0;   // WalksVV is zero-initialised (SURVEY F10)
-}
-
-// ------------------------------------------------------------------------------ second-order tables (p, q != 1)
-// PreprocessNode (bin@0x411f40): every directed edge (t -> v) owns an alias table over v's out-neighbours x with the
-// unnormalised weights  w(v,x)/p if x == t;  w(v,x) if x is an out-neighbour of t;  w(v,x)/q otherwise  -- the
-// sum over edges of outdeg(v) entries the reference keeps in a hash map per node.  Here: one flat array, the table
-// of CSR edge e at off2[e], built by one thread per edge with the oracle's exact fp64 operation order (sequential sum,
-// division by the sum, Vose with LIFO stacks), adjacency membership by binary search in t's sorted neighbour list.
+// Second order (p, q != 1), PreprocessNode (bin@0x411f40): every directed edge (t -> v) owns an alias table over v's
+// out-neighbours x with the unnormalised weights  w(v,x)/p if x == t;  w(v,x) if x is an out-neighbour of t;  w(v,x)/q
+// otherwise  -- the sum over edges of outdeg(v) entries the reference keeps in a hash map per node.  Here: one flat
+// array, the table of CSR edge e at off2[e], built by one thread per edge, adjacency membership by binary search in t's
+// sorted neighbour list.
 __global__ void edge_degree_kernel(int64_t nnz, const int32_t *__restrict__ indptr, const int32_t *__restrict__ idx,
                                    long long *__restrict__ deg_out) {
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x) {
@@ -152,7 +121,6 @@ __global__ void alias2_build_kernel(int64_t n, int64_t nnz, const int32_t *__res
     if (d == 0) return;
     const int ts = indptr[t], te = indptr[t + 1];
     const long long o = off2[e];
-    int32_t *K = K2 + o, *st = scratch + o;
     double *U = U2 + o;
     double psum = 0.0;
     for (int j = 0; j < d; j++) {
@@ -165,30 +133,19 @@ __global__ void alias2_build_kernel(int64_t n, int64_t nnz, const int32_t *__res
         U[j] = val;
         psum = __dadd_rn(psum, val);
     }
-    int nu = 0, no = 0;
-    for (int i = 0; i < d; i++) {
-        const double u = __dmul_rn(__ddiv_rn(U[i], psum), (double)d);
-        K[i] = 0;
-        U[i] = u;
-        if (u < 1.0) st[nu++] = i; else st[d - 1 - (no++)] = i;
-    }
-    while (nu > 0 && no > 0) {
-        const int small = st[--nu];
-        const int large = st[d - 1 - (--no)];
-        K[small] = large;
-        const double ul = __dadd_rn(__dadd_rn(U[large], U[small]), -1.0);
-        U[large] = ul;
-        if (ul < 1.0) st[nu++] = large; else st[d - 1 - (no++)] = large;
-    }
-    while (nu > 0) U[st[--nu]] = 1.0;
-    while (no > 0) U[st[d - 1 - (--no)]] = 1.0;
+    vose(d, [=](int j) { return U[j]; }, psum, K2 + o, U, scratch + o);
 }
 
-// SimulateWalk with the table of the edge just walked (bin@0x411d73); same stream offsets as walk_kernel
-__global__ void walk2_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__ idx,
-                             const int32_t *__restrict__ K2, const double *__restrict__ U2,
-                             const long long *__restrict__ off2, const int32_t *__restrict__ order, int64_t N,
-                             int walk_len, uint32_t seed, int64_t w_begin, int64_t w_end, int32_t *__restrict__ out) {
+// ------------------------------------------------------------------------------ walks
+// Thread per walk w = i*N + j (round i, shuffled position j).  Stream offset (oracle mode 1):
+//   (i+1)*(N-1) + w*(2*walk_len-3).
+// Every step after the first draws from the table of the current node (first order: at indptr[cur]) or, SECOND, from
+// the table of the CSR edge e just walked (off2[e], bin@0x411d73).
+template <bool SECOND>
+__global__ void walk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__ idx,
+                            const int32_t *__restrict__ K, const double *__restrict__ U,
+                            const long long *__restrict__ off2, const int32_t *__restrict__ order, int64_t N,
+                            int walk_len, uint32_t seed, int64_t w_begin, int64_t w_end, int32_t *__restrict__ out) {
     const int64_t w = w_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= w_end) return;
     int32_t *row = out + (w - w_begin) * walk_len;
@@ -209,19 +166,19 @@ __global__ void walk2_kernel(const int32_t *__restrict__ indptr, const int32_t *
                 s = indptr[cur];
                 d = indptr[cur + 1] - s;
                 if (d == 0) break;
-                const long long o = off2[e];
+                const long long o = SECOND ? off2[e] : s;
                 st = lcg_next(st);
                 const int x = (int)(int64_t)__dmul_rn(lcg_uni(st), (double)d);
                 st = lcg_next(st);
                 const double y = lcg_uni(st);
-                const int nx = y < U2[o + x] ? x : K2[o + x];
+                const int nx = y < U[o + x] ? x : K[o + x];
                 e = s + nx;
                 cur = idx[e];
                 row[len++] = cur;
             }
         }
     }
-    for (; len < walk_len; len++) row[len] = 0;
+    for (; len < walk_len; len++) row[len] = 0;   // WalksVV is zero-initialised (SURVEY F10)
 }
 
 // ------------------------------------------------------------------------------ vocabulary
@@ -259,12 +216,9 @@ struct SgnsParams {
     int walk_len, d, win, iters, epoch;
     float *syn_pos, *syn_neg; // rows by node id
     const int32_t *KT;        // V  (token space): first-level lookup of RndUnigramInt
-    const double *UT;         // V  (kept for reference / debugging)
-    const int32_t *tok2node;  // V
     const uint4 *ent;         // V: {thr, node(X), node(KT[X]), 0}: Y < UT[X]  <=>  draw < thr   (exact, see host)
     int64_t V;
     uint32_t seed;            // training TRnd seed
-    uint64_t seq_start;       // sequential mode: stream position where training starts (= V*d)
     int sequential;
     uint32_t *seq_state;      // sequential mode: carried RNG state across epochs/launches (device)
     unsigned long long *pair_counter;
@@ -329,8 +283,21 @@ __device__ __forceinline__ uint32_t mulmod_fold(uint32_t a, uint32_t b) {
     return (uint32_t)(r >= RNG_M ? r - RNG_M : r);
 }
 
-// one (centre = word, context = ctx) pair: 1 positive + 5 negatives.  `seqpath` processes the negatives one
-// after the other through memory (needed when a negative row repeats inside the group).
+// one sample of a pair against the context row sp: g = gradient of <sp, r> for the sample's label; neu += g r, r += g sp.
+// The positive sample (label 1) comes first and starts neu with an assignment: fmaf(g, r, 0) would turn a -0 into +0.
+template <int NV, bool POSITIVE>
+__device__ __forceinline__ void sgns_sample(const float (&sp)[NV], float (&r)[NV], float (&neu)[NV], float alpha) {
+    float f = 0.f;
+#pragma unroll
+    for (int v = 0; v < NV; v++) f = fmaf(sp[v], r[v], f);
+    f = warp_sum(f);
+    const float g = sg_grad(f, POSITIVE ? 1 : 0, alpha);
+#pragma unroll
+    for (int v = 0; v < NV; v++) { neu[v] = POSITIVE ? g * r[v] : fmaf(g, r[v], neu[v]); r[v] = fmaf(g, sp[v], r[v]); }
+}
+
+// one (centre = word, context = ctx) pair: 1 positive + 5 negatives.  The 5 negative rows are loaded together, or,
+// `seqpath`, one after the other through memory (needed when a negative row repeats inside the group).
 template <int NV, bool VEC>
 __device__ __forceinline__ void sgns_pair(const SgnsParams &P, int lane, int d, int ctx, const int (&tgt)[SG_NEG],
                                           bool seqpath, float alpha, float (&snw)[NV]) {
@@ -342,49 +309,21 @@ __device__ __forceinline__ void sgns_pair(const SgnsParams &P, int lane, int d, 
 #pragma unroll
         for (int j = 0; j < SG_NEG; j++)
             if (tgt[j] >= 0) RowIO<NV, VEC>::load(P.syn_neg + (int64_t)tgt[j] * d, d, lane, sn[j]);
-        {
-            float f = 0.f;
-#pragma unroll
-            for (int v = 0; v < NV; v++) f = fmaf(sp[v], snw[v], f);
-            f = warp_sum(f);
-            const float g = sg_grad(f, 1, alpha);
-#pragma unroll
-            for (int v = 0; v < NV; v++) { neu[v] = g * snw[v]; snw[v] = fmaf(g, sp[v], snw[v]); }
-        }
+        sgns_sample<NV, true>(sp, snw, neu, alpha);
 #pragma unroll
         for (int j = 0; j < SG_NEG; j++) {
             if (tgt[j] < 0) continue;
-            float f = 0.f;
-#pragma unroll
-            for (int v = 0; v < NV; v++) f = fmaf(sp[v], sn[j][v], f);
-            f = warp_sum(f);
-            const float g = sg_grad(f, 0, alpha);
-#pragma unroll
-            for (int v = 0; v < NV; v++) { neu[v] = fmaf(g, sn[j][v], neu[v]); sn[j][v] = fmaf(g, sp[v], sn[j][v]); }
+            sgns_sample<NV, false>(sp, sn[j], neu, alpha);
             RowIO<NV, VEC>::store(P.syn_neg + (int64_t)tgt[j] * d, d, lane, sn[j]);
         }
     } else {
-        {
-            float f = 0.f;
-#pragma unroll
-            for (int v = 0; v < NV; v++) f = fmaf(sp[v], snw[v], f);
-            f = warp_sum(f);
-            const float g = sg_grad(f, 1, alpha);
-#pragma unroll
-            for (int v = 0; v < NV; v++) { neu[v] = g * snw[v]; snw[v] = fmaf(g, sp[v], snw[v]); }
-        }
+        sgns_sample<NV, true>(sp, snw, neu, alpha);
         for (int j = 0; j < SG_NEG; j++) {
             if (tgt[j] < 0) continue;
             float sn[NV];
             float *row = P.syn_neg + (int64_t)tgt[j] * d;
             RowIO<NV, VEC>::load(row, d, lane, sn);
-            float f = 0.f;
-#pragma unroll
-            for (int v = 0; v < NV; v++) f = fmaf(sp[v], sn[v], f);
-            f = warp_sum(f);
-            const float g = sg_grad(f, 0, alpha);
-#pragma unroll
-            for (int v = 0; v < NV; v++) { neu[v] = fmaf(g, sn[v], neu[v]); sn[v] = fmaf(g, sp[v], sn[v]); }
+            sgns_sample<NV, false>(sp, sn, neu, alpha);
             RowIO<NV, VEC>::store(row, d, lane, sn);
         }
     }
@@ -393,9 +332,11 @@ __device__ __forceinline__ void sgns_pair(const SgnsParams &P, int lane, int d, 
     RowIO<NV, VEC>::store(sp_row, d, lane, sp);
 }
 
+// P is read in place from the parameter bank (__grid_constant__): a by-value copy of its fields into registers up front
+// costs the d = 128 instantiation 8 registers.
 template <int NV, bool VEC>
 __global__ void __launch_bounds__(128)
-sgns_kernel(SgnsParams P) {
+sgns_kernel(const __grid_constant__ SgnsParams P) {
     extern __shared__ int32_t s_walks[];  // warps_per_block x walk_len
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;
@@ -468,17 +409,6 @@ sgns_kernel(SgnsParams P) {
     if (lane == 0 && pairs) atomicAdd(P.pair_counter, pairs);
 }
 
-// x += y
-__global__ void axpy1_kernel(int64_t n, const float *y, float *x, float a) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        x[i] = fmaf(a, y[i], x[i]);
-}
-// d = x - x0
-__global__ void sub_kernel(int64_t n, const float *x, const float *x0, float *dd) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        dd[i] = x[i] - x0[i];
-}
-
 // ------------------------------------------------------------------------------ host pieces
 // TVec::Shuffle per round (bin@0x40d220 branch: one GetUniDevInt per swap), cumulative across rounds;
 // round i starts at stream offset i*(N-1) + i*N*(2*walk_len-3)  (oracle mode 1).
@@ -524,19 +454,17 @@ static void unigram_alias(const std::vector<int64_t> &vocab, std::vector<int32_t
 }
 
 struct N2VDev {
+    // walks only: fp64 weights; alias tables K/U (first order: a node's table at its CSR rows; second order: the table of
+    // CSR edge e at off2[e]) and their Vose scratch; the start node of every walk
     DeviceBuffer<double> w, U;
-    DeviceBuffer<int32_t> K, scratch, order, walks;
+    DeviceBuffer<int32_t> K, scratch, order;
+    DeviceBuffer<long long> off2;    // second order only: nnz + 1 table offsets
+    DeviceBuffer<int32_t> walks;
     DeviceBuffer<unsigned long long> first_pos, cnt, pairs;
     DeviceBuffer<int32_t> KT, tok2node;
     DeviceBuffer<uint4> ent;
-    DeviceBuffer<double> UT;
     DeviceBuffer<float> syn_pos, syn_neg, pos0, delta;
     DeviceBuffer<uint32_t> seq_state;
-    bool second_order = false;
-    DeviceBuffer<long long> off2;    // nnz + 1: table offset of every CSR edge
-    DeviceBuffer<int32_t> K2;
-    DeviceBuffer<double> U2;
-    long long table_entries = 0;
 };
 
 static int check_graph_for_n2v(gemb_graph *g) {
@@ -545,34 +473,23 @@ static int check_graph_for_n2v(gemb_graph *g) {
     return GEMB_OK;
 }
 
-static int build_alias2(gemb_graph *g, const double *weights64, double p, double q, N2VDev &D);
-
-static int build_alias(gemb_graph *g, const double *weights64, N2VDev &D, double p = 1.0, double q = 1.0) {
-    if (p != 1.0 || q != 1.0) return build_alias2(g, weights64, p, q, D);
+// first-order tables for p = q = 1, second-order tables (with D.off2) otherwise
+static int build_alias(gemb_graph *g, const double *weights64, double p, double q, N2VDev &D) {
     gemb_ctx *c = g->ctx;
-    const int64_t nnz = g->A.nnz;
-    GEMB_CUDA(D.K.alloc(std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(D.U.alloc(std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(D.scratch.alloc(std::max<int64_t>(nnz, 1)));
+    const int64_t nnz = g->A.nnz, n = g->n;
     if (weights64 && nnz) {
         GEMB_CUDA(D.w.alloc(nnz));
         GEMB_CUDA(cudaMemcpyAsync(D.w.get(), weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
     }
-    const int64_t n = g->n;
-    alias_build_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->stream>>>(n, g->A.indptr, D.w.get(), D.K.get(), D.U.get(),
-                                                                            D.scratch.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
-}
-
-static int build_alias2(gemb_graph *g, const double *weights64, double p, double q, N2VDev &D) {
-    gemb_ctx *c = g->ctx;
-    const int64_t nnz = g->A.nnz, n = g->n;
-    D.second_order = true;
-    if (weights64 && nnz) {
-        GEMB_CUDA(D.w.alloc(nnz));
-        GEMB_CUDA(cudaMemcpyAsync(D.w.get(), weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
+    if (p == 1.0 && q == 1.0) {
+        GEMB_CUDA(D.K.alloc(std::max<int64_t>(nnz, 1)));
+        GEMB_CUDA(D.U.alloc(std::max<int64_t>(nnz, 1)));
+        GEMB_CUDA(D.scratch.alloc(std::max<int64_t>(nnz, 1)));
+        alias_build_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->stream>>>(n, g->A.indptr, D.w.get(), D.K.get(),
+                                                                                D.U.get(), D.scratch.get());
+        GEMB_CUDA(cudaGetLastError());
+        count_launch();
+        return GEMB_OK;
     }
     GEMB_CUDA(D.off2.alloc(nnz + 1));
     long long T = 0;
@@ -594,7 +511,6 @@ static int build_alias2(gemb_graph *g, const double *weights64, double p, double
         GEMB_CUDA(cudaMemcpyAsync(&T, D.off2.get() + nnz, sizeof T, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
     }
-    D.table_entries = T;
     // the reference needs the same sum_(t->v) outdeg(v) entries in host hash maps; here they must fit in HBM
     size_t free_b = 0, total_b = 0;
     GEMB_CUDA(cudaMemGetInfo(&free_b, &total_b));
@@ -604,18 +520,18 @@ static int build_alias2(gemb_graph *g, const double *weights64, double p, double
                   "outdeg(v)) and do not fit in the %.1f GB of free device memory", p, q, T, need / 1e9, (double)free_b / 1e9);
         return GEMB_ERR_NOMEM;
     }
-    GEMB_CUDA(D.K2.alloc(std::max<long long>(T, 1)));
-    GEMB_CUDA(D.U2.alloc(std::max<long long>(T, 1)));
+    GEMB_CUDA(D.K.alloc(std::max<long long>(T, 1)));
+    GEMB_CUDA(D.U.alloc(std::max<long long>(T, 1)));
     GEMB_CUDA(D.scratch.alloc(std::max<long long>(T, 1)));
     if (nnz) {
         alias2_build_kernel<<<(unsigned)((nnz + 127) / 128), 128, 0, c->stream>>>(n, nnz, g->A.indptr, g->A.indices, D.w.get(),
-                                                                                 D.off2.get(), p, q, D.K2.get(), D.U2.get(),
+                                                                                 D.off2.get(), p, q, D.K.get(), D.U.get(),
                                                                                  D.scratch.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
     }
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    D.scratch.reset();
+    D.scratch.reset();   // 4 of the 16 bytes per entry: freed before the walks allocate theirs
     return GEMB_OK;
 }
 
@@ -623,31 +539,44 @@ static double ms_since(std::chrono::steady_clock::time_point t0) {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
-// walks [w_begin, w_end) into D.walks (device); order uploaded into D.order
-static int run_walks(gemb_graph *g, N2VDev &D, const int32_t *nids, int64_t N, int walk_len, int num_walks,
-                     uint32_t seed, int64_t w_begin, int64_t w_end, double *shuffle_ms) {
+// Alias tables (between events 0 and 1 of `ev`), then the walks [w_begin, w_end) into D.walks (device; event 2), then
+// everything only the walks needed is released.  stats (optional): zeroed, with the alias and walk fields filled in.
+template <int NEV>
+static int alias_and_walks(gemb_graph *g, const double *weights64, double p, double q, const int32_t *nids, int64_t N,
+                           int walk_len, int num_walks, uint32_t seed, int64_t w_begin, int64_t w_end, N2VDev &D,
+                           const CallEvents<NEV> &ev, gemb_n2v_stats *stats) {
     gemb_ctx *c = g->ctx;
+    GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
+    GEMB_TRY(build_alias(g, weights64, p, q, D));
+    GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
     auto t0 = std::chrono::steady_clock::now();
     std::vector<int32_t> order((size_t)num_walks * N);
     shuffle_rounds(nids, N, num_walks, walk_len, seed, order.data());
-    if (shuffle_ms) *shuffle_ms = ms_since(t0);
+    const double sh_ms = ms_since(t0);
     GEMB_CUDA(D.order.alloc(std::max<size_t>(order.size(), 1)));
     GEMB_CUDA(cudaMemcpyAsync(D.order.get(), order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, c->stream));
     const int64_t cnt = w_end - w_begin;
     GEMB_CUDA(D.walks.alloc(std::max<int64_t>(cnt * walk_len, 1)));
     if (cnt > 0) {
-        if (D.second_order)
-            walk2_kernel<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K2.get(), D.U2.get(),
-                                                                              D.off2.get(), D.order.get(), N, walk_len, seed,
-                                                                              w_begin, w_end, D.walks.get());
-        else
-            walk_kernel<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K.get(), D.U.get(),
-                                                                             D.order.get(), N, walk_len, seed, w_begin, w_end,
-                                                                             D.walks.get());
+        const long long *off2 = D.off2.get();
+        auto walk = off2 ? walk_kernel<true> : walk_kernel<false>;
+        walk<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K.get(), D.U.get(), off2,
+                                                                   D.order.get(), N, walk_len, seed, w_begin, w_end,
+                                                                   D.walks.get());
         GEMB_CUDA(cudaGetLastError());
-    count_launch();
+        count_launch();
     }
+    GEMB_CUDA(cudaEventRecord(ev[2], c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));  // `order` (host) must outlive the async copy
+    D.w.reset(); D.K.reset(); D.U.reset(); D.scratch.reset(); D.off2.reset(); D.order.reset();
+    if (stats) {
+        memset((char *)stats + sizeof(uint32_t), 0, sizeof(*stats) - sizeof(uint32_t));
+        stats->alias_ms = ev.ms(0, 1);
+        stats->shuffle_ms = sh_ms;
+        stats->walk_ms = std::max(0.0, (double)ev.ms(1, 2) - sh_ms);   // the host shuffle runs while the stream works
+        stats->n_walks = cnt;
+        stats->walk_bytes = 24.0 * (double)cnt * (double)std::max(walk_len - 1, 0);
+    }
     return GEMB_OK;
 }
 
@@ -692,7 +621,7 @@ int gemb_n2v_alias(gemb_graph *g, const double *weights64, int32_t *K_out, doubl
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     N2VDev D;
-    GEMB_TRY(build_alias(g, weights64, D));
+    GEMB_TRY(build_alias(g, weights64, 1.0, 1.0, D));
     const int64_t nnz = g->A.nnz;
     GEMB_CUDA(cudaMemcpyAsync(K_out, D.K.get(), sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(U_out, D.U.get(), sizeof(double) * nnz, cudaMemcpyDeviceToHost, c->stream));
@@ -721,25 +650,11 @@ int gemb_n2v_walks(gemb_graph *g, const double *weights64, const int32_t *nids, 
     N2VDev D;
     CallEvents<3> ev;
     GEMB_CUDA(ev.create());
-    GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
-    GEMB_TRY(build_alias(g, weights64, D, p, q));
-    GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
-    double sh_ms = 0;
-    GEMB_TRY(run_walks(g, D, nids, N, walk_len, num_walks, (uint32_t)seed, w_begin, w_end, &sh_ms));
-    GEMB_CUDA(cudaEventRecord(ev[2], c->stream));
+    GEMB_TRY(alias_and_walks(g, weights64, p, q, nids, N, walk_len, num_walks, (uint32_t)seed, w_begin, w_end, D, ev, stats));
     if (walks_out && w_end > w_begin)
         GEMB_CUDA(cudaMemcpyAsync(walks_out, D.walks.get(), sizeof(int32_t) * (size_t)(w_end - w_begin) * walk_len,
                                   cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    if (stats) {
-        const float a = ev.ms(0, 1), b = ev.ms(1, 2);
-        memset((char *)stats + sizeof(uint32_t), 0, sizeof(*stats) - sizeof(uint32_t));
-        stats->alias_ms = a;
-        stats->shuffle_ms = sh_ms;
-        stats->walk_ms = b - sh_ms > 0 ? b - sh_ms : b;
-        stats->n_walks = w_end - w_begin;
-        stats->walk_bytes = 24.0 * (double)(w_end - w_begin) * (double)std::max(walk_len - 1, 0);
-    }
     return GEMB_OK;
 }
 
@@ -758,9 +673,6 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     N2VDev D;
     CallEvents<6> ev;
     GEMB_CUDA(ev.create());
-    GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
-    GEMB_TRY(build_alias(g, weights64, D, p, q));
-    GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
 
     // ---- walks: this rank's contiguous share of the num_walks*N walks of an epoch
     const int64_t total_walks = N * (int64_t)num_walks;
@@ -768,10 +680,7 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     const int64_t w_begin = std::min<int64_t>(total_walks, per * c->rank);
     const int64_t w_end = std::min<int64_t>(total_walks, w_begin + per);
     const int64_t n_local = w_end - w_begin;
-    double sh_ms = 0;
-    GEMB_TRY(run_walks(g, D, nids, N, walk_len, num_walks, (uint32_t)seed, w_begin, w_end, &sh_ms));
-    GEMB_CUDA(cudaEventRecord(ev[2], c->stream));
-    if (D.second_order) { D.K2.reset(); D.U2.reset(); D.off2.reset(); }   // tables are walk-only
+    GEMB_TRY(alias_and_walks(g, weights64, p, q, nids, N, walk_len, num_walks, (uint32_t)seed, w_begin, w_end, D, ev, stats));
 
     // ---- vocabulary: first appearance + counts (all ranks combined), host renumbering + Vose
     auto tv0 = std::chrono::steady_clock::now();
@@ -823,10 +732,8 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     GEMB_CUDA(D.ent.alloc(V));
     GEMB_CUDA(cudaMemcpyAsync(D.ent.get(), ent.data(), sizeof(uint4) * V, cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(D.KT.alloc(V));
-    GEMB_CUDA(D.UT.alloc(V));
     GEMB_CUDA(D.tok2node.alloc(V));
     GEMB_CUDA(cudaMemcpyAsync(D.KT.get(), KT.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(D.UT.get(), UT.data(), sizeof(double) * V, cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(D.tok2node.get(), tok2node.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     const double vocab_ms = ms_since(tv0);
@@ -857,9 +764,8 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     SgnsParams P;
     P.walks = D.walks.get(); P.n_walks_local = n_local; P.walk_offset = w_begin; P.n_walks_total = total_walks;
     P.walk_len = walk_len; P.d = d; P.win = con_size; P.iters = max_iter; P.epoch = 0;
-    P.syn_pos = D.syn_pos.get(); P.syn_neg = D.syn_neg.get(); P.KT = D.KT.get(); P.UT = D.UT.get();
-    P.tok2node = D.tok2node.get(); P.ent = D.ent.get(); P.V = V;
-    P.seed = (uint32_t)seed; P.seq_start = (uint64_t)V * d; P.sequential = sequential ? 1 : 0;
+    P.syn_pos = D.syn_pos.get(); P.syn_neg = D.syn_neg.get(); P.KT = D.KT.get(); P.ent = D.ent.get(); P.V = V;
+    P.seed = (uint32_t)seed; P.sequential = sequential ? 1 : 0;
     P.seq_state = D.seq_state.get(); P.pair_counter = D.pairs.get();
     const int threads = 128;
     // Hogwild: concurrent walks race on embedding rows exactly as SNAP's OpenMP threads do.  Keep the
@@ -886,17 +792,14 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
             NcclApi *api = nccl_api();
             if (!api) return GEMB_ERR_NCCL;
             GEMB_TRY(c->t_comm.begin(c->stream));
-            const int gs = c->sm_count * 8;
             // syn_neg: delta held the pre-epoch copy
-            sub_kernel<<<gs, 256, 0, c->stream>>>(tabn, syn_neg, delta, syn_neg);       // syn_neg := d_neg
+            GEMB_TRY(axpy_launch(c, tabn, -1.f, delta, syn_neg));        // syn_neg := d_neg
             ncclResult_t r = api->AllReduce(syn_neg, syn_neg, tab, ncclFloat, ncclSum, (ncclComm_t)c->comm, c->stream);
-            axpy1_kernel<<<gs, 256, 0, c->stream>>>(tabn, delta, syn_neg, 1.f);         // + neg0
-            sub_kernel<<<gs, 256, 0, c->stream>>>(tabn, syn_pos, pos0, syn_pos);        // syn_pos := d_pos
+            GEMB_TRY(axpy_launch(c, tabn, 1.f, delta, syn_neg));         // + neg0
+            GEMB_TRY(axpy_launch(c, tabn, -1.f, pos0, syn_pos));         // syn_pos := d_pos
             if (r == ncclSuccess) r = api->AllReduce(syn_pos, syn_pos, tab, ncclFloat, ncclSum, (ncclComm_t)c->comm, c->stream);
-            axpy1_kernel<<<gs, 256, 0, c->stream>>>(tabn, pos0, syn_pos, 1.f);          // + pos0
+            GEMB_TRY(axpy_launch(c, tabn, 1.f, pos0, syn_pos));          // + pos0
             if (r != ncclSuccess) { set_error("nccl embedding allreduce: %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
-            GEMB_CUDA(cudaGetLastError());
-    count_launch();
             GEMB_TRY(c->t_comm.end(c->stream));
         }
     }
@@ -908,20 +811,14 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     if (c->nranks > 1) { comm_ms = c->t_comm.total_ms(); c->t_comm.reset(); }
     if (stats) {
-        memset((char *)stats + sizeof(uint32_t), 0, sizeof(*stats) - sizeof(uint32_t));
-        stats->alias_ms = ev.ms(0, 1);
-        stats->shuffle_ms = sh_ms;
-        stats->walk_ms = std::max(0.0, (double)ev.ms(1, 2) - sh_ms);
         stats->vocab_ms = vocab_ms;
         stats->sgns_ms = ev.ms(3, 4);
         stats->total_ms = ev.ms(0, 4);
         stats->d2h_ms = ev.ms(4, 5);
         stats->comm_ms = comm_ms;
         stats->n_tokens = V;
-        stats->n_walks = n_local;
         stats->pairs = (int64_t)h_pairs;
         stats->sgns_bytes = (double)h_pairs * 14.0 * 4.0 * (double)d;
-        stats->walk_bytes = 24.0 * (double)n_local * (double)std::max(walk_len - 1, 0);
     }
     return GEMB_OK;
 }
