@@ -23,6 +23,13 @@ EXPORTS = [
 ]
 
 
+class _Stats(ctypes.Structure):
+    """Base of the statistics structs the library fills in."""
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != 'struct_size'}
+
+
 class HopeOpts(ctypes.Structure):
     _fields_ = [('struct_size', ctypes.c_uint32), ('oversample', ctypes.c_int32),
                 ('max_iters', ctypes.c_int32), ('min_iters', ctypes.c_int32), ('tol', ctypes.c_float),
@@ -32,7 +39,7 @@ class HopeOpts(ctypes.Structure):
                 ('stop_rule', ctypes.c_int32), ('algorithm3_basis', ctypes.c_int32), ('spectral_mode', ctypes.c_int32)]
 
 
-class HopeStats(ctypes.Structure):
+class HopeStats(_Stats):
     _fields_ = [('struct_size', ctypes.c_uint32), ('iters', ctypes.c_int32), ('katz_terms', ctypes.c_int32),
                 ('block', ctypes.c_int32), ('converged', ctypes.c_int32), ('algorithm', ctypes.c_int32),
                 ('spmm_count', ctypes.c_int64),
@@ -43,19 +50,13 @@ class HopeStats(ctypes.Structure):
                 ('halo_rows', ctypes.c_int64), ('push_rows', ctypes.c_int64), ('pushes', ctypes.c_int64),
                 ('beta_used', ctypes.c_float), ('push_bytes', ctypes.c_double)]
 
-    def as_dict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_ if k != 'struct_size'}
 
-
-class N2VStats(ctypes.Structure):
+class N2VStats(_Stats):
     _fields_ = [('struct_size', ctypes.c_uint32), ('alias_ms', ctypes.c_double), ('shuffle_ms', ctypes.c_double),
                 ('walk_ms', ctypes.c_double), ('vocab_ms', ctypes.c_double), ('sgns_ms', ctypes.c_double),
                 ('total_ms', ctypes.c_double), ('h2d_ms', ctypes.c_double), ('d2h_ms', ctypes.c_double),
                 ('comm_ms', ctypes.c_double), ('n_tokens', ctypes.c_int64), ('n_walks', ctypes.c_int64),
                 ('pairs', ctypes.c_int64), ('sgns_bytes', ctypes.c_double), ('walk_bytes', ctypes.c_double)]
-
-    def as_dict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_ if k != 'struct_size'}
 
 
 def lib():
@@ -171,8 +172,31 @@ def mem_live_blocks():
     return int(lib().gemb_mem_live_blocks())
 
 
-class Context:
+class _Handle:
+    """An opaque library handle `_h`, released once by `_destroy` (the gemb_* function that frees it): explicitly, at
+    the end of a `with` block, or when the object is collected."""
+
+    def _release(self):
+        if self._h:
+            getattr(lib(), self._destroy)(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self._release()
+
+    def __del__(self):
+        try:
+            self._release()
+        except Exception:
+            pass
+
+
+class Context(_Handle):
     """One CUDA device (+ optional NCCL communicator)."""
+    _destroy = 'gemb_ctx_destroy'
 
     def __init__(self, device=0):
         self._h = ctypes.c_void_p()
@@ -223,16 +247,7 @@ class Context:
         check(lib().gemb_eigh(self._h, b, _ptr(G), float(rel_tol), _ptr(w), _ptr(Z)))
         return w, Z
 
-    def close(self):
-        if self._h:
-            lib().gemb_ctx_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    close = _Handle._release
 
 
 def synth_rmat(ctx, scale, edge_factor=8, a=0.57, b=0.19, c=0.19, seed=42, permute=True, row0=0, n_rows=-1):
@@ -268,8 +283,9 @@ def comm_unique_id():
     return buf.raw
 
 
-class DeviceGraph:
+class DeviceGraph(_Handle):
     """A CSR row shard (and its transpose) resident in HBM."""
+    _destroy = 'gemb_graph_free'
 
     def __init__(self, ctx, n, indptr, indices, data=None, indptr_t=None, indices_t=None, data_t=None,
                  row0=0):
@@ -369,43 +385,29 @@ class DeviceGraph:
                                   n_rows, _ptr(X), ctypes.byref(st)))
         return X, st.as_dict()
 
-    def free(self):
-        if self._h:
-            lib().gemb_graph_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
+    free = _Handle._release
 
 
 RECON_DOT, RECON_SPLIT, RECON_GAUSS = 0, 1, 2
 
 
-class Reconstruction:
+class Reconstruction(_Handle):
     """The reconstruction of an embedding X resident on the device: gemb_recon_* (include/gemb200.h).
 
     kind 0 (or False): A_hat = X X^T; kind 1 (or True, or any other value but 2): A_hat = L R^T with L, R the two
     halves of the columns.  For both, dense / pairs / the w of top return A_hat (0 on the diagonal).
     kind 2: score exp(-delta) with delta = |x_i - x_j|^2 (fp32).  dense / pairs / the w of top return delta itself,
     +inf on the diagonal and where the fp64 score underflows to 0 (delta > 745.1332), so exp(-out) is the score
-    everywhere; ranks / top order by delta ascending.  A non-finite X raises.
-    `split=` is the keyword of the earlier signature and means the same as `kind`."""
+    everywhere; ranks / top order by delta ascending.  A non-finite X raises."""
+    _destroy = 'gemb_recon_free'
 
-    def __init__(self, ctx, X, kind=None, *, split=None):
-        if (kind is None) == (split is None):
-            raise TypeError('Reconstruction: give kind (or split) once')
-        if kind is None:
-            kind = split
+    def __init__(self, ctx, X, kind):
         X = np.ascontiguousarray(X, dtype=np.float32)
         assert X.ndim == 2
         self.ctx = ctx
         self.n, self.d = int(X.shape[0]), int(X.shape[1])
         kind = int(kind)
         self.kind = kind if kind in (RECON_DOT, RECON_GAUSS) else RECON_SPLIT
-        self.split = self.kind == RECON_SPLIT
         self._h = ctypes.c_void_p()
         check(lib().gemb_recon_create(ctx._h, _ptr(X), self.n, self.d, self.kind, ctypes.byref(self._h)))
 
@@ -445,13 +447,4 @@ class Reconstruction:
                                        ctypes.byref(m)))
         return i, j, w
 
-    def free(self):
-        if self._h:
-            lib().gemb_recon_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
+    free = _Handle._release

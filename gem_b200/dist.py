@@ -2,6 +2,8 @@
 
 The same formulas are used inside libgemb200 (core.cu::gemb_graph_upload, n2v.cu::gemb_node2vec);
 keeping them here lets the CPU test-suite check them with gloo (tests/test_dist_cpu.py)."""
+import os
+
 import numpy as np
 
 
@@ -28,6 +30,22 @@ def pad_rows(X, n_shard):
     out = np.zeros((n_shard,) + X.shape[1:], dtype=X.dtype)
     out[:X.shape[0]] = X
     return out
+
+
+def spmd(device=None):
+    """(torch.distributed module, rank, world, device) of this process.  world > 1 only under an initialised process
+    group; the device is the given one, else LOCAL_RANK when world > 1, else 0."""
+    dist_mod, rank, world = None, 0, 1
+    if int(os.environ.get('WORLD_SIZE', '1')) > 1:
+        try:
+            import torch.distributed as td
+        except ImportError:
+            td = None
+        if td is not None and td.is_available() and td.is_initialized():
+            dist_mod, rank, world = td, td.get_rank(), td.get_world_size()
+    if device is None:
+        device = int(os.environ.get('LOCAL_RANK', '0')) if world > 1 else 0
+    return dist_mod, rank, world, device
 
 
 def init_comm_from_torch(ctx, dist_module, rank, world):

@@ -17,7 +17,6 @@ import numpy as np
 
 from gem_b200 import _native
 from gem_b200 import graph as _graph
-from gem_b200.embedding.hope import _graph_is_empty
 from gem_b200.embedding.static_graph_embedding import StaticGraphEmbedding
 
 
@@ -59,11 +58,9 @@ class GraphFactorization(StaticGraphEmbedding):
         return n, e[:, 0].astype(np.int32), e[:, 1].astype(np.int32), e[:, 2].astype(np.float32)
 
     def learn_embedding(self, graph=None, is_weighted=False, no_python=True, X0=None, **ignored):
-        if _graph_is_empty(graph):
-            raise ValueError('graph needed')
+        self._check_graph(graph)
         n, src, dst, w = self._edges(graph)
         d = int(self._d)
-        self._node_num = n
         if X0 is None:
             X0 = 0.01 * np.random.randn(n, d)                      # gf.py:94 (NumPy's global RNG, like the reference)
         mode = 1 if (src.size < 2 or bool(np.all(src[1:] >= src[:-1]))) else 0
@@ -75,16 +72,11 @@ class GraphFactorization(StaticGraphEmbedding):
             warnings.warn('GraphFactorization: graph.edges() is not grouped by source and %d x %d sequential updates exceed '
                           'sequential_limit; the edges were grouped by source row (a different SGD schedule)' % (src.size, self._max_iter),
                           RuntimeWarning, stacklevel=2)
-        ctx = _native.Context(int(getattr(self, '_device', 0)))
-        try:
+        with _native.Context(int(getattr(self, '_device', 0))) as ctx:
             X, ms = _native.graph_factorization(ctx, n, src, dst, w, d, float(self._eta), float(self._regu), int(self._max_iter),
                                                 np.asarray(X0, dtype=np.float32), mode=mode)
-        finally:
-            ctx.close()
         self.stats = {'device_ms': ms, 'mode': mode, 'edges': int(src.size), 'epochs': int(self._max_iter)}
-        dt = getattr(self, '_dtype', np.float32)
-        self._X = X if np.dtype(dt) == np.float32 else X.astype(dt)
-        return self._X
+        return self._result(X, n)
 
     def get_edge_weight(self, i, j):
         return np.dot(self._X[i, :], self._X[j, :])

@@ -19,13 +19,12 @@ learn_embedding with the same graph and receives ITS row shard of X (rows [rank*
 `graph` may also be a scipy.sparse matrix or a gem_b200.graph.HostCSR (rows = 0..n-1) so that
 million-node inputs need not go through networkx.
 """
-import os
-import warnings
+import contextlib
 
 import numpy as np
 
 from gem_b200 import _native
-from gem_b200 import graph as _graph
+from gem_b200 import dist as _gd
 from gem_b200.embedding.static_graph_embedding import StaticGraphEmbedding
 
 _OPT_KEYS = ('tol', 'max_iters', 'min_iters', 'oversample', 'katz_terms', 'katz_tol', 'seed',
@@ -34,20 +33,6 @@ _OPT_KEYS = ('tol', 'max_iters', 'min_iters', 'oversample', 'katz_terms', 'katz_
 
 
 _SPMD_CTX = {}     # (device, rank, world) -> _native.Context holding the process's NCCL communicator
-
-
-def _graph_is_empty(graph):
-    """`if not graph` of hope.py:25 for every accepted input type, checked in this order: HostCSR (.n), anything with a
-    .shape (scipy sparse matrices AND arrays raise TypeError from __len__), then len() (networkx graphs)."""
-    if graph is None:
-        return True
-    if isinstance(graph, _graph.HostCSR):
-        return graph.n == 0
-    if hasattr(graph, 'shape'):
-        return graph.shape[0] == 0
-    if hasattr(graph, '__len__'):
-        return len(graph) == 0
-    return False
 
 
 class HOPE(StaticGraphEmbedding):
@@ -69,105 +54,68 @@ class HOPE(StaticGraphEmbedding):
         self.stats = None
         self._sigma = None
 
-    def _to_csr(self, graph):
-        if isinstance(graph, _graph.HostCSR):
-            return graph
-        if hasattr(graph, 'nodes') and hasattr(graph, 'edges'):
-            return _graph.from_networkx(graph)
-        return _graph.from_scipy(graph)
-
     def learn_embedding(self, graph=None, is_weighted=False, no_python=False, out=None, **ignored):
-        if _graph_is_empty(graph):
-            raise ValueError('graph needed')
         csr = self._to_csr(graph)
         opts = {k: getattr(self, '_' + k) for k in _OPT_KEYS if hasattr(self, '_' + k)}
-        dist_mod, rank, world = self._spmd()
-        device = getattr(self, '_device', None)
-        if device is None:
-            device = int(os.environ.get('LOCAL_RANK', '0')) if world > 1 else 0
-        # SPMD: the context and its NCCL communicator are created once per process and kept (communicator set-up costs
-        # 0.5-1 s -- ten times the solve); single GPU: a context is a stream + a few small buffers, made per call
-        ctx = _SPMD_CTX.get((device, rank, world)) if world > 1 else None
-        fresh = ctx is None
-        if fresh:
-            ctx = _native.Context(device)
-        try:
-            if world > 1:
-                # SPMD contract (INTEGRATION.md C): every rank calls learn_embedding with the same graph; the library
-                # communicator is bootstrapped through the already initialised torch.distributed group; the call
-                # returns THIS rank's rows of X.
-                if fresh:
-                    from gem_b200 import dist as _gd
-                    _gd.init_comm_from_torch(ctx, dist_mod, rank, world)
-                    _SPMD_CTX[(device, rank, world)] = ctx
-                if not csr.is_symmetric():
-                    r0, ip, ix, dat = csr.row_shard(rank, world)
-                    t = csr.transpose()
-                    _, tp, tx, tdat = t.row_shard(rank, world)
-                    g = _native.DeviceGraph(ctx, csr.n, ip, ix, None if dat is None else dat.astype(np.float32),
-                                            tp, tx, None if tdat is None else tdat.astype(np.float32), row0=r0)
-                else:
-                    r0, ip, ix, dat = csr.row_shard(rank, world)
-                    g = _native.DeviceGraph(ctx, csr.n, ip, ix, None if dat is None else dat.astype(np.float32), row0=r0)
-                self._row0 = r0
-            elif csr.is_symmetric():
-                g = _native.DeviceGraph(ctx, csr.n, csr.indptr, csr.indices, csr.data_f32())
-            else:
-                t = csr.transpose()
-                g = _native.DeviceGraph(ctx, csr.n, csr.indptr, csr.indices, csr.data_f32(),
-                                        t.indptr, t.indices, t.data_f32())
-            try:
-                # beta_over_rho=c (extra hyper-parameter): beta = c / rho_hat(A), estimated on the device (BASELINE configs[3])
-                bor = getattr(self, '_beta_over_rho', None)
-                beta_arg = float(self._beta) if bor is None else -float(bor)
-                X, sigma, st = g.hope(int(self._d), beta_arg, out=out, **opts)
-                if bor is not None:
-                    self._beta = float(st['beta_used'])
-                self._svd_error = None
-                want_err = getattr(self, '_svd_error_probes', None)
-                if world == 1 and (csr.n <= 4096 if want_err is None else want_err is not False):
-                    # hope.py:38-40.  Exact up to 4096 nodes (where the reference itself is practical); beyond that
-                    # only on request, as a Hutchinson estimate with svd_error_probes Rademacher vectors (SURVEY H8).
-                    probes = 0 if (want_err is None or want_err is True or csr.n <= 4096) else int(want_err)
-                    try:
-                        self._svd_error = g.hope_svd_error(int(self._d), float(self._beta), X, probes)
-                        print('SVD error (low rank): %f' % self._svd_error)
-                    except RuntimeError as exc:        # e.g. beta*||A||_2 >= 1: the reference would print inv()'s answer
-                        print('SVD error (low rank): unavailable (%s)' % exc)
-            finally:
-                g.free()
-        finally:
-            if world == 1:
-                ctx.close()
+        dist_mod, rank, world, device = _gd.spmd(getattr(self, '_device', None))
+        if world > 1:
+            # SPMD: the context and its NCCL communicator are created once per process and kept (communicator set-up
+            # costs 0.5-1 s -- ten times the solve); single GPU: a context is a stream + a few small buffers, made per call
+            ctx = _SPMD_CTX.get((device, rank, world))
+            if ctx is None:
+                ctx = _native.Context(device)
+                _gd.init_comm_from_torch(ctx, dist_mod, rank, world)
+                _SPMD_CTX[(device, rank, world)] = ctx
+            ctx_scope = contextlib.nullcontext(ctx)
+        else:
+            ctx_scope = _native.Context(device)
+        with ctx_scope as ctx, self._upload(ctx, csr, rank, world) as g:
+            # beta_over_rho=c (extra hyper-parameter): beta = c / rho_hat(A), estimated on the device (BASELINE configs[3])
+            bor = getattr(self, '_beta_over_rho', None)
+            beta_arg = float(self._beta) if bor is None else -float(bor)
+            X, sigma, st = g.hope(int(self._d), beta_arg, out=out, **opts)
+            if bor is not None:
+                self._beta = float(st['beta_used'])
+            self._svd_error = None
+            want_err = getattr(self, '_svd_error_probes', None)
+            if world == 1 and (csr.n <= 4096 if want_err is None else want_err is not False):
+                # hope.py:38-40.  Exact up to 4096 nodes (where the reference itself is practical); beyond that
+                # only on request, as a Hutchinson estimate with svd_error_probes Rademacher vectors (SURVEY H8).
+                probes = 0 if (want_err is None or want_err is True or csr.n <= 4096) else int(want_err)
+                try:
+                    self._svd_error = g.hope_svd_error(int(self._d), float(self._beta), X, probes)
+                    print('SVD error (low rank): %f' % self._svd_error)
+                except RuntimeError as exc:        # e.g. beta*||A||_2 >= 1: the reference would print inv()'s answer
+                    print('SVD error (low rank): unavailable (%s)' % exc)
         self.stats = st
         self._sigma = sigma
-        self._node_num = csr.n
-        if not st['converged']:
-            msg = ('HOPE: the solver stopped at max_iters=%d without meeting tol=%g (singular values still moving by '
-                   '%.3g per round); the embedding is less accurate than requested -- raise max_iters / oversample '
-                   'or use algorithm=3 on power-law graphs' % (st['iters'], opts.get('tol', 1e-6), st['ritz_change']))
-            if getattr(self, '_strict', False):
-                raise RuntimeError(msg)
-            warnings.warn(msg, RuntimeWarning, stacklevel=2)
-        dt = getattr(self, '_dtype', np.float32)
-        self._X = X if np.dtype(dt) == np.float32 else X.astype(dt)
+        self._check_converged(st, 'HOPE: the solver stopped at max_iters=%d without meeting tol=%g (singular values still '
+                              'moving by %.3g per round); the embedding is less accurate than requested -- raise max_iters / '
+                              'oversample or use algorithm=3 on power-law graphs'
+                              % (st['iters'], opts.get('tol', 1e-6), st['ritz_change']))
+        self._result(X, csr.n)
         if getattr(self, '_verbose', 0):
             print('HOPE: algorithm %d, %d iterations, J=%d Katz terms, block %d, ritz change %.3g, converged %d' %
                   (st['algorithm'], st['iters'], st['katz_terms'], st['block'], st['ritz_change'], st['converged']))
         return self._X
 
-    @staticmethod
-    def _spmd():
-        """(torch.distributed module, rank, world) when the process runs under an initialised process group."""
-        if int(os.environ.get('WORLD_SIZE', '1')) <= 1:
-            return None, 0, 1
-        try:
-            import torch.distributed as dist_mod
-        except ImportError:
-            return None, 0, 1
-        if not (dist_mod.is_available() and dist_mod.is_initialized()):
-            return None, 0, 1
-        return dist_mod, dist_mod.get_rank(), dist_mod.get_world_size()
+    def _upload(self, ctx, csr, rank, world):
+        """The graph on the device: under SPMD (INTEGRATION.md C) every rank is called with the same graph, uploads
+        its row shard and returns THIS rank's rows of X; a general (non-symmetric) graph also uploads its transpose."""
+        if world == 1:
+            if csr.is_symmetric():
+                return _native.DeviceGraph(ctx, csr.n, csr.indptr, csr.indices, csr.data_f32())
+            t = csr.transpose()
+            return _native.DeviceGraph(ctx, csr.n, csr.indptr, csr.indices, csr.data_f32(),
+                                       t.indptr, t.indices, t.data_f32())
+        r0, ip, ix, dat = csr.row_shard(rank, world)
+        self._row0 = r0
+        dat = None if dat is None else dat.astype(np.float32)
+        if csr.is_symmetric():
+            return _native.DeviceGraph(ctx, csr.n, ip, ix, dat, row0=r0)
+        _, tp, tx, tdat = csr.transpose().row_shard(rank, world)
+        return _native.DeviceGraph(ctx, csr.n, ip, ix, dat, tp, tx, None if tdat is None else tdat.astype(np.float32),
+                                   row0=r0)
 
     def get_edge_weight(self, i, j):
         return np.dot(self._X[i, :self._d // 2], self._X[j, self._d // 2:])

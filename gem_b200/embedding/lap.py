@@ -12,13 +12,10 @@ Extra, optional hyper-parameters: tol (default 1e-6: relative change of every wa
 stop_rule=1 switches to the residual estimate, which fp32 Gram matrices cannot certify below ~3e-4), max_iters, oversample,
 cheb_degree, cheb_range_log2, seed, device, dtype, strict, verbose.
 `graph` may also be a scipy.sparse matrix or a gem_b200.graph.HostCSR (rows = 0..n-1)."""
-import warnings
-
 import numpy as np
 
 from gem_b200 import _native
 from gem_b200 import graph as _graph
-from gem_b200.embedding.hope import _graph_is_empty
 from gem_b200.embedding.static_graph_embedding import StaticGraphEmbedding
 
 _OPT_KEYS = ('tol', 'max_iters', 'min_iters', 'oversample', 'seed', 'verbose', 'cheb_degree', 'cheb_range_log2', 'stop_rule')
@@ -69,6 +66,22 @@ def undirected_normalised(csr):
     return out, l_fro2
 
 
+def spectral_solve(model, op, d, name):
+    """(V, lam): the d + 1 largest algebraic eigenpairs of the symmetric HostCSR `op` by the Chebyshev-filtered subspace
+    iteration of gemb_hope (spectral_mode = 1), with the model's solver options; sets model.stats and warns (raises
+    under strict) when the solver stopped unconverged."""
+    opts = {k: getattr(model, '_' + k) for k in _OPT_KEYS if hasattr(model, '_' + k)}
+    opts.setdefault('tol', 1e-6)
+    opts.setdefault('max_iters', 300)
+    with _native.Context(int(getattr(model, '_device', 0))) as ctx, \
+            _native.DeviceGraph(ctx, op.n, op.indptr, op.indices, op.data_f32()) as g:
+        V, lam, st = g.hope(d + 1, 0.0, spectral_mode=1, **opts)
+    model.stats = st
+    model._check_converged(st, '%s: the solver stopped at max_iters=%d without meeting tol=%g (eigenvalues still moving '
+                           'by %.3g per round)' % (name, st['iters'], opts['tol'], st['ritz_change']), stacklevel=4)
+    return V, lam
+
+
 class LaplacianEigenmaps(StaticGraphEmbedding):
 
     _recon_score = 'gaussian'      # get_edge_weight is exp(-|x_i - x_j|^2): reconstructed and evaluated on the GPU
@@ -87,46 +100,16 @@ class LaplacianEigenmaps(StaticGraphEmbedding):
         self.stats = None
         self._w = None
 
-    def _to_csr(self, graph):
-        if isinstance(graph, _graph.HostCSR):
-            return graph
-        if hasattr(graph, 'nodes') and hasattr(graph, 'edges'):
-            return _graph.from_networkx(graph)
-        return _graph.from_scipy(graph)
-
     def learn_embedding(self, graph=None, is_weighted=False, no_python=False, **ignored):
-        if _graph_is_empty(graph):
-            raise ValueError('graph needed')
         csr = self._to_csr(graph)
         d = int(self._d)
         if d + 1 > csr.n:
             raise ValueError('d + 1 eigenvectors asked of a %d-node graph' % csr.n)
         ahat, l_fro2 = undirected_normalised(csr)
-        opts = {k: getattr(self, '_' + k) for k in _OPT_KEYS if hasattr(self, '_' + k)}
-        opts.setdefault('tol', 1e-6)
-        opts.setdefault('max_iters', 300)
-        ctx = _native.Context(int(getattr(self, '_device', 0)))
-        try:
-            g = _native.DeviceGraph(ctx, ahat.n, ahat.indptr, ahat.indices, ahat.data_f32())
-            try:
-                V, lam, st = g.hope(d + 1, 0.0, spectral_mode=1, **opts)
-            finally:
-                g.free()
-        finally:
-            ctx.close()
-        self.stats = st
+        V, lam = spectral_solve(self, ahat, d, 'LaplacianEigenmaps')
         w = 1.0 - np.asarray(lam, dtype=np.float64)              # ascending eigenvalues of L_sym (lap.py:29-31)
         self._w = w
-        self._node_num = csr.n
-        if not st['converged']:
-            msg = ('LaplacianEigenmaps: the solver stopped at max_iters=%d without meeting tol=%g (eigenvalues still moving by %.3g per round)'
-                   % (st['iters'], opts['tol'], st['ritz_change']))
-            if getattr(self, '_strict', False):
-                raise RuntimeError(msg)
-            warnings.warn(msg, RuntimeWarning, stacklevel=2)
-        dt = getattr(self, '_dtype', np.float32)
-        X = V[:, 1:]
-        self._X = np.ascontiguousarray(X if np.dtype(dt) == np.float32 else X.astype(dt))
+        self._result(V[:, 1:], csr.n)
         # lap.py:34-36: || V diag(w) V^T - L_sym ||_F; with orthonormal eigenvectors that is sqrt(||L_sym||_F^2 - sum w_i^2)
         eig_err = float(np.sqrt(max(l_fro2 - float(np.sum(w * w)), 0.0)))
         self._eig_err = eig_err

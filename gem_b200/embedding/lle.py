@@ -12,17 +12,11 @@ host (scipy.sparse product P^T P, sum_v deg(v)^2 entries -- fine for bounded deg
 two fused sweeps inside the solver instead is the next step (DESIGN.md section 9).  No CPU path for the solve.
 
 Extra, optional hyper-parameters: tol (default 1e-6), max_iters, oversample, cheb_degree, cheb_range_log2, seed, device, dtype, strict."""
-import warnings
-
 import numpy as np
 
-from gem_b200 import _native
 from gem_b200 import graph as _graph
-from gem_b200.embedding.hope import _graph_is_empty
-from gem_b200.embedding.lap import undirected_coo
+from gem_b200.embedding.lap import spectral_solve, undirected_coo
 from gem_b200.embedding.static_graph_embedding import StaticGraphEmbedding
-
-_OPT_KEYS = ('tol', 'max_iters', 'min_iters', 'oversample', 'seed', 'verbose', 'cheb_degree', 'cheb_range_log2', 'stop_rule')
 
 
 def lle_operator(csr):
@@ -62,46 +56,15 @@ class LocallyLinearEmbedding(StaticGraphEmbedding):
         self.stats = None
         self._s = None
 
-    def _to_csr(self, graph):
-        if isinstance(graph, _graph.HostCSR):
-            return graph
-        if hasattr(graph, 'nodes') and hasattr(graph, 'edges'):
-            return _graph.from_networkx(graph)
-        return _graph.from_scipy(graph)
-
     def learn_embedding(self, graph=None, is_weighted=False, no_python=False, **ignored):
-        if _graph_is_empty(graph):
-            raise ValueError('graph needed')
         csr = self._to_csr(graph)
         d = int(self._d)
         if d + 1 > csr.n:
             raise ValueError('d + 1 singular vectors asked of a %d-node graph' % csr.n)
         C, c = lle_operator(csr)
-        opts = {k: getattr(self, '_' + k) for k in _OPT_KEYS if hasattr(self, '_' + k)}
-        opts.setdefault('tol', 1e-6)
-        opts.setdefault('max_iters', 300)
-        ctx = _native.Context(int(getattr(self, '_device', 0)))
-        try:
-            g = _native.DeviceGraph(ctx, C.n, C.indptr, C.indices, C.data_f32())
-            try:
-                V, lam, st = g.hope(d + 1, 0.0, spectral_mode=1, **opts)
-            finally:
-                g.free()
-        finally:
-            ctx.close()
-        self.stats = st
+        V, lam = spectral_solve(self, C, d, 'LocallyLinearEmbedding')
         self._s = np.sqrt(np.maximum(c - np.asarray(lam, dtype=np.float64), 0.0))     # ascending singular values of I - P
-        self._node_num = csr.n
-        if not st['converged']:
-            msg = ('LocallyLinearEmbedding: the solver stopped at max_iters=%d without meeting tol=%g (eigenvalues still moving by '
-                   '%.3g per round)' % (st['iters'], opts['tol'], st['ritz_change']))
-            if getattr(self, '_strict', False):
-                raise RuntimeError(msg)
-            warnings.warn(msg, RuntimeWarning, stacklevel=2)
-        dt = getattr(self, '_dtype', np.float32)
-        X = V[:, 1:]
-        self._X = np.ascontiguousarray(X if np.dtype(dt) == np.float32 else X.astype(dt))
-        return self._X
+        return self._result(V[:, 1:], csr.n)
 
     def get_edge_weight(self, i, j):
         return np.exp(

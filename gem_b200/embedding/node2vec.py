@@ -16,11 +16,10 @@ Extra optional hyper-parameters: seed (the binary uses time(NULL); default 1), d
 sequential (parity mode: one warp follows the single-threaded binary's RNG stream), dtype.
 There is no CPU path: without a GPU learn_embedding raises RuntimeError.
 """
-import os
-
 import numpy as np
 
 from gem_b200 import _native
+from gem_b200 import dist as _gd
 from gem_b200 import graph as _graph
 from gem_b200.embedding.static_graph_embedding import StaticGraphEmbedding
 
@@ -48,40 +47,25 @@ class node2vec(StaticGraphEmbedding):
         self.stats = None
 
     def learn_embedding(self, graph=None, is_weighted=False, no_python=False, **ignored):
-        if graph is None or (hasattr(graph, '__len__') and len(graph) == 0):
-            raise ValueError('graph needed')
+        self._check_graph(graph)
         if isinstance(graph, tuple):          # (HostCSR, nids): large inputs without networkx
             csr, nids = graph
         else:
             csr, nids = _graph.n2v_inputs_from_networkx(graph)
-        from gem_b200.embedding.hope import HOPE as _H
-        dist_mod, rank, world = _H._spmd()
-        device = getattr(self, '_device', None)
-        if device is None:
-            device = int(os.environ.get('LOCAL_RANK', '0')) if world > 1 else 0
-        ctx = _native.Context(device)
-        try:
+        dist_mod, rank, world, device = _gd.spmd(getattr(self, '_device', None))
+        with _native.Context(device) as ctx:
             if world > 1:
                 # SPMD (INTEGRATION.md C): every rank holds the whole graph, walks its share of the walk index space and
                 # trains on it; the embedding deltas are all-reduced once per epoch, so every rank returns the same X
-                from gem_b200 import dist as _gd
                 _gd.init_comm_from_torch(ctx, dist_mod, rank, world)
-            g = _native.DeviceGraph(ctx, csr.n, csr.indptr, csr.indices, None)
-            try:
+            with _native.DeviceGraph(ctx, csr.n, csr.indptr, csr.indices, None) as g:
                 X, st = g.node2vec(nids, int(self._d), int(self._walk_len), int(self._num_walks),
                                    int(self._con_size), int(self._max_iter), float(self._ret_p),
                                    float(self._inout_p), seed=int(getattr(self, '_seed', 1)),
                                    sequential=bool(getattr(self, '_sequential', False)),
                                    n_rows=csr.n, weights64=csr.data)
-            finally:
-                g.free()
-        finally:
-            ctx.close()
         self.stats = st
-        self._node_num = csr.n
-        dt = getattr(self, '_dtype', np.float32)
-        self._X = X if np.dtype(dt) == np.float32 else X.astype(dt)
-        return self._X
+        return self._result(X, csr.n)
 
     def get_edge_weight(self, i, j):
         return np.dot(self._X[i, :], self._X[j, :])

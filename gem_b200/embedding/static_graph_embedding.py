@@ -6,9 +6,26 @@ halves, hope.py:43-44; False: dot product, node2vec.py:56-57) or `_recon_score =
 (exp(-|x_i - x_j|^2), lap.py:39-42 / lle.py:37-40) gets the matrix from the GPU (gemb_recon_create /
 gemb_recon_dense, fp32 arithmetic, returned as fp64 with a zero diagonal); there is no CPU path for it -- without a
 GPU it raises RuntimeError."""
+import warnings
 from abc import ABC, abstractmethod
 
 import numpy as np
+
+from gem_b200 import graph as _graph
+
+
+def _graph_is_empty(graph):
+    """`if not graph` of the reference for every accepted input type, checked in this order: HostCSR (.n), anything with
+    a .shape (scipy sparse matrices AND arrays raise TypeError from __len__), then len() (networkx graphs, tuples)."""
+    if graph is None:
+        return True
+    if isinstance(graph, _graph.HostCSR):
+        return graph.n == 0
+    if hasattr(graph, 'shape'):
+        return graph.shape[0] == 0
+    if hasattr(graph, '__len__'):
+        return len(graph) == 0
+    return False
 
 
 def recon_kind(model):
@@ -52,6 +69,37 @@ class StaticGraphEmbedding(ABC):
     def get_method_summary(self):
         return '{}_{:d}'.format(self._method_name, self._d)
 
+    # -- steps shared by the learn_embedding of the subclasses
+    @staticmethod
+    def _check_graph(graph):
+        if _graph_is_empty(graph):
+            raise ValueError('graph needed')
+
+    def _to_csr(self, graph):
+        """The input step: the empty-graph guard, then a HostCSR of a HostCSR, networkx graph or scipy.sparse matrix."""
+        self._check_graph(graph)
+        if isinstance(graph, _graph.HostCSR):
+            return graph
+        if hasattr(graph, 'nodes') and hasattr(graph, 'edges'):
+            return _graph.from_networkx(graph)
+        return _graph.from_scipy(graph)
+
+    def _check_converged(self, stats, msg, stacklevel=3):
+        """A solver that stopped unconverged raises RuntimeError(msg) under `strict` and warns otherwise.  stacklevel
+        counts the frames from here up to the line that called learn_embedding, which the warning points at."""
+        if stats['converged']:
+            return
+        if getattr(self, '_strict', False):
+            raise RuntimeError(msg)
+        warnings.warn(msg, RuntimeWarning, stacklevel=stacklevel)
+
+    def _result(self, X, node_num):
+        """The result step: X in the requested dtype (default float32, returned as it is), C-contiguous; the node count."""
+        self._node_num = node_num
+        dt = np.dtype(getattr(self, '_dtype', np.float32))
+        self._X = X if X.dtype == dt and X.flags.c_contiguous else np.ascontiguousarray(X, dtype=dt)
+        return self._X
+
     def get_reconstructed_adj(self, X=None, node_l=None):
         """A_hat[i, j] = get_edge_weight(i, j) off the diagonal, 0 on it (reference :48-65).  As there, a given X
         replaces the stored embedding and `node_l` is accepted but unused."""
@@ -67,17 +115,10 @@ class StaticGraphEmbedding(ABC):
             return np.array([[0.0 if i == j else score(i, j) for j in range(rows)] for i in range(rows)],
                             dtype=np.float64).reshape(rows, rows)
         from gem_b200 import _native
-        ctx = _native.Context(getattr(self, '_device', 0))
-        try:
-            rec = _native.Reconstruction(ctx, np.asarray(self._X)[:rows], kind)
-            try:
-                if kind == _native.RECON_GAUSS:
-                    return np.exp(-rec.dense().astype(np.float64))     # delta is +inf on the diagonal: exp gives 0
-                return rec.dense().astype(np.float64)
-            finally:
-                rec.free()
-        finally:
-            ctx.close()
+        with _native.Context(getattr(self, '_device', 0)) as ctx, \
+                _native.Reconstruction(ctx, np.asarray(self._X)[:rows], kind) as rec:
+            A = rec.dense().astype(np.float64)
+        return np.exp(-A) if kind == _native.RECON_GAUSS else A     # delta is +inf on the diagonal: exp gives 0
 
     @abstractmethod
     def learn_embedding(self, graph):

@@ -60,102 +60,56 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
     if X.shape[0] != node_num:
         raise ValueError('embedding has %d rows, graph has %d nodes' % (X.shape[0], node_num))
     indptr, indices = _true_csr(digraph, node_num)
-    keys = np.repeat(np.arange(node_num, dtype=np.int64), np.diff(indptr)) * node_num + indices
-
-    def has_edge(i, j):
-        if keys.size == 0:
-            return np.zeros(np.shape(i), dtype=bool)
-        q = np.asarray(i, dtype=np.int64) * node_num + np.asarray(j, dtype=np.int64)
-        pos = np.minimum(np.searchsorted(keys, q), keys.size - 1)
-        return keys[pos] == q
-
+    has_edge = metrics.csr_has_edge(node_num, indptr, indices)
     dev = device if device is not None else getattr(graph_embedding, '_device', 0)
-    ctx = _native.Context(dev)
-    try:
-        rec = _native.Reconstruction(ctx, X, kind)
-        try:
-            if sample_ratio_e:
-                # evaluation_util.py:5-18 + :25-28: random pairs, kept when A_hat >= 0
-                from gem_b200.utils import evaluation_util
-                pairs = np.array(evaluation_util.get_random_edge_pairs(node_num, sample_ratio_e, is_undirected),
-                                 dtype=np.int64).reshape(-1, 2)
-                w = rec.pairs(pairs[:, 0], pairs[:, 1])
-                if gauss:
-                    # exp(-delta) >= 0 keeps every pair; ordering by -delta (exact) is ordering by the score
-                    keep = np.ones(w.shape, dtype=bool)
-                    w = -w
-                else:
-                    keep = w >= 0.0
-                pi, pj, pw = pairs[keep, 0], pairs[keep, 1], w[keep]
-                MAP, _, _ = _map_of_list(node_num, pi, pj, pw, indptr, has_edge, is_undirected)
-                order = np.argsort(-pw.astype(np.float64), kind='stable')
-                delta = has_edge(pi[order], pj[order]).astype(np.float64)
-                prec_curv = (np.cumsum(delta) / np.arange(1, order.size + 1)).tolist()
+    with _native.Context(dev) as ctx, _native.Reconstruction(ctx, X, kind) as rec:
+        if sample_ratio_e:
+            # evaluation_util.py:5-18 + :25-28: random pairs, kept when A_hat >= 0
+            from gem_b200.utils import evaluation_util
+            pairs = np.array(evaluation_util.get_random_edge_pairs(node_num, sample_ratio_e, is_undirected),
+                             dtype=np.int64).reshape(-1, 2)
+            w = rec.pairs(pairs[:, 0], pairs[:, 1])
+            if gauss:
+                # exp(-delta) >= 0 keeps every pair; ordering by -delta (exact) is ordering by the score
+                keep = np.ones(w.shape, dtype=bool)
+                w = -w
             else:
-                ranks, _ = rec.ranks(indptr, indices, is_undirected)
-                MAP, _, _ = metrics.map_from_ranks(node_num, indptr, ranks, is_undirected)
-                ti, tj, tw = rec.top(is_undirected, max_k)
-                if gauss:
-                    tw = -tw                              # delta ascending = -delta descending
-                prec_curv, _ = metrics.precision_curve_from_top(ti, tj, tw, has_edge, max_k)
-            if is_weighted:
-                # :37-40 -- nx.to_numpy_matrix(digraph) has rows/columns in list(digraph.nodes) order while the
-                # reconstruction is indexed by node id; edge (u -> v) is therefore compared with A_hat[pos u][pos v]
-                if isinstance(digraph, HostCSR):                  # rows already in id order
-                    pos = np.arange(node_num, dtype=np.int64)
-                    eu = np.repeat(np.arange(node_num, dtype=np.int64), np.diff(indptr))
-                    ev = indices
-                    a = np.ones(ev.size) if digraph.data is None else np.asarray(digraph.data, dtype=np.float64)
-                else:
-                    pos = np.empty(node_num, dtype=np.int64)
-                    pos[np.array([int(u) for u in digraph.nodes], dtype=np.int64)] = np.arange(node_num)
-                    ed = [(int(u), int(v), float(wt)) for u, v, wt in digraph.edges(data='weight', default=1)]
-                    if not digraph.is_directed():             # nx.to_numpy_matrix of an nx.Graph is symmetric
-                        ed = ed + [(v, u, wt) for u, v, wt in ed if u != v]
-                    eu = np.array([t[0] for t in ed], dtype=np.int64)
-                    ev = np.array([t[1] for t in ed], dtype=np.int64)
-                    a = np.array([t[2] for t in ed], dtype=np.float64)
-                est = rec.pairs(pos[eu], pos[ev]).astype(np.float64)
-                if gauss:
-                    est = np.exp(-est)
-                nz = a != 0
-                err = float(np.sqrt(np.sum((a[nz] - est[nz]) ** 2)))
-                err_baseline = float(np.sqrt(np.sum(a ** 2)))
+                keep = w >= 0.0
+            pi, pj, pw = pairs[keep, 0], pairs[keep, 1], w[keep]
+            total, count = metrics.node_ap_sum(node_num, pi, pj, pw, has_edge, np.diff(indptr), is_undirected)
+            MAP = total / count if count else float('nan')
+            prec_curv, _ = metrics.precision_curve(pi, pj, pw, has_edge)
+        else:
+            ranks, _ = rec.ranks(indptr, indices, is_undirected)
+            MAP, _, _ = metrics.map_from_ranks(node_num, indptr, ranks, is_undirected)
+            ti, tj, tw = rec.top(is_undirected, max_k)
+            if gauss:
+                tw = -tw                              # delta ascending = -delta descending
+            prec_curv, _ = metrics.precision_curve_from_top(ti, tj, tw, has_edge, max_k)
+        if is_weighted:
+            # :37-40 -- nx.to_numpy_matrix(digraph) has rows/columns in list(digraph.nodes) order while the
+            # reconstruction is indexed by node id; edge (u -> v) is therefore compared with A_hat[pos u][pos v]
+            if isinstance(digraph, HostCSR):                  # rows already in id order
+                pos = np.arange(node_num, dtype=np.int64)
+                eu = np.repeat(np.arange(node_num, dtype=np.int64), np.diff(indptr))
+                ev = indices
+                a = np.ones(ev.size) if digraph.data is None else np.asarray(digraph.data, dtype=np.float64)
             else:
-                err = None
-                err_baseline = None
-        finally:
-            rec.free()
-    finally:
-        ctx.close()
+                pos = np.empty(node_num, dtype=np.int64)
+                pos[np.array([int(u) for u in digraph.nodes], dtype=np.int64)] = np.arange(node_num)
+                ed = [(int(u), int(v), float(wt)) for u, v, wt in digraph.edges(data='weight', default=1)]
+                if not digraph.is_directed():             # nx.to_numpy_matrix of an nx.Graph is symmetric
+                    ed = ed + [(v, u, wt) for u, v, wt in ed if u != v]
+                eu = np.array([t[0] for t in ed], dtype=np.int64)
+                ev = np.array([t[1] for t in ed], dtype=np.int64)
+                a = np.array([t[2] for t in ed], dtype=np.float64)
+            est = rec.pairs(pos[eu], pos[ev]).astype(np.float64)
+            if gauss:
+                est = np.exp(-est)
+            nz = a != 0
+            err = float(np.sqrt(np.sum((a[nz] - est[nz]) ** 2)))
+            err_baseline = float(np.sqrt(np.sum(a ** 2)))
+        else:
+            err = None
+            err_baseline = None
     return MAP, prec_curv, err, err_baseline
-
-
-def _map_of_list(node_num, pi, pj, pw, indptr, has_edge, is_undirected):
-    """computeMAP (metrics.py:28-46) of an explicit, small predicted-edge list (the sampled-pairs branch)."""
-    order = np.argsort(pi, kind='stable')
-    pi, pj, pw = pi[order], pj[order], pw[order]
-    starts = np.searchsorted(pi, np.arange(node_num + 1))
-    outdeg = np.diff(indptr)
-    node_ap = [0.0] * node_num
-    count = 0
-    for v in range(node_num):
-        if not is_undirected and outdeg[v] == 0:
-            continue
-        count += 1
-        s, e = starts[v], starts[v + 1]
-        if e == s:
-            continue
-        o = np.argsort(-pw[s:e].astype(np.float64), kind='stable')
-        delta = has_edge(pi[s:e][o], pj[s:e][o]).astype(np.float64)
-        prec = np.cumsum(delta) / np.arange(1, e - s + 1)
-        sp = 0.0
-        sd = 0.0
-        for p, dl in zip(prec.tolist(), delta.tolist()):
-            sp += p * dl
-            sd += dl
-        node_ap[v] = 0.0 if sd == 0 else float(sp / sd)
-    total = 0.0
-    for a in node_ap:
-        total += a
-    return (total / count if count else float('nan')), node_ap, count

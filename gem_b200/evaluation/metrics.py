@@ -49,22 +49,67 @@ def precision_curve_from_top(i, j, w, has_edge, max_k=-1):
     return prec.tolist(), delta.tolist()
 
 
+def csr_has_edge(n, indptr, indices):
+    """Vectorised has_edge(i, j) of an n-node CSR graph whose rows hold sorted column ids: a binary search of the
+    sorted keys i * n + j."""
+    keys = np.repeat(np.arange(n, dtype=np.int64), np.diff(indptr)) * n + np.asarray(indices, dtype=np.int64)
+
+    def has_edge(i, j):
+        if keys.size == 0:
+            return np.zeros(np.shape(i), dtype=bool)
+        q = np.asarray(i, dtype=np.int64) * n + np.asarray(j, dtype=np.int64)
+        pos = np.minimum(np.searchsorted(keys, q), keys.size - 1)
+        return keys[pos] == q
+    return has_edge
+
+
+def precision_curve(i, j, w, has_edge, max_k=-1):
+    """metrics.py:6-24 on an explicit predicted-edge list (arrays i, j, w in list order): precision@1..max_k of the list
+    sorted by weight (descending, stable).  -> (precision_scores, delta_factors) as python lists"""
+    max_k = i.size if max_k == -1 else min(max_k, i.size)
+    order = np.argsort(-np.asarray(w, dtype=np.float64), kind='stable')[:max_k]
+    delta = has_edge(i[order], j[order]).astype(np.float64) if max_k else np.zeros(0)
+    prec = np.cumsum(delta) / np.arange(1, max_k + 1, dtype=np.float64)
+    return prec.tolist(), delta.tolist()
+
+
+def node_ap_sum(node_num, i, j, w, has_edge, outdeg, is_undirected, max_k=-1):
+    """metrics.py:28-46 on an explicit predicted-edge list (arrays i, j, w in list order): the average precision of
+    each node's edges (list order, sorted by weight descending and stable, cut at max_k), nodes without out-edges
+    skipped unless is_undirected.  -> (sum of the APs in node order, number of nodes counted); MAP = sum / count."""
+    order = np.argsort(i, kind='stable')                      # node_edges[st].append(...) keeps list order per node
+    i, j, w = i[order], j[order], np.asarray(w, dtype=np.float64)[order]
+    starts = np.searchsorted(i, np.arange(node_num + 1))
+    total = 0.0
+    count = 0
+    for v in range(node_num):
+        if not is_undirected and outdeg[v] == 0:
+            continue
+        count += 1
+        s, e = int(starts[v]), int(starts[v + 1])
+        k = e - s if max_k == -1 else min(max_k, e - s)
+        if k == 0:
+            continue
+        o = np.argsort(-w[s:e], kind='stable')[:k]
+        delta = has_edge(i[s:e][o], j[s:e][o]).astype(np.float64)
+        prec = np.cumsum(delta) / np.arange(1, k + 1, dtype=np.float64)
+        sp = sd = 0.0
+        for p, dl in zip(prec.tolist(), delta.tolist()):      # sum(precision_rectified), sum(delta_factors): sequential
+            sp += p * dl
+            sd += dl
+        if sd != 0:
+            total += float(sp / sd)
+    return total, count
+
+
 # ---- the reference's own entry points (gem/evaluation/metrics.py:6-46), same names, arguments and results, for
 # callers that already hold an explicit predicted edge list [(st, ed, w), ...].  The list sorts are NumPy stable
 # argsorts (= Python's stable sorted(..., reverse=True) on the weight), the sums run in the reference's order.
 def _has_edge_fn(true_digraph):
     from gem_b200.graph import HostCSR
     if isinstance(true_digraph, HostCSR):
-        n = true_digraph.n
-        keys = np.repeat(np.arange(n, dtype=np.int64), np.diff(true_digraph.indptr)) * n + true_digraph.indices
-
-        def has_edge(i, j):
-            if keys.size == 0:
-                return np.zeros(np.shape(i), dtype=bool)
-            q = np.asarray(i, dtype=np.int64) * n + np.asarray(j, dtype=np.int64)
-            pos = np.minimum(np.searchsorted(keys, q), keys.size - 1)
-            return keys[pos] == q
-        return has_edge, n, np.diff(true_digraph.indptr)
+        outdeg = np.diff(true_digraph.indptr)
+        return csr_has_edge(true_digraph.n, true_digraph.indptr, true_digraph.indices), true_digraph.n, outdeg
     n = len(true_digraph.nodes)
     he = true_digraph.has_edge
 
@@ -87,40 +132,11 @@ def _edge_arrays(predicted_edge_list):
 def computePrecisionCurve(predicted_edge_list, true_digraph, max_k=-1):
     """metrics.py:6-24: precision@1..max_k of the edge list sorted by weight (descending, stable)."""
     has_edge, _, _ = _has_edge_fn(true_digraph)
-    i, j, w = _edge_arrays(predicted_edge_list)
-    max_k = i.size if max_k == -1 else min(max_k, i.size)
-    order = np.argsort(-w, kind='stable')[:max_k]
-    delta = has_edge(i[order], j[order]).astype(np.float64) if max_k else np.zeros(0)
-    prec = np.cumsum(delta) / np.arange(1, max_k + 1, dtype=np.float64)
-    return prec.tolist(), delta.tolist()
+    return precision_curve(*_edge_arrays(predicted_edge_list), has_edge, max_k)
 
 
 def computeMAP(predicted_edge_list, true_digraph, max_k=-1, is_undirected=False):
     """metrics.py:27-46: mean over the counted nodes of the average precision of each node's predicted edges."""
     has_edge, node_num, outdeg = _has_edge_fn(true_digraph)
-    i, j, w = _edge_arrays(predicted_edge_list)
-    order = np.argsort(i, kind='stable')                      # node_edges[st].append(...) keeps list order per node
-    i, j, w = i[order], j[order], w[order]
-    starts = np.searchsorted(i, np.arange(node_num + 1))
-    node_ap = [0.0] * node_num
-    count = 0
-    for v in range(node_num):
-        if not is_undirected and outdeg[v] == 0:
-            continue
-        count += 1
-        s, e = int(starts[v]), int(starts[v + 1])
-        k = e - s if max_k == -1 else min(max_k, e - s)
-        if k == 0:
-            continue
-        o = np.argsort(-w[s:e], kind='stable')[:k]
-        delta = has_edge(i[s:e][o], j[s:e][o]).astype(np.float64)
-        prec = np.cumsum(delta) / np.arange(1, k + 1, dtype=np.float64)
-        sp = sd = 0.0
-        for p, dl in zip(prec.tolist(), delta.tolist()):      # sum(precision_rectified), sum(delta_factors): sequential
-            sp += p * dl
-            sd += dl
-        node_ap[v] = 0 if sd == 0 else float(sp / sd)
-    total = 0.0
-    for a in node_ap:
-        total += a
+    total, count = node_ap_sum(node_num, *_edge_arrays(predicted_edge_list), has_edge, outdeg, is_undirected, max_k)
     return total / count

@@ -136,7 +136,7 @@ def test_graph_and_reconstruction_lifetimes(gpu_ctx, sbm):
     assert _live() == before
     n = 700
     X = np.abs(np.random.default_rng(5).standard_normal((n, 16))).astype(np.float32)
-    r = _native.Reconstruction(gpu_ctx, X, split=True)
+    r = _native.Reconstruction(gpu_ctx, X, kind=_native.RECON_SPLIT)
     r.dense()
     r.pairs(np.arange(10), np.arange(10, 20))
     nbr = np.stack(((np.arange(n) + 1) % n, (np.arange(n) + 7) % n), axis=1)
@@ -181,7 +181,7 @@ def test_upload_with_out_of_range_column(gpu_ctx, sbm):
 def test_recon_top_with_too_small_cap(gpu_ctx):
     from gem_b200 import _native
     X = np.abs(np.random.default_rng(7).standard_normal((300, 16))).astype(np.float32)
-    r = _native.Reconstruction(gpu_ctx, X, split=True)
+    r = _native.Reconstruction(gpu_ctx, X, kind=_native.RECON_SPLIT)
     try:
         i, j, w = (np.empty(1, dtype=t) for t in (np.int32, np.int32, np.float32))
         m = ctypes.c_int64(0)

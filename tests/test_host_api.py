@@ -170,7 +170,8 @@ def test_synthetic_generators_match_the_survey_configs():
 def test_scipy_inputs_get_past_the_empty_graph_guard():
     """ADVICE r1: scipy sparse matrices AND arrays raise TypeError from len(); the guard must look at .shape first."""
     import scipy.sparse as sp
-    from gem_b200.embedding.hope import HOPE, _graph_is_empty
+    from gem_b200.embedding.hope import HOPE
+    from gem_b200.embedding.static_graph_embedding import _graph_is_empty
     from gem_b200.graph import HostCSR
     A = sp.random(12, 12, 0.3, format='csr', random_state=0)
     for M in (A, sp.csr_array(A), sp.coo_matrix(A)):

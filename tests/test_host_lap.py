@@ -100,6 +100,8 @@ def test_gf_schedule_choice(monkeypatch):
     class FakeCtx:
         def __init__(self, device=0): pass
         def close(self): pass
+        def __enter__(self): return self
+        def __exit__(self, *exc): self.close()
 
     def fake_gf(ctx, n, src, dst, w, d, eta, regu, max_iter, X0, mode=0):
         calls.append((mode, src.tolist()))
