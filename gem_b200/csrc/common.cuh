@@ -224,7 +224,8 @@ int apply_fp32_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const fl
                       float *Out, int ldo);
 // Small b x b factorizations, single CTA, fp64 (device pointers):
 //  chol_inverse: G (b x b, SPD up to rank deficiency) -> Minv fp32 (b x b) with G = R^T R, Minv = R^-1
-//  (columns whose pivot falls below eps*max are zeroed: Q*Minv then has zero columns there).
+//  (columns whose pivot of the unit-diagonal scaled G falls below GEMB_PIV_EPS are zeroed: Q*Minv then has zero columns
+//  there).  G is overwritten where the matrix does not fit in shared memory (b > 168 on H100).
 int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_out_dev, double *Minv64 = nullptr);
 //  C (fp64) and/or C32 (fp32) = op(A) * B for b x b fp64 matrices (one CTA)
 int small_gemm_launch(gemb_ctx *ctx, int b, const double *A, int transA, const double *B, double *C, float *C32);
@@ -235,7 +236,8 @@ int gram_tc_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float
 // out[i] = sum_{c < parts} part[c * count + i] is added in a fixed order, so a result is the same on every run.
 int red_scratch(gemb_ctx *ctx, size_t doubles, double **out);
 int sum_partials_launch(gemb_ctx *ctx, int parts, int64_t count, const double *part, double *out);
-//  eigh: G -> eigenvalues w ascending (b), eigenvectors Z (b x b, column j <-> w[j]); G destroyed.
+//  eigh: G -> eigenvalues w ascending (b), eigenvectors Z (b x b, column j <-> w[j]); G destroyed where the matrix does
+//  not fit in shared memory (b >= 168).
 // rel_tol: stop the Jacobi sweeps when ||offdiag||_F <= rel_tol * ||G||_F
 int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch /* b x b */, double rel_tol = 1e-11);
 int randn_launch(gemb_ctx *ctx, int64_t n, int b, uint64_t seed, uint64_t row_offset, float *X);

@@ -2,7 +2,8 @@
 //
 //   gram   : G = P^T Q      (n x b1, n x b2 -> b1 x b2), the CholeskyQR / Rayleigh-Ritz contraction
 //   apply  : Out = Q * M    (n x b1 times b1 x b2)
-//   chol_inverse, eigh : single-CTA fp64 factorizations of the b x b matrices
+//   chol_inverse, eigh : single-CTA fp64 factorizations of the b x b matrices, one kernel each; the working matrices
+//                        live in shared memory where they fit and in global memory (L2 resident) beyond
 // These replace numpy.linalg.qr / svd inside scipy's svds (hope.py:33 -> _svds.py:508-533).
 // fp32 data, fp32 FMA inside a CTA's partial sums, fp64 across CTAs and in the b x b algebra.
 #include "common.cuh"
@@ -255,123 +256,38 @@ int apply_fp32_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const fl
 // scale free.  A pivot below PIV_EPS marks the column numerically dependent: its column of Minv is
 // zero (the orthonormalised block then carries a zero column, which stays zero under S).
 #define GEMB_PIV_EPS 1e-5
-// SMEM: the b x b matrix lives in shared memory for the whole factorization (b <= 166).
+// Two block barriers per Cholesky column (the <= 3 warps that own the column compute the pivot themselves), and the
+// triangular inverse without block barriers -- each column of L^-1 belongs to 8 lanes of one warp that split the dot
+// products.  Index walks are division free.  Since b <= 1024, one thread per row of a column of L.
+// SMEM: the scaled matrix lives in shared memory with an odd leading dimension (column walks are bank-conflict free),
+// and G is only read.  Otherwise the kernel works in place in G (leading dimension b) and overwrites it.
 // Gg is not __restrict__: without SMEM it is the work matrix that other threads write between barriers, and with
-// __restrict__ nvcc kept the pivot G[j][j] that every thread loaded before thread 0 replaced it by sqrt(G[j][j]) across
-// the barrier (all entries of a column of L but the first below the diagonal were divided by the pivot, not its root).
+// __restrict__ nvcc once kept a pivot G[j][j] that every thread had loaded before another thread replaced it by its
+// root across the barrier (a column of L was divided by the pivot, not its root).
 template <bool SMEM>
 __global__ void __launch_bounds__(1024)
 chol_inverse_kernel(int b, double *Gg, float *__restrict__ Minv, double *__restrict__ Minv64,
                     int *__restrict__ rank_out) {
     extern __shared__ double sh[];
+    const int ld = SMEM ? (b | 1) : b;
     double *dscale = sh;           // b : 1/sqrt(G_jj) (0 if G_jj <= 0)
-    double *keep = sh + b;         // b : 1.0 if column j kept, 0.0 if numerically dependent
-    double *xdiag = sh + 2 * b;    // b
-    double *G = SMEM ? sh + 3 * b : Gg;
-    __shared__ int s_rank;
-    const int tid = threadIdx.x, nt = blockDim.x;
-    if (SMEM) {
-        for (int idx = tid; idx < b * b; idx += nt) G[idx] = Gg[idx];
-        __syncthreads();
-    }
-    for (int j = tid; j < b; j += nt) {
-        const double d = G[(size_t)j * b + j];
-        dscale[j] = d > 0.0 ? rsqrt(d) : 0.0;
-    }
-    if (tid == 0) s_rank = 0;
-    __syncthreads();
-    for (int idx = tid; idx < b * b; idx += nt) {
-        const int i = idx / b, j = idx - i * b;
-        G[idx] = G[idx] * dscale[i] * dscale[j];
-    }
-    __syncthreads();
-    // right-looking Cholesky on the lower triangle: L overwrites G (lower)
-    for (int j = 0; j < b; j++) {
-        if (tid == 0) {
-            const double d = G[(size_t)j * b + j];
-            if (d > GEMB_PIV_EPS) {
-                G[(size_t)j * b + j] = sqrt(d);
-                keep[j] = 1.0;
-                s_rank++;
-            } else {
-                G[(size_t)j * b + j] = 0.0;
-                keep[j] = 0.0;
-            }
-        }
-        __syncthreads();
-        const double ljj = G[(size_t)j * b + j];
-        const double inv = ljj > 0.0 ? 1.0 / ljj : 0.0;
-        for (int i = j + 1 + tid; i < b; i += nt) G[(size_t)i * b + j] *= inv;
-        __syncthreads();
-        // trailing update of the lower triangle: G[i][k] -= L[i][j] * L[k][j], j < k <= i
-        const int m = b - j - 1;
-        for (int idx = tid; idx < m * m; idx += nt) {
-            const int ii = idx / m, kk = idx - ii * m;
-            if (kk <= ii) {
-                const int i = j + 1 + ii, k = j + 1 + kk;
-                G[(size_t)i * b + k] -= G[(size_t)i * b + j] * G[(size_t)k * b + j];
-            }
-        }
-        __syncthreads();
-    }
-    // R^-1 = D^-1/2 * L^-T.  Column c of L^-1 by forward substitution (one warp per column, the dot
-    // products split across lanes); x_i (i > c) is kept in the free strict upper triangle G[c][i].
-    const int lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
-    for (int c = warp; c < b; c += nwarps) {
-        const bool okc = keep[c] != 0.0;
-        const double xc = okc ? 1.0 / G[(size_t)c * b + c] : 0.0;
-        if (lane == 0) xdiag[c] = xc;
-        for (int i = c + 1; i < b; i++) {
-            double s = 0.0;
-            if (okc && keep[i] != 0.0) {
-                for (int k = c + 1 + lane; k < i; k += 32) s += G[(size_t)i * b + k] * G[(size_t)c * b + k];
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-                s += G[(size_t)i * b + c] * xc;
-                s = -s / G[(size_t)i * b + i];
-            }
-            __syncwarp();
-            if (lane == 0) G[(size_t)c * b + i] = s;  // (L^-1)[i][c]
-            __syncwarp();
-        }
-    }
-    __syncthreads();
-    for (int idx = tid; idx < b * b; idx += nt) {
-        const int r = idx / b, c = idx - r * b;  // Minv[r][c] = dscale[r] * (L^-1)[c][r], r <= c
-        double v = 0.0;
-        if (r == c) v = xdiag[r] * dscale[r];
-        else if (r < c) v = G[(size_t)r * b + c] * dscale[r];
-        Minv[idx] = (float)v;
-        if (Minv64) Minv64[idx] = v;
-    }
-    if (tid == 0 && rank_out) *rank_out = s_rank;
-}
-
-// Fast variant (b*b fp64 fits in shared memory): two block barriers per Cholesky column (the <= 3 warps that own
-// the column compute the pivot themselves), and the triangular inverse without block barriers -- each column
-// of L^-1 belongs to 8 lanes of one warp that split the dot products.  ~4x faster than the generic kernel
-// (0.21 ms -> measured below) for b = 80; same arithmetic (fp64), same pivot rule.
-__global__ void __launch_bounds__(1024)
-chol_inverse_fast_kernel(int b, const double *__restrict__ Gg, float *__restrict__ Minv, double *__restrict__ Minv64,
-                         int *__restrict__ rank_out) {
-    extern __shared__ double sh[];
-    const int ld = b | 1;          // odd leading dimension: column walks are bank-conflict free
-    double *dscale = sh;           // b
     double *ldiag = sh + b;        // b : L_jj (0 if the column was dropped)
     double *colj = sh + 2 * b;     // b : scaled column j of L
-    double *G = sh + 3 * b;        // b x ld
+    double *G = SMEM ? sh + 3 * b : Gg;   // b x ld
+    const double *__restrict__ Gin = Gg;  // read only, and only when SMEM: its loads may take the read-only data path
     const int tid = threadIdx.x, nt = blockDim.x;
     for (int j = tid; j < b; j += nt) {
-        const double d = Gg[(size_t)j * b + j];
+        const double d = (SMEM ? Gin : Gg)[(size_t)j * b + j];
         dscale[j] = d > 0.0 ? rsqrt(d) : 0.0;
     }
     __syncthreads();
     for (int idx = tid; idx < b * b; idx += nt) {
         const int i = idx / b, j = idx - i * b;
-        G[i * ld + j] = Gg[idx] * dscale[i] * dscale[j];
+        G[i * ld + j] = (SMEM ? Gin : Gg)[idx] * dscale[i] * dscale[j];
     }
     __syncthreads();
     const int gi0 = tid / b, gk0 = tid - gi0 * b, gdi = nt / b, gdk = nt - gdi * b;
+    int si = gi0, sk = gk0;   // where the walk starts; in global memory it skips the rows <= j, which hold no update
     for (int j = 0; j < b; j++) {
         const int m = b - j - 1;
         if (tid < m || tid == 0) {   // the column's owners each derive the pivot (no broadcast barrier)
@@ -389,7 +305,8 @@ chol_inverse_fast_kernel(int b, const double *__restrict__ Gg, float *__restrict
         }
         __syncthreads();
         // every thread owns the same (i, k) positions of the b x b grid in all steps (no index division)
-        for (int i = gi0, k = gk0; i < b;) {
+        if (!SMEM) while (si <= j) { sk += gdk; si += gdi; if (sk >= b) { sk -= b; si++; } }
+        for (int i = si, k = sk; i < b;) {
             if (k > j && k <= i) G[i * ld + k] -= colj[i] * colj[k];
             k += gdk; i += gdi;
             if (k >= b) { k -= b; i++; }
@@ -435,163 +352,59 @@ chol_inverse_fast_kernel(int b, const double *__restrict__ Gg, float *__restrict
 }
 
 int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_out_dev, double *Minv64) {
-    const size_t small = sizeof(double) * 3 * (size_t)b;
-    const size_t big = small + sizeof(double) * (size_t)b * b;
-    const size_t fast = small + sizeof(double) * (size_t)b * (b | 1);
-    if (fast <= 200 * 1024 && b <= 128) {
-        static bool attr_fast = false;
-        if (!attr_fast) {
-            GEMB_CUDA(cudaFuncSetAttribute(chol_inverse_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            attr_fast = true;
-        }
-        chol_inverse_fast_kernel<<<1, 1024, fast, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
-    } else if (big <= 220 * 1024) {
-        static bool attr_set = false;
-        if (!attr_set) {
-            GEMB_CUDA(cudaFuncSetAttribute(chol_inverse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));  // + 4 B static
-            attr_set = true;
-        }
-        chol_inverse_kernel<true><<<1, 1024, big, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
-    } else {
-        chol_inverse_kernel<false><<<1, 1024, small, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
+    const size_t vecs = sizeof(double) * 3 * (size_t)b;
+    const size_t smem = vecs + sizeof(double) * (size_t)b * (b | 1);
+    static int optin = 0;    // the device's per-block opt-in limit (227 KB on H100: b <= 168 in shared memory)
+    if (!optin) {
+        int v = 0;
+        GEMB_CUDA(cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+        GEMB_CUDA(cudaFuncSetAttribute(chol_inverse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
+        optin = v;
     }
+    if (smem <= (size_t)optin) chol_inverse_kernel<true><<<1, 1024, smem, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
+    else chol_inverse_kernel<false><<<1, 1024, vecs, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     return GEMB_OK;
 }
 
 // ------------------------------------------------------------------------------------ eigh
-// Two-sided cyclic Jacobi with round-robin (circle-method) pair ordering, one CTA, fp64.
-// A is destroyed; w ascending; Z column j <-> w[j].  Zt is b x b scratch.
-// A and Zt in global memory (eigh_launch takes it where the fast kernel's shared-memory matrix does not fit).
-__global__ void __launch_bounds__(1024)
-eigh_jacobi_kernel(int b, double *A, double *__restrict__ w, double *__restrict__ Z,
-                   double *Zt, int max_sweeps, double rel_tol) {   // A, Zt: written by other threads (no __restrict__)
-    extern __shared__ double sh[];
-    const int m = (b + 1) & ~1;     // even number of players; index >= b is a dummy
-    const int half = m / 2;
-    double *cs = sh;                // half
-    double *sn = sh + half;         // half
-    int *pp = (int *)(sh + 2 * half);
-    int *qq = pp + half;
-    __shared__ double s_woff[32], s_wdiag[32];   // per-warp partials, added in warp order (same result every run)
-    const int tid = threadIdx.x, nt = blockDim.x;
-    for (int idx = tid; idx < b * b; idx += nt) Zt[idx] = (idx / b == idx % b) ? 1.0 : 0.0;
-    __syncthreads();
-    for (int sweep = 0; sweep < max_sweeps; sweep++) {
-        __syncthreads();                 // the previous sweep has read s_woff / s_wdiag
-        double off = 0.0, dg = 0.0;
-        for (int idx = tid; idx < b * b; idx += nt) {
-            const int i = idx / b, j = idx - i * b;
-            const double v = A[idx];
-            if (i == j) dg += v * v; else off += v * v;
-        }
-        for (int o = 16; o > 0; o >>= 1) {
-            off += __shfl_xor_sync(0xffffffffu, off, o);
-            dg += __shfl_xor_sync(0xffffffffu, dg, o);
-        }
-        if ((tid & 31) == 0) { s_woff[tid >> 5] = off; s_wdiag[tid >> 5] = dg; }
-        __syncthreads();
-        double s_off = 0.0, s_diag = 0.0;
-        for (int w = 0; w < (nt >> 5); w++) { s_off += s_woff[w]; s_diag += s_wdiag[w]; }
-        if (s_off <= rel_tol * rel_tol * (s_diag + s_off) || s_diag + s_off == 0.0) break;
-        for (int r = 0; r < m - 1; r++) {
-            if (tid < half) {
-                int p, q;
-                if (tid == 0) { p = m - 1; q = r % (m - 1); }
-                else { p = (r + tid) % (m - 1); q = (r + m - 1 - tid) % (m - 1); }
-                if (p > q) { int t = p; p = q; q = t; }
-                double c = 1.0, s = 0.0;
-                if (q < b) {
-                    const double apq = A[(size_t)p * b + q];
-                    if (apq != 0.0) {
-                        const double app = A[(size_t)p * b + p], aqq = A[(size_t)q * b + q];
-                        const double theta = (aqq - app) / (2.0 * apq);
-                        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-                        c = rsqrt(t * t + 1.0);
-                        s = t * c;
-                    }
-                } else { q = -1; }
-                pp[tid] = p; qq[tid] = q; cs[tid] = c; sn[tid] = s;
-            }
-            __syncthreads();
-            // columns: A <- A J, Zt <- Zt J   (consecutive threads -> different pairs, same row)
-            for (int idx = tid; idx < half * b; idx += nt) {
-                const int k = idx / half, pi = idx - k * half;
-                const int p = pp[pi], q = qq[pi];
-                if (q < 0) continue;
-                const double c = cs[pi], s = sn[pi];
-                if (s == 0.0) continue;
-                double x = A[(size_t)k * b + p], y = A[(size_t)k * b + q];
-                A[(size_t)k * b + p] = c * x - s * y;
-                A[(size_t)k * b + q] = s * x + c * y;
-                x = Zt[(size_t)k * b + p]; y = Zt[(size_t)k * b + q];
-                Zt[(size_t)k * b + p] = c * x - s * y;
-                Zt[(size_t)k * b + q] = s * x + c * y;
-            }
-            __syncthreads();
-            // rows: A <- J^T A   (consecutive threads -> consecutive columns)
-            for (int idx = tid; idx < half * b; idx += nt) {
-                const int pi = idx / b, k = idx - pi * b;
-                const int p = pp[pi], q = qq[pi];
-                if (q < 0) continue;
-                const double c = cs[pi], s = sn[pi];
-                if (s == 0.0) continue;
-                const double x = A[(size_t)p * b + k], y = A[(size_t)q * b + k];
-                A[(size_t)p * b + k] = c * x - s * y;
-                A[(size_t)q * b + k] = s * x + c * y;
-            }
-            __syncthreads();
-        }
-    }
-    __syncthreads();
-    // sort ascending by rank counting, permute eigenvector columns (one warp per eigenvalue)
-    const int lane = tid & 31, warp = tid >> 5, nwarps = nt >> 5;
-    for (int j = warp; j < b; j += nwarps) {
-        const double wj = A[(size_t)j * b + j];
-        int rank = 0;
-        for (int i = lane; i < b; i += 32) {
-            const double wi = A[(size_t)i * b + i];
-            rank += (wi < wj) || (wi == wj && i < j);
-        }
-        for (int o = 16; o > 0; o >>= 1) rank += __shfl_xor_sync(0xffffffffu, rank, o);
-        if (lane == 0) w[rank] = wj;
-        for (int k = lane; k < b; k += 32) Z[(size_t)k * b + rank] = Zt[(size_t)k * b + j];
-    }
-}
-
-// Fast variant for b*(b|1)*16 bytes <= shared memory (b <= 117).  The generic kernel is ISSUE bound, not
-// bandwidth bound (ncu: 558 warp instructions per warp per round, 63 % issue-active, fp64 pipe 11 %): runtime
-// integer divisions and four parameter loads per element.  Here
+// Two-sided cyclic Jacobi with round-robin (circle-method) pair ordering, one CTA, fp64: w ascending, Z column j <->
+// w[j].  Zt is b x b scratch.  b <= 1024: one rotation pair per thread.
 //   * the two-sided update A <- J^T A J is done per 2x2 BLOCK {p,q} x {r,s} of two rotation pairs by one thread
-//     (4 loads, both rotations in registers, 4 stores): half the shared-memory traffic and one block barrier per
-//     round less than column phase + row phase;
+//     (4 loads, both rotations in registers, 4 stores): half the A traffic and one block barrier per round less
+//     than a column phase followed by a row phase;
 //   * the eigenvector accumulator is kept transposed so that its update is a row walk;
 //   * (pair, column) indices advance incrementally (no division in the loops), rotation parameters are one
-//     16-byte and one 8-byte load, the leading dimension is odd (conflict-free row and column walks).
-// ZT_GLOBAL (117 < b <= 167, the Rayleigh-Ritz matrix of the thick-restart Lanczos solver): A alone fills the shared
-// memory, the eigenvector accumulator lives in global memory (L2 resident, 200 KB) and is updated by coalesced row
-// walks -- a generic kernel with A in shared memory needed 15.2 ms for b = 160 (10.9 us per Jacobi round, 43 % of an
-// R-MAT solve).
-template <bool ZT_GLOBAL>
+//     16-byte and one 8-byte load, the shared-memory leading dimension is odd (conflict-free row and column walks).
+// Where the matrices live (eigh_launch takes the first that fits in shared memory):
+//   JAC_SHARED     A and Z^T in shared memory (b <= 117);
+//   JAC_ZT_GLOBAL  A alone fills the shared memory (b <= 167, e.g. the Rayleigh-Ritz matrix of the thick-restart
+//                  Lanczos solver); Z^T is Zt (L2 resident, 200 KB), updated by coalesced row walks;
+//   JAC_GLOBAL     A is G itself (leading dimension b, destroyed) and Z^T is Zt.
+// G and Zt are not __restrict__: in global memory they are written by other threads between barriers.
+enum JacobiStore { JAC_SHARED, JAC_ZT_GLOBAL, JAC_GLOBAL };
+template <JacobiStore STORE>
 __global__ void __launch_bounds__(1024)
-eigh_jacobi_fast_kernel(int b, const double *__restrict__ Ag, double *__restrict__ w, double *__restrict__ Z,
-                        double *Ztg, int max_sweeps, double rel_tol) {   // Ztg: as A of eigh_jacobi_kernel
+eigh_jacobi_kernel(int b, double *Ag, double *__restrict__ w, double *__restrict__ Z, double *Ztg, int max_sweeps,
+                   double rel_tol) {
+    constexpr bool A_GLOBAL = STORE == JAC_GLOBAL, ZT_GLOBAL = STORE != JAC_SHARED;
     extern __shared__ __align__(16) unsigned char sh_fast[];
     double *sh = (double *)sh_fast;
     const int m = (b + 1) & ~1;
     const int half = m / 2;
-    const int ld = b | 1;
+    const int ld = A_GLOBAL ? b : (b | 1);
     double2 *csn = (double2 *)sh;                 // half : (c, s)
     int2 *pq = (int2 *)(sh + 2 * half);           // half : (p, q), q = -1 for the dummy partner
-    double *A = sh + 3 * half + 2;                // b x ld
+    double *A = A_GLOBAL ? Ag : sh + 3 * half + 2;       // b x ld
     double *ZT = ZT_GLOBAL ? Ztg : A + (size_t)b * ld;   // ZT[j][k] = component k of eigenvector j
     const int ldz = ZT_GLOBAL ? b : ld;
     __shared__ double s_woff[32], s_wdiag[32];   // per-warp partials, added in warp order (same result every run)
     const int tid = threadIdx.x, nt = blockDim.x;
+    const double *__restrict__ Ain = Ag;          // read only, and only when A is in shared memory (read-only data path)
     for (int idx = tid; idx < b * b; idx += nt) {
         const int i = idx / b, j = idx - i * b;
-        A[i * ld + j] = Ag[idx];
+        if (!A_GLOBAL) A[i * ld + j] = Ain[idx];
         ZT[i * ldz + j] = (i == j) ? 1.0 : 0.0;
     }
     // incremental (pair, column) walks: idx = tid + t * nt  ->  (idx / div, idx % div)
@@ -727,22 +540,16 @@ int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Z
     const int half = ((b + 1) & ~1) / 2;
     const size_t base = sizeof(double) * (3 * half + 2);
     const size_t cap = 220 * 1024;
-    const size_t fast = base + 2 * sizeof(double) * (size_t)b * (b | 1);
-    const size_t fast_a = base + sizeof(double) * (size_t)b * (b | 1);       // A only; eigenvectors in global memory
-    if (fast <= cap || fast_a <= cap) {
-        static bool attr_fast = false;
-        if (!attr_fast) {
-            GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_fast_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
-            GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_fast_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
-            attr_fast = true;
-        }
-        if (fast <= cap) eigh_jacobi_fast_kernel<false><<<1, 1024, fast, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
-        else eigh_jacobi_fast_kernel<true><<<1, 1024, fast_a, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-        return GEMB_OK;
+    const size_t mat = sizeof(double) * (size_t)b * (b | 1);
+    static bool attr_set = false;
+    if (!attr_set) {
+        GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_kernel<JAC_SHARED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
+        GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_kernel<JAC_ZT_GLOBAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
+        attr_set = true;
     }
-    eigh_jacobi_kernel<<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
+    if (base + 2 * mat <= cap) eigh_jacobi_kernel<JAC_SHARED><<<1, 1024, base + 2 * mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
+    else if (base + mat <= cap) eigh_jacobi_kernel<JAC_ZT_GLOBAL><<<1, 1024, base + mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
+    else eigh_jacobi_kernel<JAC_GLOBAL><<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     return GEMB_OK;
@@ -890,7 +697,8 @@ extern "C" int gemb_gram(gemb_ctx *c, int64_t n, const float *P, int b1, const f
 }
 
 // The b x b hooks run the solvers' own launchers, so b picks the kernel variant exactly as in a solve.  b is limited to
-// the solvers' block limit (gemb_hope: b <= 1024), which eigh_jacobi_kernel relies on (one rotation per thread).
+// the solvers' block limit (gemb_hope: b <= 1024), which both kernels rely on (one thread per row of a column of L, one
+// rotation pair per thread).
 extern "C" int gemb_chol_inverse(gemb_ctx *c, int b, const double *G, double *Minv64_out, float *Minv32_out,
                                  int *rank_out) {
     using namespace gemb;

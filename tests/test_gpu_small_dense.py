@@ -3,21 +3,21 @@
   gemb_chol_inverse -> chol_inverse_launch: Minv = R^-1 of CholeskyQR (G = R^T R) with the scale-free rank test
   gemb_eigh         -> eigh_launch: cyclic Jacobi, w ascending, Z column j <-> w[j]
 
-Both launchers choose the kernel by b; the sizes below sit on each side of every switch:
-  chol_inverse_fast_kernel          b <= 128         (matrix in shared memory)
-  chol_inverse_kernel<true>         129 <= b <= 166  (matrix in shared memory)
-  chol_inverse_kernel<false>        b >= 167         (matrix in global memory)
-  eigh_jacobi_fast_kernel<false>    b <= 117         (matrix and eigenvectors in shared memory)
-  eigh_jacobi_fast_kernel<true>     118 <= b <= 167  (eigenvectors in global memory)
-  eigh_jacobi_kernel                b >= 168         (global memory)
+Both launchers choose where the kernel keeps its matrices by b; the sizes below sit on each side of every switch, and
+b = 1024 is the widest block the solvers use:
+  chol_inverse_kernel<true>             b <= 168         (matrix in shared memory; 168 on H100, 227 KB per block)
+  chol_inverse_kernel<false>            b >= 169         (matrix in global memory)
+  eigh_jacobi_kernel<JAC_SHARED>        b <= 117         (matrix and eigenvectors in shared memory)
+  eigh_jacobi_kernel<JAC_ZT_GLOBAL>     118 <= b <= 167  (eigenvectors in global memory)
+  eigh_jacobi_kernel<JAC_GLOBAL>        b >= 168         (matrix and eigenvectors in global memory)
 Odd b gives the round-robin Jacobi ordering a dummy player."""
 import numpy as np
 import pytest
 from scipy.linalg import solve_triangular
 
 PIV_EPS = 1e-5                   # GEMB_PIV_EPS of dense.cu
-CHOL_SIZES = [1, 2, 16, 80, 127, 128, 129, 144, 166, 167, 200, 256]
-EIGH_SIZES = [1, 2, 3, 80, 117, 118, 144, 167, 168, 192, 256, 400]
+CHOL_SIZES = [1, 2, 16, 80, 127, 128, 129, 144, 166, 167, 168, 169, 200, 256, 1024]
+EIGH_SIZES = [1, 2, 3, 80, 117, 118, 144, 167, 168, 192, 256, 400, 1024]
 
 
 def chol_inverse_ref(G):
