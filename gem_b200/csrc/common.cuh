@@ -122,6 +122,7 @@ struct gemb_ctx {
     int device = 0;
     int sm_count = 132;
     cudaStream_t stream = nullptr;
+    cudaStream_t side = nullptr;     // work that runs beside a single-CTA kernel of `stream` (forked and joined by events)
     // multi-GPU
     int rank = 0, nranks = 1;
     void *comm = nullptr;  // ncclComm_t
@@ -239,7 +240,8 @@ int sum_partials_launch(gemb_ctx *ctx, int parts, int64_t count, const double *p
 //  eigh: G -> eigenvalues w ascending (b), eigenvectors Z (b x b, column j <-> w[j]); G destroyed where the matrix does
 //  not fit in shared memory (b >= 168).
 // rel_tol: stop the Jacobi sweeps when ||offdiag||_F <= rel_tol * ||G||_F
-int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch /* b x b */, double rel_tol = 1e-11);
+int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch /* b x b */, double rel_tol = 1e-11,
+                bool symmetrize = false /* decompose (G + G^T) / 2 */);
 int randn_launch(gemb_ctx *ctx, int64_t n, int b, uint64_t seed, uint64_t row_offset, float *X);
 // sum of squares of all entries (fp64 accumulate) -> out_dev[0]
 int sumsq_launch(gemb_ctx *ctx, int64_t count, const float *X, double *out_dev);

@@ -216,6 +216,7 @@ int gemb_ctx_create(int device, gemb_ctx **out) {
     c->device = device;
     c->sm_count = prop.multiProcessorCount;
     GEMB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+    GEMB_CUDA(cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking));
     *out = c;
     return GEMB_OK;
 }
@@ -235,6 +236,7 @@ int gemb_ctx_destroy(gemb_ctx *c) {
     dfree(c->spmm_scratch);
     dfree(c->red_scratch);
     if (c->stream) cudaStreamDestroy(c->stream);
+    if (c->side) cudaStreamDestroy(c->side);
     delete c;
     return GEMB_OK;
 }

@@ -382,12 +382,14 @@ int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_
 //   JAC_ZT_GLOBAL  A alone fills the shared memory (b <= 167, e.g. the Rayleigh-Ritz matrix of the thick-restart
 //                  Lanczos solver); Z^T is Zt (L2 resident, 200 KB), updated by coalesced row walks;
 //   JAC_GLOBAL     A is G itself (leading dimension b, destroyed) and Z^T is Zt.
+// symmetrize: the decomposition is that of (G + G^T) / 2, formed while the matrix is loaded (a Rayleigh-Ritz matrix
+// V^T (A V) is symmetric only up to rounding).
 // G and Zt are not __restrict__: in global memory they are written by other threads between barriers.
 enum JacobiStore { JAC_SHARED, JAC_ZT_GLOBAL, JAC_GLOBAL };
 template <JacobiStore STORE>
 __global__ void __launch_bounds__(1024)
 eigh_jacobi_kernel(int b, double *Ag, double *__restrict__ w, double *__restrict__ Z, double *Ztg, int max_sweeps,
-                   double rel_tol) {
+                   double rel_tol, bool symmetrize) {
     constexpr bool A_GLOBAL = STORE == JAC_GLOBAL, ZT_GLOBAL = STORE != JAC_SHARED;
     extern __shared__ __align__(16) unsigned char sh_fast[];
     double *sh = (double *)sh_fast;
@@ -404,7 +406,8 @@ eigh_jacobi_kernel(int b, double *Ag, double *__restrict__ w, double *__restrict
     const double *__restrict__ Ain = Ag;          // read only, and only when A is in shared memory (read-only data path)
     for (int idx = tid; idx < b * b; idx += nt) {
         const int i = idx / b, j = idx - i * b;
-        if (!A_GLOBAL) A[i * ld + j] = Ain[idx];
+        if (!A_GLOBAL) A[i * ld + j] = (symmetrize && i != j) ? 0.5 * (Ain[idx] + Ain[j * b + i]) : Ain[idx];
+        else if (symmetrize && i < j) Ag[idx] = Ag[j * b + i] = 0.5 * (Ag[idx] + Ag[j * b + i]);   // the pair's only owner
         ZT[i * ldz + j] = (i == j) ? 1.0 : 0.0;
     }
     // incremental (pair, column) walks: idx = tid + t * nt  ->  (idx / div, idx % div)
@@ -536,7 +539,7 @@ eigh_jacobi_kernel(int b, double *Ag, double *__restrict__ w, double *__restrict
     }
 }
 
-int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch, double rel_tol) {
+int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Zscratch, double rel_tol, bool symmetrize) {
     const int half = ((b + 1) & ~1) / 2;
     const size_t base = sizeof(double) * (3 * half + 2);
     const size_t cap = 220 * 1024;
@@ -547,9 +550,9 @@ int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Z
         GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_kernel<JAC_ZT_GLOBAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
         attr_set = true;
     }
-    if (base + 2 * mat <= cap) eigh_jacobi_kernel<JAC_SHARED><<<1, 1024, base + 2 * mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
-    else if (base + mat <= cap) eigh_jacobi_kernel<JAC_ZT_GLOBAL><<<1, 1024, base + mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
-    else eigh_jacobi_kernel<JAC_GLOBAL><<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol);
+    if (base + 2 * mat <= cap) eigh_jacobi_kernel<JAC_SHARED><<<1, 1024, base + 2 * mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
+    else if (base + mat <= cap) eigh_jacobi_kernel<JAC_ZT_GLOBAL><<<1, 1024, base + mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
+    else eigh_jacobi_kernel<JAC_GLOBAL><<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     return GEMB_OK;

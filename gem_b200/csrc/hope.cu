@@ -52,6 +52,7 @@ struct HopeWork {
     DeviceBuffer<double> G, G2, w, Z, Zs, scal;
     DeviceBuffer<float> Minv, M1, M2;
     DeviceBuffer<int> rank_dev;
+    CallEvents<2> fork_join;    // c->stream -> c->side and back (ritz_eigh)
     int64_t spmm_wide = 0, spmm_all = 0;
     bool halo = false;       // multi-GPU: needed-rows-only exchange over peer memory (halo.cu); buf[] = g->halo.buf[]
     int64_t pushes = 0;      // blocks whose rows were pushed to the peers
@@ -260,15 +261,24 @@ __global__ void coldiff_sumsq_kernel(int64_t n, int b, const float *__restrict__
     atomicAdd(out + j, acc);
 }
 
-// T <- (T + T^T) / 2
-__global__ void symmetrize_kernel(int b, double *__restrict__ T) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= b * b) return;
-    const int i = idx / b, j = idx - i * b;
-    if (i < j) {
-        const double v = 0.5 * (T[(size_t)i * b + j] + T[(size_t)j * b + i]);
-        T[(size_t)i * b + j] = v;
-        T[(size_t)j * b + i] = v;
+// q[col] = z^T H z for every column z of Z (b x b, row-major), H = (AV)^T (AV): the squared norm of A V z, from which
+// the stop rule takes the residual of the Ritz pair.  One CTA per column; the sums run in index order with separately
+// rounded products (t = sum_s H[r][s] Z[s][col], then q = sum_r Z[r][col] t), so the value does not depend on the
+// launch shape.  Dynamic shared memory: b doubles.
+__global__ void ritz_quadform_kernel(int b, const double *__restrict__ H, const double *__restrict__ Z,
+                                     double *__restrict__ q) {
+    extern __shared__ double s_term[];
+    const int col = blockIdx.x;
+    for (int r = threadIdx.x; r < b; r += blockDim.x) {
+        double t = 0.0;
+        for (int s = 0; s < b; s++) t = __dadd_rn(t, __dmul_rn(H[(size_t)r * b + s], Z[(size_t)s * b + col]));
+        s_term[r] = __dmul_rn(Z[(size_t)r * b + col], t);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double acc = 0.0;
+        for (int r = 0; r < b; r++) acc = __dadd_rn(acc, s_term[r]);
+        q[col] = acc;
     }
 }
 
@@ -466,16 +476,36 @@ static int residual_check(HopeWork &W, float beta, int J, const float *P, const 
     return GEMB_OK;
 }
 
-// Rayleigh-Ritz eigen step: (W.w, W.Z) = eigh(W.G2) (G2 destroyed), the eigenvalues (ascending) read back into lam.
+// Rayleigh-Ritz eigen step: (W.w, W.Z) = eigh(W.G2) (G2 destroyed; `symmetrize`: eigh of (G2 + G2^T) / 2), the
+// eigenvalues (ascending) read back into lam[0..b).  Given AV (the residual stop rule), lam[b..2b) receives z^T H z of
+// every Ritz vector z, H = (AV)^T (AV), in the same copy: one host round trip per step.  H does not depend on the
+// eigen-decomposition, and the Jacobi is one CTA: the Gram launch runs on c->side while the Jacobi has the other SMs to
+// spare (the Jacobi is launched first so that it is not queued behind the Gram's one-CTA-per-SM grid).  The Gram's
+// partial sums are added in a fixed order, so H is the same whenever it runs; the all-reduce stays on c->stream.
 // Jacobi accuracy follows the requested tolerance (Z only pre-rotates the CholeskyQR and forms the Ritz vectors:
 // an off-diagonal remainder of 1e-2 tol is invisible at tol; one sweep less per round at the bench setting)
-static int ritz_eigh(HopeWork &W, float tol, std::vector<double> &lam) {
+static int ritz_eigh(HopeWork &W, float tol, bool symmetrize, std::vector<double> &lam, const float *AV = nullptr) {
     gemb_ctx *c = W.c;
     const int b = W.b;
     GEMB_TRY(c->t_dense.begin(c->stream));
-    GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)tol))));
+    if (AV) GEMB_CUDA(cudaEventRecord(W.fork_join[0], c->stream));   // AV and the reduction scratch are free from here
+    GEMB_TRY(eigh_launch(c, b, W.G2.get(), W.w.get(), W.Z.get(), W.Zs.get(), std::min(1e-5, std::max(1e-13, 1e-2 * (double)tol)),
+                         symmetrize));
+    if (AV) {
+        GEMB_CUDA(cudaStreamWaitEvent(c->side, W.fork_join[0], 0));
+        std::swap(c->stream, c->side);                               // the launchers take their stream from the context
+        const int s = gram_launch(c, W.rows, AV, b, AV, b, W.G.get());
+        std::swap(c->stream, c->side);
+        GEMB_TRY(s);
+        GEMB_CUDA(cudaEventRecord(W.fork_join[1], c->side));
+        GEMB_CUDA(cudaStreamWaitEvent(c->stream, W.fork_join[1], 0));
+        GEMB_TRY(comm_allreduce_f64(W, W.G.get(), (size_t)b * b));
+        ritz_quadform_kernel<<<b, 128, sizeof(double) * b, c->stream>>>(b, W.G.get(), W.Z.get(), W.w.get() + b);
+        GEMB_CUDA(cudaGetLastError());
+        count_launch();
+    }
     GEMB_TRY(c->t_dense.end(c->stream));
-    return copy_sync(c, lam.data(), W.w.get(), sizeof(double) * b, cudaMemcpyDeviceToHost);
+    return copy_sync(c, lam.data(), W.w.get(), sizeof(double) * (AV ? 2 * b : b), cudaMemcpyDeviceToHost);
 }
 
 // stop measure: per-value relative change of the k SINGULAR values (theta = sigma^2) since the last round, floored at
@@ -506,7 +536,7 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         GEMB_TRY(katz(W, false, beta, J, V, U, T1, T2));              // U = S V
         GEMB_TRY(gram_full(W, U, U, W.G.get()));                            // T = U^T U
         GEMB_CUDA(cudaMemcpyAsync(W.G2.get(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToDevice, c->stream));
-        GEMB_TRY(ritz_eigh(W, o.tol, theta));
+        GEMB_TRY(ritz_eigh(W, o.tol, false, theta));
         const double tmax = std::max(theta[b - 1], 1e-300);
         const double change = sigma_change(&theta[b - k], &theta_prev[b - k], k, tmax);
         R.change = change;
@@ -711,8 +741,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         }
     }
 
-    std::vector<double> lam(b), gval(b), th_sorted(b), th_prev(b, 0.0);
-    std::vector<double> Wh(o.stop_rule == 1 ? (size_t)b * b : 0), Zr(o.stop_rule == 1 ? (size_t)b * b : 0);
+    std::vector<double> lam(2 * b), gval(b), th_sorted(b), th_prev(b, 0.0);   // lam[b..2b): z^T (AV)^T (AV) z (stop rule 1)
     std::vector<int> order(b);
 
     // scaled three-term Chebyshev recurrence of degree deg on [c0 - e, c0 + e], normalised at the dominant end by
@@ -746,13 +775,10 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         // Rayleigh-Ritz on A: T = V^T A V, (l, Z) = eigh(T)
         GEMB_TRY(dist_spmm(W, false, b, 1.f, V, nullptr, AV, true));
         GEMB_TRY(gram_full(W, V, AV, W.G2.get()));
-        symmetrize_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, W.G2.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
         // (Measured: running the single-CTA Jacobi on a side stream while the filter starts with the PREVIOUS
         // round's interval costs two extra rounds -- 75 instead of 56 SpMM sweeps -- and is slower overall;
         // the eigen-decomposition therefore stays on the critical path.)
-        GEMB_TRY(ritz_eigh(W, o.tol, lam));
+        GEMB_TRY(ritz_eigh(W, o.tol, true, lam, o.stop_rule == 1 ? AV : nullptr));
         if (ritz_bound) map.tighten(lam.data(), b, 1.05);
         for (int i = 0; i < b; i++) gval[i] = map.key(lam[i]);
         std::iota(order.begin(), order.end(), 0);
@@ -773,19 +799,10 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
             // residual of the Ritz pairs from the Rayleigh-Ritz products alone: with V orthonormal and (l, z) an
             // eigenpair of V^T A V,  ||A V z - l V z||^2 = z^T (AV)^T (AV) z - l^2.  Mapped to the Katz operator
             // through |f'(l)| = beta / (1 - beta l)^2 and measured against sigma_max, like compute_residual does.
-            GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
-            GEMB_CUDA(cudaMemcpyAsync(Wh.data(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost, c->stream));
-            GEMB_TRY(copy_sync(c, Zr.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost));
             double worst = 0.0;
             for (int j = 0; j < k; j++) {
                 const int col = order[j];
-                double q = 0.0;
-                for (int r = 0; r < b; r++) {
-                    double t = 0.0;
-                    for (int s2 = 0; s2 < b; s2++) t += Wh[(size_t)r * b + s2] * Zr[(size_t)s2 * b + col];
-                    q += Zr[(size_t)r * b + col] * t;
-                }
-                const double r2 = std::max(q - lam[col] * lam[col], 0.0);
+                const double r2 = std::max(lam[b + col] - lam[col] * lam[col], 0.0);
                 worst = std::max(worst, map.slope(lam[col]) * sqrt(r2) / std::max(gval[order[0]], 1e-300));
             }
             stop_measure = worst;
@@ -833,7 +850,9 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     // I - A_hat, the order lap.py:28-31 sorts into)
     std::vector<double> Zh((size_t)b * b);
     GEMB_TRY(copy_sync(c, Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost));
-    std::vector<float> M1((size_t)b * k), M2((size_t)b * k), sig(k);
+    // M = [M1 | M2] (b x d; LE / LLE: M1 alone, b x k): one apply writes whole rows of X
+    const int xw = mode ? k : 2 * k;
+    std::vector<float> M((size_t)b * xw), sig(k);
     std::vector<int> sel(k);
     for (int j = 0; j < k; j++) {
         const int col = order[j], q = map.out_col(j, k);
@@ -842,18 +861,16 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         sig[q] = (float)t.sigma;
         for (int i = 0; i < b; i++) {
             const double z = Zh[(size_t)i * b + col];
-            M2[(size_t)i * k + q] = (float)(z * t.scale);
-            M1[(size_t)i * k + q] = (float)((t.neg ? -z : z) * t.scale);
+            M[(size_t)i * xw + q] = (float)((t.neg ? -z : z) * t.scale);
+            if (!mode) M[(size_t)i * xw + k + q] = (float)(z * t.scale);
         }
     }
     R.sigma_max = gval[order[0]];
     GEMB_TRY(place_output(W, R, pool[0], d));
-    GEMB_CUDA(cudaMemcpyAsync(W.M1.get(), M1.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(W.M2.get(), M2.data(), sizeof(float) * b * k, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(W.M1.get(), M.data(), sizeof(float) * b * xw, cudaMemcpyHostToDevice, c->stream));
     GEMB_TRY(copy_sync(c, R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice));   // host staging goes out of scope
     GEMB_TRY(c->t_dense.begin(c->stream));
-    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), k, k, R.Xd, d));
-    if (!mode) GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));   // LE / LLE: no right half
+    GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), xw, xw, R.Xd, d));
     GEMB_TRY(c->t_dense.end(c->stream));
     if (mode || !o.compute_residual) return GEMB_OK;
 
@@ -1314,12 +1331,13 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     GEMB_CUDA(W.G2.alloc(b * b));
     GEMB_CUDA(W.Z.alloc(b * b));
     GEMB_CUDA(W.Zs.alloc(b * b));
-    GEMB_CUDA(W.w.alloc(b));
+    GEMB_CUDA(W.w.alloc(2 * b));                           // eigenvalues, then the stop rule's quadratic forms
     GEMB_CUDA(W.scal.alloc(b + 8));
     GEMB_CUDA(W.Minv.alloc(b * b));
-    GEMB_CUDA(W.M1.alloc(b * b));
+    GEMB_CUDA(W.M1.alloc((size_t)b * std::max(b, d)));     // b x b maps; the symmetric solver's b x d extraction map
     GEMB_CUDA(W.M2.alloc(b * b));
     GEMB_CUDA(W.rank_dev.alloc(1));
+    GEMB_CUDA(W.fork_join.create());
 
     c->t_spmm.reset(); c->t_dense.reset(); c->t_comm.reset(); c->t_misc.reset();
     const double t_alloc = now();
