@@ -20,6 +20,7 @@ EXPORTS = [
     'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
+    'gemb_recon_exclude',
 ]
 
 
@@ -115,6 +116,7 @@ def lib():
     L.gemb_recon_pairs.argtypes = [vp, vp, vp, i64, vp]
     L.gemb_recon_ranks.argtypes = [vp, vp, vp, ctypes.c_int, vp, vp]
     L.gemb_recon_top.argtypes = [vp, ctypes.c_int, i64, i64, vp, vp, vp, ctypes.POINTER(i64)]
+    L.gemb_recon_exclude.argtypes = [vp, vp, vp]
     _lib = L
     return L
 
@@ -446,5 +448,17 @@ class Reconstruction(_Handle):
             check(lib().gemb_recon_top(self._h, int(bool(is_undirected)), int(max_k), cnt, _ptr(i), _ptr(j), _ptr(w),
                                        ctypes.byref(m)))
         return i, j, w
+
+    def exclude(self, indptr, indices):
+        """gemb_recon_exclude: from now on ranks / top see only the candidates outside this CSR (n + 1 offsets,
+        strictly ascending column ids per row) -- the training edges of a link-prediction split.
+        indptr None clears it."""
+        if indptr is None:
+            check(lib().gemb_recon_exclude(self._h, None, None))
+            return
+        indptr = np.ascontiguousarray(indptr, dtype=np.int32)
+        indices = np.ascontiguousarray(indices, dtype=np.int32)
+        assert indptr.shape[0] == self.n + 1 and indices.shape[0] >= int(indptr[-1])
+        check(lib().gemb_recon_exclude(self._h, _ptr(indptr), _ptr(indices)))
 
     free = _Handle._release

@@ -177,3 +177,38 @@ def saveEmbedding(X, file_name, ids=None):
         f.write('%d %d\n' % X.shape)
         for i in ids:
             f.write('%d %s\n' % (i, ' '.join('%g' % v for v in X[i])))
+
+
+def sample_graph(di_graph, n_sampled_nodes=None, rng=None):
+    """gem/utils/graph_util.py:42-58: when n_sampled_nodes is given and smaller than the node count,
+    node_l = choice(n, n_sampled_nodes, replace=False) and the graph induced on node_l, node node_l[k] relabelled k;
+    otherwise (di_graph, arange(n)) without a draw.  di_graph: a networkx graph with nodes 0..n-1 (returns a
+    networkx DiGraph whose edges carry 'weight', default 1, added in di_graph.edges order, as the reference does) or
+    a gem_b200.graph.HostCSR (returns a HostCSR).  rng: a np.random.RandomState, None = the global np.random."""
+    from gem_b200.graph import HostCSR
+    node_num = di_graph.n if isinstance(di_graph, HostCSR) else len(di_graph.nodes)
+    if not (n_sampled_nodes and node_num > n_sampled_nodes):
+        return di_graph, np.arange(node_num)
+    node_l = (np.random if rng is None else rng).choice(node_num, n_sampled_nodes, replace=False)
+    return induced_graph(di_graph, node_l), node_l
+
+
+def induced_graph(di_graph, node_l):
+    """The graph sample_graph builds for a given node_l: the edges with both ends in node_l, node node_l[k] -> k."""
+    from gem_b200.graph import HostCSR, from_edges
+    node_l = np.asarray(node_l, dtype=np.int64)
+    s = node_l.size
+    if isinstance(di_graph, HostCSR):
+        inv = np.full(di_graph.n, -1, dtype=np.int64)
+        inv[node_l] = np.arange(s)
+        rows = np.repeat(np.arange(di_graph.n, dtype=np.int64), np.diff(np.asarray(di_graph.indptr, dtype=np.int64)))
+        u, v = inv[rows], inv[np.asarray(di_graph.indices, dtype=np.int64)]
+        keep = (u >= 0) & (v >= 0)
+        return from_edges(s, u[keep], v[keep], None if di_graph.data is None else di_graph.data[keep])
+    import networkx as nx
+    inv = {int(v): k for k, v in enumerate(node_l.tolist())}
+    sampled_graph = nx.DiGraph()
+    sampled_graph.add_nodes_from(range(s))
+    sampled_graph.add_weighted_edges_from((inv[st], inv[ed], w) for st, ed, w in di_graph.edges(data='weight', default=1)
+                                          if st in inv and ed in inv)
+    return sampled_graph

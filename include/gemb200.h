@@ -307,6 +307,17 @@ int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indice
 int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap, int32_t *i_out, int32_t *j_out,
                    float *w_out, int64_t *m_out);
 
+/* Link prediction: rank held-out edges among the candidates that are not training edges.  Replaces, on top of the
+ * two calls above, the train/test split's consequence in the evaluation -- the predicted list filtered edge by edge,
+ * [e for e in pred if not train.has_edge(e[0], e[1])], after split_di_graph_to_train_test (evaluation_util.py:39-53).
+ * ex_indptr (n + 1 offsets) / ex_indices (host, int32, strictly ascending column ids per row) is the exclusion, copied
+ * to the device; ex_indptr == NULL clears it.  While it is set, gemb_recon_ranks and gemb_recon_top report their
+ * results over the candidates NOT in it: a true edge that is itself excluded gets rank 0, n_pred_row counts only the
+ * remaining candidates, and top selects among them.  Without an exclusion both are unchanged.  Setting or clearing it
+ * drops the cached top selection.  Cost: ranks O(sum_i true_deg_i * ex_deg_i) gathers after the usual pass; top
+ * sorts the excluded values once per call that selects and filters the collected entries by binary search. */
+int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *ex_indices);
+
 /* ---- wire formats (SURVEY 8(f) rank 2): the reference's text files, read and written natively and in parallel.
  * HOST code only -- these entry points need no GPU.
  * Edge list: every non-blank line "src dst [weight]" (loadGraphFromEdgeListTxt, graph_util.py:143-158: exactly three
