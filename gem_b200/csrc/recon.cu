@@ -28,15 +28,14 @@
 // distinct distances.  delta is summed in the difference form (recon_sqdist_kernel): exact 0 for equal rows.
 //
 // Link prediction (evaluation_util.py:39-53 splits the graph; the held-out edges are ranked among the candidates that
-// are not training edges): gemb_recon_exclude sets an exclusion CSR.  The counting kernels above stay as they are;
-// ranks are corrected per row by recon_exclude_rank_kernel (O(test_deg * train_deg) gathers, no second n^2 pass),
-// and top subtracts the excluded values >= T from each bisection count and drops the excluded entries of the
-// collected set (recon_exclude_compact_kernel).  Integer counts: the results do not depend on run order.
+// are not training edges): gemb_recon_exclude keeps the panel offsets of the training edges.  An entry that holds 0
+// is not a candidate in any counting kernel (nor, for the Gaussian kind, key 0), so ranks and top run unchanged on
+// the panels with those entries set to 0: recon_swap_kernel zeroes them and keeps their values for the length of
+// the call, and puts them back before it returns (dense and pairs always see the unmasked values).
 #include "common.cuh"
 #include <algorithm>
 #include <cmath>
 #include <vector>
-#include <cub/cub.cuh>
 
 struct gemb_recon {
     gemb_ctx *ctx = nullptr;
@@ -44,13 +43,14 @@ struct gemb_recon {
     int k = 0;
     int kind = 0;             // GEMB_RECON_DOT, _SPLIT or _GAUSS
     float *adj = nullptr;     // n x n_pad, panel-major
-    // gemb_recon_top cache (the bisection is 31 passes; the caller asks for the count first, then the entries).
-    // top_raw: entries >= top_bits before the exclusion is taken out (what the COLLECT pass gathers)
+    // gemb_recon_top cache (the bisection is 31 passes; the caller asks for the count first, then the entries)
     int top_valid = 0, top_und = 0;
-    int64_t top_k = 0, top_count = 0, top_raw = 0;
+    int64_t top_k = 0, top_count = 0;
     uint32_t top_bits = 0;
-    // exclusion CSR (gemb_recon_exclude): n + 1 offsets, sorted column ids per row; nullptr = none
-    int32_t *ex_ptr = nullptr, *ex_idx = nullptr;
+    // exclusion (gemb_recon_exclude): ex_nnz distinct panel offsets, and their values while a ranks / top call has
+    // them masked (0 between calls); nullptr = none
+    int64_t *ex_off = nullptr;
+    float *ex_saved = nullptr;
     int64_t ex_nnz = 0;
 };
 
@@ -58,7 +58,7 @@ namespace gemb {
 
 constexpr int PW = 64;   // panel width
 
-__device__ __forceinline__ size_t adj_index(int64_t i, int64_t j, int64_t n) {
+__host__ __device__ __forceinline__ size_t adj_index(int64_t i, int64_t j, int64_t n) {
     return ((size_t)(j >> 6) * (size_t)n + (size_t)i) * PW + (size_t)(j & 63);
 }
 
@@ -302,112 +302,14 @@ __global__ void recon_key_to_delta_kernel(int64_t m, float *__restrict__ w) {
 }
 
 // ---- exclusion (link prediction)
-// value of excluded entry (i, j) when it is a candidate (j != i, j > i under undirected, a > 0), else 0.  The raw
-// panel value: for the Gaussian kind the key, which orders as the score does.
-__device__ __forceinline__ float excluded_value(int64_t i, int64_t j, int undirected, const float *__restrict__ adj,
-                                                int64_t n) {
-    if (j == i || (undirected && j < i)) return 0.f;
-    const float v = adj[adj_index(i, j, n)];
-    return v > 0.f ? v : 0.f;
-}
-
-// One warp per row i, after recon_rank_kernel.  For each true edge e = (i -> j_e) with rank r > 0, subtract the
-// excluded candidates that sort before it (weight greater, or equal with a smaller column); an edge that is itself
-// excluded gets rank 0.  n_pred_row[i] loses the number of excluded candidates of the row.
-__global__ void __launch_bounds__(256)
-recon_exclude_rank_kernel(int64_t n, const int32_t *__restrict__ indptr, const int32_t *__restrict__ indices,
-                          const int32_t *__restrict__ ex_ptr, const int32_t *__restrict__ ex_idx, int undirected,
-                          const float *__restrict__ adj, int32_t *__restrict__ rank_out,
-                          int32_t *__restrict__ n_pred_row) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t i = warp; i < n; i += nwarps) {
-        const int x_begin = ex_ptr[i], x_end = ex_ptr[i + 1];
-        if (x_begin == x_end) continue;
-        int nvalid = 0;
-        for (int x = x_begin + lane; x < x_end; x += 32)
-            nvalid += excluded_value(i, ex_idx[x], undirected, adj, n) > 0.f ? 1 : 0;
-        for (int o = 16; o > 0; o >>= 1) nvalid += __shfl_xor_sync(0xffffffffu, nvalid, o);
-        if (lane == 0) n_pred_row[i] -= nvalid;
-        const int e_begin = indptr[i], e_end = indptr[i + 1];
-        for (int e0 = e_begin; e0 < e_end; e0 += 32) {
-            const int e = e0 + lane;
-            int r = 0;
-            long long je = -1;
-            float se = 0.f;
-            if (e < e_end) {
-                je = indices[e];
-                r = rank_out[e];
-                if (r > 0) se = adj[adj_index(i, je, n)];
-            }
-            int sub = 0;
-            bool hit = false;
-            for (int x0 = x_begin; x0 < x_end; x0 += 32) {
-                const int x = x0 + lane;
-                long long jx = -1;
-                float vx = 0.f;
-                if (x < x_end) {
-                    jx = ex_idx[x];
-                    vx = excluded_value(i, jx, undirected, adj, n);
-                }
-                const int cnt = min(32, x_end - x0);
-                for (int t = 0; t < cnt; t++) {
-                    const float vt = __shfl_sync(0xffffffffu, vx, t);
-                    const long long jt = __shfl_sync(0xffffffffu, jx, t);
-                    hit |= jt == je;
-                    sub += (vt > 0.f && (vt > se || (vt == se && jt < je))) ? 1 : 0;
-                }
-            }
-            if (e < e_end) rank_out[e] = (hit || r == 0) ? 0 : r - sub;
-        }
-    }
-}
-
-// bits[x] = bit pattern of excluded entry x when it is a candidate, else 0 (one warp per row)
-__global__ void __launch_bounds__(256)
-recon_exclude_values_kernel(int64_t n, const int32_t *__restrict__ ex_ptr, const int32_t *__restrict__ ex_idx,
-                            int undirected, const float *__restrict__ adj, uint32_t *__restrict__ bits) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t i = warp; i < n; i += nwarps)
-        for (int x = ex_ptr[i] + lane; x < ex_ptr[i + 1]; x += 32)
-            bits[x] = __float_as_uint(excluded_value(i, ex_idx[x], undirected, adj, n));
-}
-
-// keep the collected entries (i, j, w) that are not in row i of the exclusion (binary search of its sorted columns)
-__global__ void __launch_bounds__(256)
-recon_exclude_compact_kernel(int64_t m, const int32_t *__restrict__ ii, const int32_t *__restrict__ jj,
-                             const float *__restrict__ ww, const int32_t *__restrict__ ex_ptr,
-                             const int32_t *__restrict__ ex_idx, unsigned long long *__restrict__ counter, int64_t cap,
-                             int32_t *__restrict__ oi, int32_t *__restrict__ oj, float *__restrict__ ow) {
-    const int lane = threadIdx.x & 31;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    const int64_t t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    for (int64_t base_t = t0 - lane; base_t < m; base_t += stride) {      // whole warps iterate together
-        const int64_t t = base_t + lane;
-        bool keep = false;
-        int32_t i = 0, j = 0;
-        if (t < m) {
-            i = ii[t]; j = jj[t];
-            int lo = ex_ptr[i], hi = ex_ptr[i + 1];
-            while (lo < hi) {
-                const int mid = lo + (hi - lo) / 2;
-                if (ex_idx[mid] < j) lo = mid + 1; else hi = mid;
-            }
-            keep = !(lo < ex_ptr[i + 1] && ex_idx[lo] == j);
-        }
-        const unsigned mask = __ballot_sync(0xffffffffu, keep);
-        if (mask) {
-            unsigned long long base = 0;
-            if (lane == 0) base = atomicAdd(counter, (unsigned long long)__popc(mask));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (keep) {
-                const int64_t slot = (int64_t)base + __popc(mask & ((1u << lane) - 1u));
-                if (slot < cap) { oi[slot] = i; oj[slot] = j; ow[slot] = ww[t]; }
-            }
-        }
+// adj[off[t]] <-> saved[t]: with saved all 0 the first launch masks the excluded entries, the second restores them.
+// The offsets are distinct, so no two threads touch one entry.
+__global__ void recon_swap_kernel(int64_t m, const int64_t *__restrict__ off, float *__restrict__ saved,
+                                  float *__restrict__ adj) {
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) {
+        const float v = adj[off[t]];
+        adj[off[t]] = saved[t];
+        saved[t] = v;
     }
 }
 
@@ -443,36 +345,22 @@ static int decode_out(const gemb_recon *r, int64_t m, float *w) {
     return GEMB_OK;
 }
 
-// the bit patterns of the excluded candidates, sorted ascending, on the host (for count(>= T) during the bisection)
-static int excluded_sorted(gemb_recon *r, int undirected, std::vector<uint32_t> *out) {
-    out->clear();
-    if (!r->ex_ptr || r->ex_nnz == 0) return GEMB_OK;
-    gemb_ctx *c = r->ctx;
+static int swap_excluded(gemb_recon *r) {
     const int64_t m = r->ex_nnz;
-    GEMB_ARG(m < ((int64_t)1 << 31), "exclusion too large for one sort");
-    DeviceBuffer<uint32_t> bits, sorted;
-    DeviceBuffer<char> tmp;
-    GEMB_CUDA(bits.alloc((size_t)m));
-    GEMB_CUDA(sorted.alloc((size_t)m));
-    recon_exclude_values_kernel<<<grid_for(c, r->n * 32, 256), 256, 0, c->stream>>>(r->n, r->ex_ptr, r->ex_idx,
-                                                                                    undirected, r->adj, bits.get());
+    if (m == 0) return GEMB_OK;
+    recon_swap_kernel<<<grid_for(r->ctx, m, 256), 256, 0, r->ctx->stream>>>(m, r->ex_off, r->ex_saved, r->adj);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    size_t tb = 0;
-    GEMB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, bits.get(), sorted.get(), (int)m, 0, 32, c->stream));
-    GEMB_CUDA(tmp.alloc(std::max<size_t>(tb, 1)));
-    GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.get(), tb, bits.get(), sorted.get(), (int)m, 0, 32, c->stream));
-    count_launch();
-    std::vector<uint32_t> h((size_t)m);
-    GEMB_CUDA(cudaMemcpyAsync(h.data(), sorted.get(), sizeof(uint32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    out->assign(std::upper_bound(h.begin(), h.end(), 0u), h.end());   // 0 = not a candidate
     return GEMB_OK;
 }
 
-// number of sorted excluded values >= bits
-static int64_t excluded_ge(const std::vector<uint32_t> &ex, uint32_t bits) {
-    return (int64_t)(ex.end() - std::lower_bound(ex.begin(), ex.end(), bits));
+// run body() on the panels with the excluded entries set to 0, and restore them whatever body() returns; the first
+// error wins.  Without an exclusion, body() alone.
+template <class F> static int with_exclusion_masked(gemb_recon *r, F body) {
+    GEMB_TRY(swap_excluded(r));
+    const int st = body();
+    const int st_restore = swap_excluded(r);
+    return st != GEMB_OK ? st : st_restore;
 }
 
 }  // namespace gemb
@@ -563,8 +451,8 @@ int gemb_recon_free(gemb_recon *r) {
     if (!r) return GEMB_OK;
     cudaSetDevice(r->ctx->device);
     dfree(r->adj);
-    dfree(r->ex_ptr);
-    dfree(r->ex_idx);
+    dfree(r->ex_off);
+    dfree(r->ex_saved);
     delete r;
     return GEMB_OK;
 }
@@ -621,27 +509,23 @@ int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indice
     const int64_t nnz = indptr[n];
     GEMB_ARG(indptr[0] == 0 && nnz >= 0 && (nnz == 0 || (indices && rank_out)), "CSR");
     for (int64_t t = 0; t < nnz; t++) GEMB_ARG(indices[t] >= 0 && indices[t] < n, "column id out of range");
-    DeviceBuffer<int32_t> dp, dix, drank, dnp;
-    GEMB_CUDA(dp.alloc((size_t)(n + 1)));
-    GEMB_CUDA(dix.alloc((size_t)std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(drank.alloc((size_t)std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(dnp.alloc((size_t)n));
-    GEMB_CUDA(cudaMemcpyAsync(dp.get(), indptr, sizeof(int32_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, c->stream));
-    if (nnz) GEMB_CUDA(cudaMemcpyAsync(dix.get(), indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, c->stream));
-    recon_rank_kernel<<<grid_for(c, n * 32, 256), 256, 0, c->stream>>>(n, dp.get(), dix.get(), is_undirected ? 1 : 0, r->adj,
-                                                                       drank.get(), dnp.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    if (r->ex_ptr) {
-        recon_exclude_rank_kernel<<<grid_for(c, n * 32, 256), 256, 0, c->stream>>>(
-            n, dp.get(), dix.get(), r->ex_ptr, r->ex_idx, is_undirected ? 1 : 0, r->adj, drank.get(), dnp.get());
+    return with_exclusion_masked(r, [&]() -> int {
+        DeviceBuffer<int32_t> dp, dix, drank, dnp;
+        GEMB_CUDA(dp.alloc((size_t)(n + 1)));
+        GEMB_CUDA(dix.alloc((size_t)std::max<int64_t>(nnz, 1)));
+        GEMB_CUDA(drank.alloc((size_t)std::max<int64_t>(nnz, 1)));
+        GEMB_CUDA(dnp.alloc((size_t)n));
+        GEMB_CUDA(cudaMemcpyAsync(dp.get(), indptr, sizeof(int32_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, c->stream));
+        if (nnz) GEMB_CUDA(cudaMemcpyAsync(dix.get(), indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, c->stream));
+        recon_rank_kernel<<<grid_for(c, n * 32, 256), 256, 0, c->stream>>>(n, dp.get(), dix.get(), is_undirected ? 1 : 0,
+                                                                           r->adj, drank.get(), dnp.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-    }
-    if (nnz) GEMB_CUDA(cudaMemcpyAsync(rank_out, drank.get(), sizeof(int32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(n_pred_row, dnp.get(), sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+        if (nnz) GEMB_CUDA(cudaMemcpyAsync(rank_out, drank.get(), sizeof(int32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(n_pred_row, dnp.get(), sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        return GEMB_OK;
+    });
 }
 
 int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *ex_indices) {
@@ -649,33 +533,37 @@ int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *e
     gemb_ctx *c = r->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     const int64_t n = r->n;
+    std::vector<int64_t> off;
     if (ex_indptr) {
         const int64_t nnz = ex_indptr[n];
         GEMB_ARG(ex_indptr[0] == 0 && nnz >= 0 && (nnz == 0 || ex_indices), "exclusion CSR");
+        off.reserve((size_t)nnz);
         for (int64_t i = 0; i < n; i++) {
             GEMB_ARG(ex_indptr[i + 1] >= ex_indptr[i], "exclusion offsets non-decreasing");
             for (int64_t t = ex_indptr[i]; t < ex_indptr[i + 1]; t++) {
                 GEMB_ARG(ex_indices[t] >= 0 && ex_indices[t] < n, "exclusion column id out of range");
                 GEMB_ARG(t == ex_indptr[i] || ex_indices[t] > ex_indices[t - 1], "exclusion columns strictly ascending");
+                off.push_back((int64_t)adj_index(i, ex_indices[t], n));
             }
         }
     }
-    dfree(r->ex_ptr);
-    dfree(r->ex_idx);
-    r->ex_ptr = r->ex_idx = nullptr;
+    dfree(r->ex_off);
+    dfree(r->ex_saved);
+    r->ex_off = nullptr;
+    r->ex_saved = nullptr;
     r->ex_nnz = 0;
     r->top_valid = 0;
-    if (!ex_indptr) return GEMB_OK;
-    const int64_t nnz = ex_indptr[n];
-    DeviceBuffer<int32_t> dp, dix;
-    GEMB_CUDA(dp.alloc((size_t)(n + 1)));
-    GEMB_CUDA(dix.alloc((size_t)std::max<int64_t>(nnz, 1)));
-    GEMB_CUDA(cudaMemcpyAsync(dp.get(), ex_indptr, sizeof(int32_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, c->stream));
-    if (nnz) GEMB_CUDA(cudaMemcpyAsync(dix.get(), ex_indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, c->stream));
+    if (off.empty()) return GEMB_OK;
+    DeviceBuffer<int64_t> doff;
+    DeviceBuffer<float> dsaved;
+    GEMB_CUDA(doff.alloc(off.size()));
+    GEMB_CUDA(dsaved.alloc(off.size()));
+    GEMB_CUDA(cudaMemcpyAsync(doff.get(), off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemsetAsync(dsaved.get(), 0, sizeof(float) * off.size(), c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    r->ex_ptr = dp.release();
-    r->ex_idx = dix.release();
-    r->ex_nnz = nnz;
+    r->ex_off = doff.release();
+    r->ex_saved = dsaved.release();
+    r->ex_nnz = (int64_t)off.size();
     return GEMB_OK;
 }
 
@@ -686,76 +574,53 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
     gemb_ctx *c = r->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     const int und = is_undirected ? 1 : 0;
-    DeviceBuffer<unsigned long long> dcounter;
-    GEMB_CUDA(dcounter.alloc(1));
-    if (!(r->top_valid && r->top_und == und && r->top_k == max_k)) {
-        // with an exclusion set, every count is count(>= T) over all candidates minus the excluded values >= T
-        std::vector<uint32_t> ex;
-        GEMB_TRY(excluded_sorted(r, und, &ex));
-        int64_t raw = 0;
-        GEMB_TRY(count_ge(r, und, 1u, dcounter.get(), &raw));
-        const int64_t total = raw - excluded_ge(ex, 1u);
-        uint32_t bits = 1u;
-        int64_t count = total;
-        if (max_k >= 0 && total > max_k) {
-            // largest bit pattern T with count(>= T) >= max_k:  count(>= lo) >= K  and  count(>= hi) < K
-            uint32_t lo = 1u, hi = 0x7f800001u;
-            while (hi - lo > 1u) {
-                const uint32_t mid = lo + (hi - lo) / 2u;
-                int64_t cm = 0;
-                GEMB_TRY(count_ge(r, und, mid, dcounter.get(), &cm));
-                const int64_t kept = cm - excluded_ge(ex, mid);
-                if (kept >= std::max<int64_t>(max_k, 1)) { lo = mid; count = kept; raw = cm; } else { hi = mid; }
+    return with_exclusion_masked(r, [&]() -> int {
+        DeviceBuffer<unsigned long long> dcounter;
+        GEMB_CUDA(dcounter.alloc(1));
+        if (!(r->top_valid && r->top_und == und && r->top_k == max_k)) {
+            int64_t total = 0;
+            GEMB_TRY(count_ge(r, und, 1u, dcounter.get(), &total));
+            uint32_t bits = 1u;
+            int64_t count = total;
+            if (max_k >= 0 && total > max_k) {
+                // largest bit pattern T with count(>= T) >= max_k:  count(>= lo) >= K  and  count(>= hi) < K
+                uint32_t lo = 1u, hi = 0x7f800001u;
+                while (hi - lo > 1u) {
+                    const uint32_t mid = lo + (hi - lo) / 2u;
+                    int64_t cm = 0;
+                    GEMB_TRY(count_ge(r, und, mid, dcounter.get(), &cm));
+                    if (cm >= std::max<int64_t>(max_k, 1)) { lo = mid; count = cm; } else { hi = mid; }
+                }
+                bits = lo;
+                if (max_k == 0) count = 0;
             }
-            bits = lo;
-            if (max_k == 0) count = 0;
+            r->top_valid = 1; r->top_und = und; r->top_k = max_k; r->top_bits = bits; r->top_count = count;
         }
-        r->top_valid = 1; r->top_und = und; r->top_k = max_k; r->top_bits = bits; r->top_count = count;
-        r->top_raw = raw;
-    }
-    *m_out = r->top_count;
-    if (cap <= 0 || r->top_count <= 0) return GEMB_OK;
-    if (cap < r->top_count) {
-        set_error("gemb_recon_top: %lld entries reach the threshold, cap is %lld", (long long)r->top_count, (long long)cap);
-        return GEMB_ERR_ARG;
-    }
-    const int64_t m = r->top_count;
-    DeviceBuffer<int32_t> di, dj;
-    DeviceBuffer<float> dw;
-    GEMB_CUDA(di.alloc((size_t)m));
-    GEMB_CUDA(dj.alloc((size_t)m));
-    GEMB_CUDA(dw.alloc((size_t)m));
-    GEMB_CUDA(cudaMemsetAsync(dcounter.get(), 0, sizeof(unsigned long long), c->stream));
-    const int64_t n_panels = r->n_pad / PW;
-    if (!r->ex_ptr) {
+        *m_out = r->top_count;
+        if (cap <= 0 || r->top_count <= 0) return GEMB_OK;
+        if (cap < r->top_count) {
+            set_error("gemb_recon_top: %lld entries reach the threshold, cap is %lld", (long long)r->top_count, (long long)cap);
+            return GEMB_ERR_ARG;
+        }
+        const int64_t m = r->top_count;
+        DeviceBuffer<int32_t> di, dj;
+        DeviceBuffer<float> dw;
+        GEMB_CUDA(di.alloc((size_t)m));
+        GEMB_CUDA(dj.alloc((size_t)m));
+        GEMB_CUDA(dw.alloc((size_t)m));
+        GEMB_CUDA(cudaMemsetAsync(dcounter.get(), 0, sizeof(unsigned long long), c->stream));
+        const int64_t n_panels = r->n_pad / PW;
         recon_select_kernel<true><<<grid_for(c, n_panels * r->n * 32, 256), 256, 0, c->stream>>>(
             r->n, n_panels, und, r->top_bits, r->adj, dcounter.get(), m, di.get(), dj.get(), dw.get());
         GEMB_CUDA(cudaGetLastError());
         count_launch();
-    } else {
-        // gather every candidate >= T (excluded ones too), then keep those outside the exclusion
-        const int64_t m_raw = r->top_raw;
-        DeviceBuffer<int32_t> ri, rj;
-        DeviceBuffer<float> rw;
-        GEMB_CUDA(ri.alloc((size_t)m_raw));
-        GEMB_CUDA(rj.alloc((size_t)m_raw));
-        GEMB_CUDA(rw.alloc((size_t)m_raw));
-        recon_select_kernel<true><<<grid_for(c, n_panels * r->n * 32, 256), 256, 0, c->stream>>>(
-            r->n, n_panels, und, r->top_bits, r->adj, dcounter.get(), m_raw, ri.get(), rj.get(), rw.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-        GEMB_CUDA(cudaMemsetAsync(dcounter.get(), 0, sizeof(unsigned long long), c->stream));
-        recon_exclude_compact_kernel<<<grid_for(c, m_raw, 256), 256, 0, c->stream>>>(
-            m_raw, ri.get(), rj.get(), rw.get(), r->ex_ptr, r->ex_idx, dcounter.get(), m, di.get(), dj.get(), dw.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
-    GEMB_TRY(decode_out(r, m, dw.get()));
-    GEMB_CUDA(cudaMemcpyAsync(i_out, di.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(j_out, dj.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(w_out, dw.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+        GEMB_TRY(decode_out(r, m, dw.get()));
+        GEMB_CUDA(cudaMemcpyAsync(i_out, di.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(j_out, dj.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaMemcpyAsync(w_out, dw.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        return GEMB_OK;
+    });
 }
 
 }  // extern "C"

@@ -314,8 +314,9 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
  * to the device; ex_indptr == NULL clears it.  While it is set, gemb_recon_ranks and gemb_recon_top report their
  * results over the candidates NOT in it: a true edge that is itself excluded gets rank 0, n_pred_row counts only the
  * remaining candidates, and top selects among them.  Without an exclusion both are unchanged.  Setting or clearing it
- * drops the cached top selection.  Cost: ranks O(sum_i true_deg_i * ex_deg_i) gathers after the usual pass; top
- * sorts the excluded values once per call that selects and filters the collected entries by binary search. */
+ * drops the cached top selection.  Cost: ranks and top run their usual passes with the excluded entries set to 0
+ * for the length of the call -- one scatter over the exclusion before them and one after, which puts the values
+ * back, so gemb_recon_dense and gemb_recon_pairs never see the zeros. */
 int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *ex_indices);
 
 /* ---- wire formats (SURVEY 8(f) rank 2): the reference's text files, read and written natively and in parallel.

@@ -1,7 +1,8 @@
 """Link prediction on the GPU: the exclusion set of gemb_recon_exclude and evaluateStaticLinkPrediction.
 
   1. ranks, n_pred_row and top-k with an exclusion set are BIT-EXACT against oracle/linkpred_oracle.py run on the
-     matrix the GPU produced (for the Gaussian kind: on the order keys the device stores, which order as the score);
+     matrix the GPU produced (for the Gaussian kind: on the order keys the device stores, which order as the score),
+     and dense / pairs still return the unmasked values while the exclusion is set;
   2. an empty exclusion, and a cleared one, give exactly what the calls give without one;
   3. end to end with the repository's HOPE / LaplacianEigenmaps on the golden graphs and seeds: the split and the
      sample are the reference's, MAP is within 2e-3 of the reference's (the bar of test_gpu_recon.py), HostCSR and
@@ -100,6 +101,10 @@ def test_ranks_and_top_with_exclusion_exact(gpu_ctx, kind, n, d):
                 got = np.sort(ti.astype(np.int64) * n + tj)
                 assert np.array_equal(got, np.sort(i[sel] * n + j[sel]))
                 assert np.array_equal(tw, D[ti, tj])
+            # ranks and top zero the excluded entries only while they run: dense and pairs see the plain values
+            assert np.array_equal(rec.dense().view(np.uint32), D.view(np.uint32))
+            xr = np.repeat(np.arange(n), np.diff(xp))
+            assert np.array_equal(rec.pairs(xr, xi).view(np.uint32), D[xr, xi].view(np.uint32))
             # clearing gives back the plain results
             rec.exclude(None, None)
             r2, np2 = rec.ranks(tp, ti_, und)

@@ -1,6 +1,7 @@
 """oracle/linkpred_oracle.py pinned against the reference's own functions (goldens made by
 tests/golden/make_golden_linkpred.py): split, node_l, filtered list, precision curve and MAP exact given the golden X;
-and its vectorised forms against the statement-by-statement loops."""
+its vectorised forms against the statement-by-statement loops; and the identity the device's exclusion relies on:
+filtering out the training edges is setting their entries to 0."""
 import os
 import sys
 
@@ -8,6 +9,7 @@ import numpy as np
 import pytest
 
 from conftest import REPO, golden_path
+from test_gpu_linkpred import _case
 
 sys.path.insert(0, os.path.join(REPO, 'oracle'))
 import eval_gauss_oracle as go  # noqa: E402
@@ -18,8 +20,9 @@ CASES = ['linkpred_karate_hope', 'linkpred_sbm1024_hope', 'linkpred_sbm1024_hope
          'linkpred_randw200_split', 'linkpred_sbm1024_lap']
 
 
-def oracle_run(z):
-    """Steps 1-6 of the oracle with the golden's seed and X.  -> dict"""
+def oracle_inputs(z):
+    """Steps 1-3 of the oracle with the golden's seed and X: split, sample, reconstruct.
+    -> (adj of the sample, test and train EdgeSet of the sample, train and test masks of the edges, node_l)"""
     n = int(z['n'])
     e = z['edges']
     src, dst = e[:, 0].astype(np.int64), e[:, 1].astype(np.int64)
@@ -34,8 +37,14 @@ def oracle_run(z):
     Xs = z['X'][node_l]
     score = str(z['score'])
     adj = go.reconstruct_gaussian(Xs) if score == 'gaussian' else eo.reconstruct(Xs, score == 'split')
-    r = lo.evaluate(adj, lo.edge_set(ns, ute, vte), lo.edge_set(ns, utr, vtr), is_undirected=und)
-    r.update(train=e[tr], test=e[te], node_l=node_l)
+    return adj, lo.edge_set(ns, ute, vte), lo.edge_set(ns, utr, vtr), tr, te, node_l
+
+
+def oracle_run(z):
+    """Steps 1-6 of the oracle with the golden's seed and X.  -> dict"""
+    adj, test, train, tr, te, node_l = oracle_inputs(z)
+    r = lo.evaluate(adj, test, train, is_undirected=bool(z['is_undirected']))
+    r.update(train=z['edges'][tr], test=z['edges'][te], node_l=node_l)
     return r
 
 
@@ -49,6 +58,44 @@ def test_oracle_matches_reference_link_prediction(name):
     assert abs(r['MAP'] - float(z['MAP'])) < 1e-13
     assert np.array_equal(r['prec_curve'][:4096], z['prec_head'])
     assert np.array_equal(r['prec_curve'][::997], z['prec_stride'])
+
+
+def _assert_zeroing_is_filtering(adj, test, train, und):
+    """What gemb_recon_ranks / _top rely on: an entry that holds 0 is not a candidate, so ranks, n_pred_row and the
+    candidate list among the candidates not in train equal those on adj with the entries of train set to 0 and no
+    exclusion."""
+    masked = np.array(adj, dtype=np.float64)
+    masked[np.repeat(np.arange(train.n), np.diff(train.indptr)), train.indices] = 0
+    none = lo.edge_set(train.n, [], [])
+    for got, exp in zip(lo.ranks(masked, test, none, und), lo.ranks(adj, test, train, und)):
+        assert np.array_equal(got, exp)
+    full = eo.edge_list_from_adj(adj, is_undirected=und)
+    kept = lo.filtered(*full, train)
+    assert kept[0].size < full[0].size
+    for got, exp in zip(eo.edge_list_from_adj(masked, is_undirected=und), kept):
+        assert np.array_equal(got, exp)
+
+
+@pytest.mark.parametrize('name', CASES)
+def test_zeroed_training_entries_are_the_filter_on_goldens(name):
+    z = np.load(golden_path(name + '.npz'))
+    adj, test, train = oracle_inputs(z)[:3]
+    _assert_zeroing_is_filtering(adj, test, train, bool(z['is_undirected']))
+
+
+@pytest.mark.parametrize('und', [True, False])
+@pytest.mark.parametrize('kind', [0, 1, 2])
+def test_zeroed_training_entries_are_the_filter_on_corner_cases(kind, und):
+    """_case's corners: excluded entries tied with held-out ones, excluded entries at the max_k = 1 and 1000
+    thresholds, a row with every candidate excluded, held-out edges that are excluded."""
+    n = 500 + 100 * kind
+    rng = np.random.default_rng(n + kind)
+    X = rng.standard_normal((n, 16)) * (0.3 if kind != 2 else 0.6)
+    X[:50] = np.round(X[:50], 1)
+    X[100:150] = X[0:50]                                 # duplicated rows: exact ties
+    adj = go.reconstruct_gaussian(X, exact=False) if kind == 2 else eo.reconstruct(X, kind == 1, exact=False)
+    (tp, ti), (xp, xi) = _case(rng, n, adj, und)
+    _assert_zeroing_is_filtering(adj, eo.EdgeSet(n, tp, ti), eo.EdgeSet(n, xp, xi), und)
 
 
 def _graph(rng, n, m, sym):
