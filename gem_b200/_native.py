@@ -20,7 +20,7 @@ EXPORTS = [
     'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
-    'gemb_recon_exclude',
+    'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk',
 ]
 
 
@@ -58,6 +58,15 @@ class N2VStats(_Stats):
                 ('total_ms', ctypes.c_double), ('h2d_ms', ctypes.c_double), ('d2h_ms', ctypes.c_double),
                 ('comm_ms', ctypes.c_double), ('n_tokens', ctypes.c_int64), ('n_walks', ctypes.c_int64),
                 ('pairs', ctypes.c_int64), ('sgns_bytes', ctypes.c_double), ('walk_bytes', ctypes.c_double)]
+
+
+class NCStats(_Stats):
+    _fields_ = [('struct_size', ctypes.c_uint32), ('panels', ctypes.c_int32), ('evaluations', ctypes.c_int64),
+                ('max_iters', ctypes.c_int32), ('unconverged', ctypes.c_int64), ('constant', ctypes.c_int64),
+                ('eval_bytes', ctypes.c_double), ('total_ms', ctypes.c_double)]
+
+
+NC_CONVERGED, NC_CONSTANT, NC_MAXITER, NC_STALLED = 1, 2, 3, 4
 
 
 def lib():
@@ -117,6 +126,9 @@ def lib():
     L.gemb_recon_ranks.argtypes = [vp, vp, vp, ctypes.c_int, vp, vp]
     L.gemb_recon_top.argtypes = [vp, ctypes.c_int, i64, i64, vp, vp, vp, ctypes.POINTER(i64)]
     L.gemb_recon_exclude.argtypes = [vp, vp, vp]
+    L.gemb_nc_fit.argtypes = [vp, i64, ctypes.c_int, vp, vp, vp, ctypes.c_int, f64, f64, ctypes.c_int, vp, vp, vp,
+                              ctypes.POINTER(NCStats)]
+    L.gemb_nc_topk.argtypes = [vp, i64, ctypes.c_int, vp, ctypes.c_int, vp, vp, vp]
     _lib = L
     return L
 
@@ -462,3 +474,33 @@ class Reconstruction(_Handle):
         check(lib().gemb_recon_exclude(self._h, _ptr(indptr), _ptr(indices)))
 
     free = _Handle._release
+
+
+def nc_fit(ctx, X, indptr, labels, L, C=1.0, tol=1e-5, max_iter=1000):
+    """gemb_nc_fit: one-vs-rest logistic regression of the n x d rows X against the label CSR (indptr n + 1, strictly
+    ascending label ids per row).  -> (W L x (d + 1) fp64 with rows (w_c, b_c), iters, status, stats dict)"""
+    X = np.ascontiguousarray(X, dtype=np.float32)
+    indptr = np.ascontiguousarray(indptr, dtype=np.int64)
+    labels = np.ascontiguousarray(labels, dtype=np.int32)
+    n, d = X.shape
+    assert indptr.shape == (n + 1,) and labels.shape[0] >= int(indptr[-1])
+    W = np.empty((int(L), d + 1), dtype=np.float64)
+    iters = np.empty(int(L), dtype=np.int32)
+    status = np.empty(int(L), dtype=np.int32)
+    st = NCStats(struct_size=ctypes.sizeof(NCStats))
+    check(lib().gemb_nc_fit(ctx._h, n, d, _ptr(X), _ptr(indptr), _ptr(labels), int(L), float(C), float(tol),
+                            int(max_iter), _ptr(W), _ptr(iters), _ptr(status), ctypes.byref(st)))
+    return W, iters, status, st.as_dict()
+
+
+def nc_topk(ctx, X, W, koff):
+    """gemb_nc_topk: row i of X gets the koff[i + 1] - koff[i] labels of largest probability (ties to the larger
+    label), highest first, in CSR order.  Rows with k = 0 get nothing."""
+    X = np.ascontiguousarray(X, dtype=np.float32)
+    W = np.ascontiguousarray(W, dtype=np.float64)
+    koff = np.ascontiguousarray(koff, dtype=np.int64)
+    m, d = X.shape
+    assert W.ndim == 2 and W.shape[1] == d + 1 and koff.shape == (m + 1,)
+    out = np.empty(max(int(koff[-1]), 1), dtype=np.int32)
+    check(lib().gemb_nc_topk(ctx._h, m, d, _ptr(X), W.shape[0], _ptr(W), _ptr(koff), _ptr(out)))
+    return out[:int(koff[-1])]

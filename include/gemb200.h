@@ -319,6 +319,45 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
  * back, so gemb_recon_dense and gemb_recon_pairs never see the zeros. */
 int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *ex_indices);
 
+/* ---- node classification (upstream GEM's evaluateNodeClassification: OneVsRestClassifier(LogisticRegression()) and
+ * its TopKRanker; not in the reference checkout).  gemb_nc_fit replaces the one-vs-rest fit: for every label c, with
+ * s_i = +1 when row i carries c and -1 otherwise, the minimiser of
+ *     f_c(w, b) = 1/2 |w|^2 + C sum_i log(1 + exp(-s_i (w . x_i + b)))      (sklearn's objective; b not penalised)
+ * by batched L-BFGS (memory 10) on the device, labels in panels of 128.  Class c stops when
+ * max|grad f_c| <= tol * max|grad f_c(0, 0)|, or after max_iter accepted steps.
+ * X: host, n x d row-major fp32 (the training rows).  indptr (n + 1, int64) / labels (int32, strictly ascending per
+ * row, in [0, L)): the rows' labels.  W_out: L x (d + 1) fp64, row c = (w_c, b_c); a label with no positive training
+ * row gets w = 0, b = -inf (p = 0), one that every training row carries w = 0, b = +inf (p = 1) -- sklearn's
+ * _ConstantPredictor.  iters_out (L, or NULL): accepted L-BFGS steps per label.  status_out (L, or NULL):
+ * GEMB_NC_CONVERGED, _CONSTANT, _MAXITER (max_iter reached) or _STALLED (no acceptable step in 40 line-search trials).
+ * Two calls on the same device give the same bits. */
+#define GEMB_NC_CONVERGED 1
+#define GEMB_NC_CONSTANT 2
+#define GEMB_NC_MAXITER 3
+#define GEMB_NC_STALLED 4
+typedef struct {
+    uint32_t struct_size;  /* = sizeof(gemb_nc_stats) */
+    int32_t panels;        /* label panels of <= 128 solved */
+    int64_t evaluations;   /* panel function / gradient evaluations (each: apply, residual, Gram, L-BFGS step) */
+    int32_t max_iters;     /* largest iters_out */
+    int64_t unconverged;   /* labels stopped by max_iter or a stalled line search */
+    int64_t constant;      /* labels that are constant on the training rows */
+    double eval_bytes;     /* compulsory HBM bytes of the evaluations' launches: per evaluation
+                              n (8 d + 16 P + 8) + 4 nnz (P = panel width) */
+    double total_ms;       /* device time of the call (events), uploads included */
+} gemb_nc_stats;
+int gemb_nc_fit(gemb_ctx *ctx, int64_t n, int d, const float *X, const int64_t *indptr, const int32_t *labels, int L,
+                double C, double tol, int max_iter, double *W_out, int32_t *iters_out, int32_t *status_out,
+                gemb_nc_stats *stats);
+
+/* The TopKRanker prediction: for test row i (X: host, m x d fp32) the k_i = koff[i + 1] - koff[i] labels with the
+ * largest p = 1 / (1 + exp(-(w_c . x_i + b_c))) (fp64 from the decision value, whose product w . x is fp32), exact
+ * ties to the larger label index.  W: L x (d + 1) fp64 as gemb_nc_fit returns it.  pred_out (koff[m] int32): row i's
+ * labels at koff[i] .. koff[i + 1] - 1, highest p first.  A row with k_i = 0 gets nothing here (upstream predicts every
+ * label for it; the caller fills that in). */
+int gemb_nc_topk(gemb_ctx *ctx, int64_t m, int d, const float *X, int L, const double *W, const int64_t *koff,
+                 int32_t *pred_out);
+
 /* ---- wire formats (SURVEY 8(f) rank 2): the reference's text files, read and written natively and in parallel.
  * HOST code only -- these entry points need no GPU.
  * Edge list: every non-blank line "src dst [weight]" (loadGraphFromEdgeListTxt, graph_util.py:143-158: exactly three
