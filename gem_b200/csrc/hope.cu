@@ -456,6 +456,32 @@ static int katz_terms_for(double beta, double nrm, double katz_tol) {
     return std::max(1, std::min(J, 4096));
 }
 
+// The Katz terms J of S = sum_{j=1..J} (beta A)^j for the general solver and the 'SVD error' diagnostic: ||A||_2 by
+// power iteration; beta ||A||_2 * 1.02 < 1 bounds the terms a priori (katz_terms_for).  Above that bound the series
+// still converges when beta rho(A) < 1, and rho(A) of a directed graph can lie far below ||A||_2 (a DAG: rho = 0), so
+// probe_katz_terms measures the decay of the terms; GEMB_ERR_DIVERGE only when they do not decay.  probe = false
+// (symmetric A, where ||A||_2 = rho(A); the halo exchange) refuses at the bound.  Leaves work blocks 2..4 dirty.
+static int general_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t seed, bool probe, double *nrm_out,
+                              int *J_out) {
+    double nrm = 0.0;
+    GEMB_TRY(estimate_norm2(W, seed, W.buf[3], W.buf[4], W.buf[2], &nrm));
+    *nrm_out = nrm;
+    if ((double)beta * nrm * 1.02 < 1.0) {
+        *J_out = katz_terms_for(beta, nrm, katz_tol);
+        return GEMB_OK;
+    }
+    double rho = nrm;
+    int s = GEMB_ERR_DIVERGE;
+    if (probe) {
+        s = probe_katz_terms(W, beta, katz_tol, seed, W.buf[3], W.buf[4], J_out, &rho);
+        if (s != GEMB_OK && s != GEMB_ERR_DIVERGE) return s;
+    }
+    if (s != GEMB_OK)
+        set_error("beta * rho(A) ~ %.4g >= 1 (||A||_2 = %.4g): the Katz series (I - beta A)^-1 beta A does not "
+                  "converge; choose beta < %.4g", (double)beta * rho, nrm, 1.0 / std::max(rho, 1e-300));
+    return s;
+}
+
 // max over `cols` of || S^T P_j - Qs_j || / smax ;  scr0..2 are scratch blocks
 static int residual_check(HopeWork &W, float beta, int J, const float *P, const float *Qs, float *scr0, float *scr1,
                           float *scr2, const std::vector<int> &cols, double smax, float *out) {
@@ -1215,12 +1241,8 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
     count_launch();
     c->t_spmm.reset(); c->t_dense.reset(); c->t_comm.reset();
     double nrm = 0.0;
-    GEMB_TRY(estimate_norm2(W, seed ? seed : 1, W.buf[3], W.buf[4], W.buf[2], &nrm));
-    if ((double)beta * nrm * 1.02 >= 1.0) {
-        set_error("beta * ||A||_2 = %.4g >= 1: the Katz series does not converge", (double)beta * nrm);
-        return GEMB_ERR_DIVERGE;
-    }
-    const int J = katz_terms_for(beta, nrm, 1e-9);
+    int J = 0;
+    GEMB_TRY(general_katz_terms(W, beta, 1e-9, seed ? seed : 1, !g->symmetric, &nrm, &J));
     GEMB_TRY(clear_scratch(W));
     float *Z = W.buf[0], *SZ = W.buf[1], *LZ = W.buf[2];
     const int64_t total_cols = probe ? n_probe : n;
@@ -1370,24 +1392,9 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         if (hard_bound <= 0.0) hard_bound = nrm;
     }
     if (need_power) {
-        GEMB_TRY(estimate_norm2(W, o.seed, W.buf[3], W.buf[4], W.buf[2], &nrm));
-        if ((double)beta * nrm * 1.02 >= 1.0) {
-            // symmetric A: ||A||_2 = rho(A), the series diverges.  Otherwise look at the series itself (ADVICE r1).
-            int Jp = 0;
-            double rho = nrm;
-            int ps = GEMB_ERR_DIVERGE;
-            if (algo == 1 && !W.halo) {
-                ps = probe_katz_terms(W, beta, o.katz_tol, o.seed, W.buf[3], W.buf[4], &Jp, &rho);
-                if (ps != GEMB_OK && ps != GEMB_ERR_DIVERGE) return ps;
-            }
-            if (ps != GEMB_OK) {
-                set_error("beta * rho(A) ~ %.4g >= 1 (||A||_2 = %.4g): the Katz series (I - beta A)^-1 beta A does not "
-                          "converge; choose beta < %.4g", (double)beta * rho, nrm, 1.0 / std::max(rho, 1e-300));
-                return GEMB_ERR_DIVERGE;
-            }
-            if (J <= 0) J = Jp;
-        }
-        if (J <= 0) J = katz_terms_for(beta, nrm, o.katz_tol);
+        int Jg = 0;
+        GEMB_TRY(general_katz_terms(W, beta, o.katz_tol, o.seed, algo == 1 && !W.halo, &nrm, &Jg));
+        if (J <= 0) J = Jg;
         if (hard_bound <= 0.0) hard_bound = nrm;
         GEMB_TRY(clear_scratch(W));
     }

@@ -33,7 +33,7 @@ typedef enum {
     GEMB_ERR_CUDA = -1,      /* no device / CUDA runtime or kernel failure */
     GEMB_ERR_ARG = -2,       /* bad argument */
     GEMB_ERR_NOMEM = -3,     /* host or device allocation failed */
-    GEMB_ERR_DIVERGE = -4,   /* beta * ||A||_2 >= 1: Katz series does not converge */
+    GEMB_ERR_DIVERGE = -4,   /* beta * rho(A) >= 1: Katz series does not converge */
     GEMB_ERR_NCCL = -5,      /* NCCL missing or collective failed */
     GEMB_ERR_UNSUPPORTED = -6
 } gemb_status;
@@ -214,6 +214,8 @@ int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts *opts, floa
  *                  n <= ~10^4, the sizes at which the reference can run at all);
  *   n_probe  > 0 : Hutchinson estimate sqrt(mean_j ||(X1 X2^T - S) z_j||^2) over n_probe Rademacher vectors
  *                  (SURVEY H8), relative standard error ~ sqrt(2 / n_probe).
+ * S takes the Katz terms of gemb_hope's general solver (a directed graph with beta ||A||_2 >= 1 is accepted when the
+ * series converges, i.e. beta rho(A) < 1); GEMB_ERR_DIVERGE when it does not.
  * Single GPU (the graph uploaded with row0 = 0, n_local = n). */
 int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float *X, int n_probe, uint64_t seed,
                         double *err_out);

@@ -227,6 +227,37 @@ def recon_rel_err(X, Xref):
     return np.linalg.norm(X1 @ X2.T - ref) / max(np.linalg.norm(ref), 1e-300)
 
 
+def svd_error(A, beta, X, S=None):
+    """hope.py:38-40, 'SVD error (low rank)': || X1 X2^T - S ||_F with S = katz_dense(A, beta) (the reference writes
+    u diag(s) vt for X1 X2^T; the two are equal for its own embedding).  S: katz_dense(A, beta) computed already."""
+    X1, X2 = split_halves(np.asarray(X, dtype=np.float64))
+    S = katz_dense(A, beta) if S is None else S
+    return float(np.linalg.norm(X1 @ X2.T - S))
+
+
+def rademacher_probes(n, cols, seed, p0=0):
+    """n x cols matrix of +-1: column c is probe p0 + c of gemb_hope_svd_error's probe_block_kernel (the same 64-bit
+    hash of (seed, row, probe), in uint64 arithmetic that wraps as the kernel's does)."""
+    r = np.arange(n, dtype=np.uint64)[:, None]
+    p = (np.uint64(p0) + np.arange(cols, dtype=np.uint64))[None, :]
+    with np.errstate(over='ignore'):
+        h = np.uint64(seed) ^ (r * np.uint64(0x9E3779B97F4A7C15)) ^ (p * np.uint64(0xBF58476D1CE4E5B9))
+        h ^= h >> np.uint64(31)
+        h *= np.uint64(0x94D049BB133111EB)
+        h ^= h >> np.uint64(29)
+    return np.where((h & np.uint64(1)) != 0, 1.0, -1.0)
+
+
+def svd_error_probes(A, beta, X, n_probe, seed, S=None):
+    """The Hutchinson estimate of svd_error: sqrt(mean_j || E z_j ||^2), E = X1 X2^T - S, over the probes z_j of
+    rademacher_probes(n, n_probe, seed)."""
+    X1, X2 = split_halves(np.asarray(X, dtype=np.float64))
+    Z = rademacher_probes(X1.shape[0], n_probe, seed)
+    S = katz_dense(A, beta) if S is None else S
+    EZ = X1 @ (X2.T @ Z) - S @ Z
+    return float(np.sqrt(np.sum(EZ * EZ) / n_probe))
+
+
 def svd_residuals(A, beta, X, terms, sigma=None):
     """Size-independent property: for each triplet  ||S v - sigma u|| / sigma_max and
     ||S^T u - sigma v|| / sigma_max, with S applied matrix-free (fp64)."""

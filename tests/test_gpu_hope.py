@@ -24,7 +24,14 @@ def _fresh_hope(**kw):
     return HOPE(**kw)
 
 
-def test_karate_golden(gpu_ctx, hope_oracle):
+def _printed_svd_error(out):
+    """The value of hope.py:38-40's line in captured stdout."""
+    lines = [ln for ln in out.splitlines() if ln.startswith('SVD error (low rank): ')]
+    assert len(lines) == 1, out
+    return float(lines[0].split(': ', 1)[1])
+
+
+def test_karate_golden(gpu_ctx, hope_oracle, capsys):
     ho = hope_oracle
     G = load_karate_nx()
     gold = np.loadtxt(golden_path('karate_HOPE.txt'))
@@ -40,6 +47,23 @@ def test_karate_golden(gpu_ctx, hope_oracle):
     # get_edge_weight / get_reconstructed_adj follow the reference (hope.py:43-44)
     A = m.get_reconstructed_adj()
     assert abs(A[3, 5] - np.dot(X[3, :2], X[5, 2:])) < 1e-7 and A[4, 4] == 0
+    # the reference prints 0.053622; X is within 2e-6 of the optimum, whose error is stationary (Eckart-Young)
+    assert abs(_printed_svd_error(capsys.readouterr().out) - 0.053622) <= 2e-6
+
+
+def test_karate_svd_error_above_the_norm_bound(gpu_ctx, hope_oracle, capsys):
+    """Karate as the reference loads it is strictly upper triangular: rho(A) = 0 while beta ||A||_2 = 1.52 at
+    beta = 0.3.  The series is finite, the solver accepts it, and the reference prints 1.541227 for d = 4; so must
+    the plugin, rather than 'unavailable'."""
+    ho = hope_oracle
+    G = load_karate_nx()
+    m = _fresh_hope(d=4, beta=0.3, oversample=32, tol=1e-9, max_iters=60)
+    X = m.learn_embedding(graph=G)
+    Xo, so = ho.hope_dense_lapack(ho.adjacency_from_nx(G), 4, 0.3)
+    assert np.allclose(m._sigma, so, rtol=SIG_RTOL)
+    assert ho.recon_rel_err(X, Xo) < RECON_TOL
+    e = _printed_svd_error(capsys.readouterr().out)
+    assert abs(e - 1.541227) <= 1e-5 * 1.541227, e
 
 
 @pytest.mark.parametrize('algorithm', [1, 2])

@@ -33,7 +33,7 @@ def fake_native(monkeypatch):
     """Replaces _native.Context / DeviceGraph / graph_factorization; `log` lists every handle made, `cfg` sets whether
     the solve raises and whether it reports convergence."""
     from gem_b200 import _native
-    log, cfg = [], {'fail': False, 'converged': 1}
+    log, cfg = [], {'fail': False, 'converged': 1, 'svd_error_probes': []}
 
     class Context(_FakeHandle):
         def __init__(self, device=0):
@@ -54,6 +54,7 @@ def fake_native(monkeypatch):
             return np.zeros((self.n, d), np.float32) if out is None else out, np.zeros(d, np.float32), st
 
         def hope_svd_error(self, d, beta, X, n_probe=0, seed=1):
+            cfg['svd_error_probes'].append(n_probe)
             return 0.0
 
         def node2vec(self, nids, d, walk_len, num_walks, con_size, max_iter, p=1.0, q=1.0, seed=1, sequential=False,
@@ -150,6 +151,22 @@ def test_dtype_of_the_result(fake_native, name):
 def test_hope_returns_the_out_buffer_itself(fake_native):
     buf = np.empty((8, 4), np.float32)
     assert _model('HOPE').learn_embedding(graph=_graph(), out=buf) is buf
+
+
+@pytest.mark.parametrize('n', [4096, 4097])
+@pytest.mark.parametrize('setting', ['unset', True, False, 8])
+def test_hope_svd_error_selection(fake_native, capsys, n, setting):
+    """When HOPE computes hope.py:38-40's 'SVD error' line and how: exact (n_probe = 0) up to 4096 nodes, above that
+    only when svd_error_probes asks -- True for the exact value, an int for a Hutchinson estimate with that many
+    probes -- and never under svd_error_probes=False."""
+    import scipy.sparse as sp
+    _, cfg = fake_native
+    extra = {} if setting == 'unset' else {'svd_error_probes': setting}
+    A = sp.csr_matrix((np.ones(n - 1), (np.arange(n - 1), np.arange(1, n))), shape=(n, n))
+    _model('HOPE', **extra).learn_embedding(graph=A)
+    expected = {'unset': [0] if n <= 4096 else [], True: [0], False: [], 8: [0] if n <= 4096 else [8]}[setting]
+    assert cfg['svd_error_probes'] == expected
+    assert capsys.readouterr().out.count('SVD error (low rank): 0.000000') == len(expected)
 
 
 # ---- evaluateStaticGraphReconstruction on a NumPy reconstruction
