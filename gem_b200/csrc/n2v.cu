@@ -580,9 +580,15 @@ static int alias_and_walks(gemb_graph *g, const double *weights64, double p, dou
     return GEMB_OK;
 }
 
+// Every warp stages its walk in shared memory: warps x walk_len int32.
+static size_t sgns_smem_bytes(int threads, int walk_len) { return sizeof(int32_t) * (threads / 32) * (size_t)walk_len; }
+
 template <int NV, bool VEC>
 static int launch_sgns(gemb_ctx *c, const SgnsParams &P, int blocks, int threads) {
-    const size_t sh = sizeof(int32_t) * (threads / 32) * P.walk_len;
+    const size_t sh = sgns_smem_bytes(threads, P.walk_len);
+    // beyond the default 48 KB the kernel has to opt in (gemb_node2vec checked sh against the device's opt-in limit)
+    if (sh > 48 * 1024)
+        GEMB_CUDA(cudaFuncSetAttribute(sgns_kernel<NV, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
     sgns_kernel<NV, VEC><<<blocks, threads, sh, c->stream>>>(P);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
@@ -670,6 +676,20 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     GEMB_ARG(!(sequential && c->nranks > 1), "sequential parity mode is single-GPU");
+    // the SGNS kernel's limits, checked before any work: at most 16 values per lane, and the walks of a block in shared memory
+    if (d > 512) {
+        set_error("node2vec: d = %d is not supported (d <= 512)", d);
+        return GEMB_ERR_UNSUPPORTED;
+    }
+    const int threads = sequential ? 32 : 128;
+    int smem_optin = 0;
+    GEMB_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    if (sgns_smem_bytes(threads, walk_len) > (size_t)smem_optin) {
+        set_error("node2vec: walk_len = %d is not supported in %s mode (walk_len <= %d: the %d walk(s) trained by a block "
+                  "are kept in its shared memory, at most %d bytes on this device)", walk_len,
+                  sequential ? "sequential" : "Hogwild", smem_optin / (int)sgns_smem_bytes(threads, 1), threads / 32, smem_optin);
+        return GEMB_ERR_UNSUPPORTED;
+    }
     N2VDev D;
     CallEvents<6> ev;
     GEMB_CUDA(ev.create());
@@ -767,7 +787,6 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     P.syn_pos = D.syn_pos.get(); P.syn_neg = D.syn_neg.get(); P.KT = D.KT.get(); P.ent = D.ent.get(); P.V = V;
     P.seed = (uint32_t)seed; P.sequential = sequential ? 1 : 0;
     P.seq_state = D.seq_state.get(); P.pair_counter = D.pairs.get();
-    const int threads = 128;
     // Hogwild: concurrent walks race on embedding rows exactly as SNAP's OpenMP threads do.  Keep the
     // number of in-flight walks far below the vocabulary size so that lost updates stay as rare as in
     // the reference (<= 1 walk in flight per 32 tokens), up to 24 warps per SM.
@@ -776,7 +795,6 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
         const int64_t max_warps = std::max<int64_t>(1, V / 32);
         blocks = (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (max_warps + 3) / 4));
     }
-    const int threads_used = sequential ? 32 : threads;
     double comm_ms = 0;
     float *syn_pos = D.syn_pos.get(), *syn_neg = D.syn_neg.get(), *pos0 = D.pos0.get(), *delta = D.delta.get();
     for (int it = 0; it < max_iter; it++) {
@@ -786,7 +804,7 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
             GEMB_CUDA(cudaMemcpyAsync(pos0, syn_pos, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
             GEMB_CUDA(cudaMemcpyAsync(delta, syn_neg, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
         }
-        if (n_local > 0) GEMB_TRY(dispatch_sgns(c, P, blocks, threads_used));
+        if (n_local > 0) GEMB_TRY(dispatch_sgns(c, P, blocks, threads));
         if (c->nranks > 1) {
             // embedding-"gradient" all-reduce once per epoch: table <- table0 + sum_ranks (table_r - table0)
             NcclApi *api = nccl_api();

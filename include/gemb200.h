@@ -258,7 +258,10 @@ int gemb_n2v_walks(gemb_graph *g, const double *weights64, const int32_t *nids, 
 /* Full pipeline.  X_out: n_rows x d host fp32 (row = node id, like loadEmbedding; rows of ids
  * that never appear stay 0) or NULL.  sequential != 0 trains with ONE warp consuming the single
  * TRnd(seed) stream in program order (parity mode: follows oracle/n2v_oracle.c up to fp32
- * rounding); sequential == 0 is the Hogwild production mode. */
+ * rounding); sequential == 0 is the Hogwild production mode.  d <= 512.  Every warp keeps its walk
+ * in shared memory, so walk_len <= (the device's opt-in shared memory per block) / (4 * warps per
+ * block): 1 warp in sequential mode, 4 in Hogwild mode (58 112 and 14 528 on an H100).  Both
+ * limits are checked before any work (GEMB_ERR_UNSUPPORTED). */
 int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, int64_t N, int d,
                   int walk_len, int num_walks, int con_size, int max_iter, double p, double q,
                   int32_t seed, int sequential, int64_t n_rows, float *X_out,

@@ -251,9 +251,18 @@ static double tpower(double base, double ex) { return exp(log(base) * ex); }
  * Outputs: *V_out tokens; token_node[V] = node id of token; syn_pos V x d.
  * Caller passes token_node with capacity >= n_ids (max node id + 1) and
  * syn_pos capacity >= n_ids * d.  syn_neg_out nullable (same capacity).
+ * walk_streams 0: training continues the ONE TRnd(seed) stream of InitPosEmb,
+ *                 walk after walk (the single-threaded binary).
+ * walk_streams 1: walk wi of epoch `it` starts at position
+ *                   2^30 + (it * n_walks + wi) * walk_len * (1 + 20 * win)
+ *                 of TRnd(seed): the per-walk streams of the GPU's Hogwild mode
+ *                 (n2v.cu, sgns_kernel).  walk_len * (1 + 20 * win) bounds the
+ *                 draws of one walk: one window draw per word, ten per pair, at
+ *                 most 2 * win pairs per word.  With one walk per epoch the
+ *                 Hogwild result is then a deterministic function of this stream.
  */
 int n2v_oracle_learn(int32_t *walks, int64_t n_walks, int walk_len, int64_t n_ids,
-                     int d, int win, int iters, int32_t seed,
+                     int d, int win, int iters, int32_t seed, int walk_streams,
                      int64_t *V_out, int32_t *token_node, double *syn_pos, double *syn_neg_out) {
     int64_t tot = n_walks * walk_len;
     int32_t *rn = (int32_t*)malloc(sizeof(int32_t) * (n_ids > 0 ? n_ids : 1));
@@ -294,6 +303,10 @@ int n2v_oracle_learn(int32_t *walks, int64_t n_walks, int walk_len, int64_t n_id
     for (int it = 0; it < iters; it++) {
         for (int64_t wi = 0; wi < n_walks; wi++) {
             const int32_t *wk = walks + wi * walk_len;
+            if (walk_streams) {
+                const uint64_t stride = (uint64_t)walk_len * (uint64_t)(1 + 2 * win * N2V_NEG * 2);
+                rnd.seed = n2v_oracle_rng_skip(seed, 0x40000000ULL + ((uint64_t)it * (uint64_t)n_walks + (uint64_t)wi) * stride);
+            }
             for (int64_t wordI = 0; wordI < walk_len; wordI++) {
                 if (word_cnt % 10000 == 0) {
                     alpha = N2V_START_ALPHA * (1 - word_cnt / (double)((int64_t)iters * tot + 1));

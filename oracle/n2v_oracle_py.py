@@ -27,7 +27,7 @@ def lib():
                                        ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.c_int32,
                                        ctypes.c_int, i32p, ctypes.c_void_p]
         L.n2v_oracle_learn.argtypes = [i32p, ctypes.c_int64, ctypes.c_int, ctypes.c_int64, ctypes.c_int,
-                                       ctypes.c_int, ctypes.c_int, ctypes.c_int32,
+                                       ctypes.c_int, ctypes.c_int, ctypes.c_int32, ctypes.c_int,
                                        ctypes.POINTER(ctypes.c_int64), i32p, f64p, ctypes.c_void_p]
         L.n2v_oracle_rng_skip.argtypes = [ctypes.c_int32, ctypes.c_uint64]
         L.n2v_oracle_rng_skip.restype = ctypes.c_int32
@@ -68,16 +68,18 @@ def walks(indptr, indices, data, nids, walk_len, num_walks, p=1.0, q=1.0, seed=1
     return (out, order) if return_order else out
 
 
-def learn(walk_matrix, n_ids, d, win, iters, seed, return_neg=False):
+def learn(walk_matrix, n_ids, d, win, iters, seed, return_neg=False, walk_streams=False):
     """word2vec phase on a walk matrix (node ids).  Returns X (n_ids x d fp64, row = node id, rows of
-    ids that never occur are 0, exactly what loadEmbedding builds) and the token->node table."""
+    ids that never occur are 0, exactly what loadEmbedding builds) and the token->node table.
+    walk_streams=False: the binary's single TRnd stream; True: every walk of every epoch starts at its
+    own stream offset, as the GPU's Hogwild mode does (see n2v_oracle_learn)."""
     wm = np.array(walk_matrix, dtype=np.int32, order='C', copy=True)
     V = ctypes.c_int64(0)
     tok = np.zeros(n_ids, np.int32)
     sp = np.zeros((n_ids, d), np.float64)
     sn = np.zeros((n_ids, d), np.float64) if return_neg else None
-    rc = lib().n2v_oracle_learn(wm, wm.shape[0], wm.shape[1], n_ids, d, win, iters, int(seed), ctypes.byref(V),
-                                tok, sp, None if sn is None else sn.ctypes.data_as(ctypes.c_void_p))
+    rc = lib().n2v_oracle_learn(wm, wm.shape[0], wm.shape[1], n_ids, d, win, iters, int(seed), int(bool(walk_streams)),
+                                ctypes.byref(V), tok, sp, None if sn is None else sn.ctypes.data_as(ctypes.c_void_p))
     assert rc == 0
     V = V.value
     X = np.zeros((n_ids, d), np.float64)

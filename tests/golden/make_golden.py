@@ -20,7 +20,12 @@ What it writes
         oracle/_ref/libfaketime_shim.so (N2V_FAKE_TIME = seed) and OMP_NUM_THREADS=1, on several
         graphs (karate directed with dead ends; weighted symmetric; second-order p,q; id offset
         -> phantom node 0).  tests/test_oracle_n2v.py requires oracle/n2v_oracle.c to reproduce
-        them to the 6 significant digits the binary prints.
+        them to the 6 significant digits the binary prints.  The `*_d<d>` cases repeat a graph at a
+        wide embedding (d = 100 ... 256: the multi-value-per-lane SGNS kernels); they store the
+        printed embedding as float32, which holds its 6 digits, to keep the fixtures small.
+
+`python make_golden.py NAME ...` rewrites only the named fixtures (file names without .npz), so
+that adding a case leaves the bytes of the others alone.
 """
 import os
 import pickle
@@ -122,13 +127,15 @@ def rand_graph(rng, n, m, sym, weighted, offset=0):
     return G
 
 
-def main():
+def main(only=()):
     import networkx as nx
+    want = lambda name: not only or name in only
     subprocess.check_call(['make', '-C', os.path.join(REPO, 'oracle'), 'all', 'ref'])
     for a, b in [('tests/data/karate.edgelist', 'karate.edgelist'),
                  ('tests/karate_res/HOPE.txt', 'karate_HOPE.txt'),
                  ('tests/karate_res/node2vec.txt', 'karate_node2vec.txt')]:
-        shutil.copyfile(os.path.join(REF, a), os.path.join(HERE, b))
+        if want(b.rsplit('.', 1)[0]):
+            shutil.copyfile(os.path.join(REF, a), os.path.join(HERE, b))
 
     # --- SBM-1024 fixture + reference goldens
     Gs = load_sbm_nx()
@@ -138,9 +145,10 @@ def main():
     labels = np.asarray(lab.argmax(axis=1)).ravel().astype(np.int16)
     hope_gold = np.loadtxt(os.path.join(REF, 'tests/smb_res/HOPE.txt'))
     n2v_gold = np.loadtxt(os.path.join(REF, 'tests/smb_res/node2vec.txt')).astype(np.float32)
-    np.savez_compressed(os.path.join(HERE, 'sbm1024.npz'), nodes=nodes.astype(np.int32),
-                        src=src.astype(np.int32), dst=dst.astype(np.int32), labels=labels,
-                        hope_golden=hope_gold, node2vec_golden=n2v_gold)
+    if want('sbm1024'):
+        np.savez_compressed(os.path.join(HERE, 'sbm1024.npz'), nodes=nodes.astype(np.int32),
+                            src=src.astype(np.int32), dst=dst.astype(np.int32), labels=labels,
+                            hope_golden=hope_gold, node2vec_golden=n2v_gold)
 
     # --- reference HOPE class outputs
     rng = np.random.default_rng(2024)
@@ -150,6 +158,8 @@ def main():
     cases = {'karate_d4': (Gk, 4, 0.01), 'karate_d16': (Gk, 16, 0.05), 'sbm1024_d256': (Gs, 256, 0.01),
              'sbm1024_d16': (Gs, 16, 0.01), 'randw200_d32': (Gw, 32, 0.02), 'cliques_d24': (Gc, 24, 0.05)}
     for name, (G, d, beta) in cases.items():
+        if not want('ref_hope_' + name):
+            continue
         X = ref_hope(G, d, beta)
         nd, s, t, ww = edges_of(G)
         np.savez_compressed(os.path.join(HERE, 'ref_hope_%s.npz' % name), nodes=nd.astype(np.int32),
@@ -170,10 +180,19 @@ def main():
         'dirw50_pq': (Gdir, dict(d=6, walk_len=15, num_walks=3, con_size=4, max_iter=1, p=4.0, q=0.25, seed=7)),
         'offset40': (Goff, dict(d=6, walk_len=15, num_walks=3, con_size=4, max_iter=1, p=1.0, q=1.0, seed=31337)),
         'sbm128': (Gsb, dict(d=16, walk_len=40, num_walks=4, con_size=5, max_iter=1, p=1.0, q=1.0, seed=5)),
+        # wide d: scalar layout with a partial last value (100), float4 layouts (128, 256)
+        'sbm128_d100': (Gsb, dict(d=100, walk_len=40, num_walks=4, con_size=5, max_iter=1, p=1.0, q=1.0, seed=5)),
+        'sbm128_d128': (Gsb, dict(d=128, walk_len=40, num_walks=4, con_size=5, max_iter=1, p=1.0, q=1.0, seed=5)),
+        'symw60_pq_d256': (Gsym, dict(d=256, walk_len=15, num_walks=3, con_size=4, max_iter=1, p=0.5, q=2.0, seed=4242)),
+        'offset40_d128': (Goff, dict(d=128, walk_len=15, num_walks=3, con_size=4, max_iter=1, p=1.0, q=1.0, seed=31337)),
     }
     for name, (G, hp) in n2v_cases.items():
+        if not want('n2v_bin_' + name):
+            continue
         nd, s, t, ww = edges_of(G)
         ids, emb = run_n2v_binary(s, t, ww, **hp)
+        if hp['d'] >= 100:
+            emb = emb.astype(np.float32)
         np.savez_compressed(os.path.join(HERE, 'n2v_bin_%s.npz' % name), nodes=nd.astype(np.int32),
                             src=s.astype(np.int32), dst=t.astype(np.int32), w=ww, ids=ids, emb=emb,
                             **{k: np.array(v) for k, v in hp.items()})
@@ -181,4 +200,4 @@ def main():
 
 
 if __name__ == '__main__':
-    main()
+    main(set(sys.argv[1:]))

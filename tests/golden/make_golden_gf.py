@@ -41,9 +41,13 @@ def save(name, G, d, max_iter, eta, regu, seed):
 
 
 if __name__ == '__main__':
+    # `python make_golden_gf.py NAME ...` rewrites only the named fixtures (file names without .npz)
+    only = set(sys.argv[1:])
+    want = lambda name, d, it: not only or 'ref_gf_%s_d%d_it%d' % (name, d, it) in only
     K = mg.load_karate_nx().to_undirected().to_directed()      # tests/test_karate.py:35 works on G.to_directed()
     K = nx.convert_node_labels_to_integers(K, ordering='sorted') if sorted(K.nodes) != list(range(len(K.nodes))) else K
-    save('karate', K, 2, 300, 1e-2, 1.0, 7)
+    if want('karate', 2, 300):
+        save('karate', K, 2, 300, 1e-2, 1.0, 7)
     rng = np.random.default_rng(3)
     R = nx.DiGraph()
     R.add_nodes_from(range(60))
@@ -51,4 +55,6 @@ if __name__ == '__main__':
         u, v = int(rng.integers(0, 60)), int(rng.integers(0, 60))
         if u != v:
             R.add_edge(u, v, weight=float(np.round(rng.uniform(0.2, 2.0), 3)))
-    save('randw60', R, 8, 60, 2e-2, 0.05, 9)
+    for d in (8, 128):                    # d = 128: four values per lane in gf.cu
+        if want('randw60', d, 60):
+            save('randw60', R, d, 60, 2e-2, 0.05, 9)

@@ -36,7 +36,7 @@ def _nx_from(z):
     return G
 
 
-@pytest.mark.parametrize('name', ['ref_gf_karate_d2_it300', 'ref_gf_randw60_d8_it60'])
+@pytest.mark.parametrize('name', ['ref_gf_karate_d2_it300', 'ref_gf_randw60_d8_it60', 'ref_gf_randw60_d128_it60'])
 def test_reference_class_outputs(native_lib, name):
     z = np.load(golden_path(name + '.npz'))
     G = _nx_from(z)

@@ -12,7 +12,7 @@ sys.path.insert(0, os.path.join(REPO, 'oracle'))
 import gf_oracle as go
 
 
-@pytest.mark.parametrize('name', ['ref_gf_karate_d2_it300', 'ref_gf_randw60_d8_it60'])
+@pytest.mark.parametrize('name', ['ref_gf_karate_d2_it300', 'ref_gf_randw60_d8_it60', 'ref_gf_randw60_d128_it60'])
 def test_reference_class_outputs_bit_exact(name):
     z = np.load(golden_path(name + '.npz'))
     e = z['edges']

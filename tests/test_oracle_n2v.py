@@ -75,3 +75,98 @@ def test_walk_edge_cases(n2v_oracle):
     # walk_len = 1
     wm1 = n2v_oracle.walks(csr.indptr, csr.indices, csr.data, nids, 1, 2, seed=3, mode=1)
     assert wm1.shape == (8, 1) and sorted(wm1[:4, 0].tolist()) == [5, 6, 7, 8]
+
+
+def _learn_restated(walks, d, win, iters, seed, walk_streams):
+    """TrainModel statement by statement in plain Python fp64 (the C file's order, no FMA): the check of the oracle's
+    stream layouts.  walk_streams: walk wi of epoch it starts at 2^30 + (it*n_walks + wi) * L * (1 + 20*win)."""
+    import math
+    M = 2147483647
+    tok, rows = {}, []
+    for row in walks:
+        rows.append([tok.setdefault(int(x), len(tok)) for x in row])
+    V, L = len(tok), len(rows[0])
+    vocab = [0] * V
+    for row in rows:
+        for t in row:
+            vocab[t] += 1
+    st = [seed]
+
+    def uni():
+        st[0] = st[0] * 16807 % M
+        return st[0] / 2147483647.0
+    sp = [[(uni() - 0.5) / d for _ in range(d)] for _ in range(V)]
+    sn = [[0.0] * d for _ in range(V)]
+    prob = [math.exp(math.log(c) * 0.75) for c in vocab]
+    tw = 0.0
+    for x in prob:
+        tw += x
+    U = [x / tw * V for x in prob]
+    K = [0] * V
+    under = [i for i in range(V) if U[i] < 1]
+    over = [i for i in range(V) if U[i] >= 1]
+    while under and over:
+        small, large = under.pop(), over.pop()
+        K[small] = large
+        U[large] = U[large] + U[small] - 1
+        (under if U[large] < 1 else over).append(large)
+    for i in under + over:
+        U[i] = 1.0
+    alpha, word_cnt, tot = 0.025, 0, len(rows) * L
+    for it in range(iters):
+        for wi, wk in enumerate(rows):
+            if walk_streams:
+                st[0] = pow(16807, 2 ** 30 + (it * len(rows) + wi) * L * (1 + 20 * win), M) * seed % M
+            for pos in range(L):
+                if word_cnt % 10000 == 0:
+                    alpha = max(0.025 * (1 - word_cnt / float(iters * tot + 1)), 0.025 * 0.0001)
+                word = wk[pos]
+                uni()
+                offset = st[0] % win
+                for a in range(offset, 2 * win + 1 - offset):
+                    c = pos - win + a
+                    if a == win or c < 0 or c >= L:
+                        continue
+                    p, neu = sp[wk[c]], [0.0] * d
+                    for j in range(6):
+                        if j == 0:
+                            target, label = word, 1
+                        else:
+                            X = K[int(uni() * V)]
+                            target = X if uni() < U[X] else K[X]
+                            if target == word:
+                                continue
+                            label = 0
+                        q = sn[target]
+                        f = 0.0
+                        for i in range(d):
+                            f += p[i] * q[i]
+                        if f > 6:
+                            g = (label - 1) * alpha
+                        elif f < -6:
+                            g = label * alpha
+                        else:
+                            e = math.exp(math.log(2.718281828459045) * (-6.0 + (int(f * 10000) + 60000) / 10000.0))
+                            g = (label - 1 + 1 / (1 + e)) * alpha
+                        for i in range(d):
+                            neu[i] += g * q[i]
+                            q[i] += g * p[i]
+                    for i in range(d):
+                        p[i] += neu[i]
+                word_cnt += 1
+    return np.array(sp), [node for node, _ in sorted(tok.items(), key=lambda kv: kv[1])]
+
+
+@pytest.mark.parametrize('walk_streams', [False, True])
+def test_learn_stream_layouts_against_plain_restatement(n2v_oracle, walk_streams):
+    """Both stream layouts of the oracle's word2vec phase: the binary's single stream, and the per-walk streams the GPU's
+    Hogwild mode draws from (tests/test_gpu_n2v_widths.py compares the GPU with the latter).  Small vocabulary, so
+    negatives hit the centre word and get skipped; two epochs, so the epoch term of the stream offset is exercised."""
+    rng = np.random.default_rng(8)
+    walks = rng.integers(3, 12, size=(3, 9)).astype(np.int32)
+    X, tok = n2v_oracle.learn(walks, 12, 5, 3, 2, 777, walk_streams=walk_streams)
+    Xr, tok_r = _learn_restated(walks, 5, 3, 2, 777, walk_streams)
+    assert tok.tolist() == tok_r
+    assert np.allclose(X[tok], Xr, rtol=1e-12, atol=1e-15)
+    other, _ = n2v_oracle.learn(walks, 12, 5, 3, 2, 777, walk_streams=not walk_streams)
+    assert not np.allclose(X, other)                             # the two layouts really are different streams
