@@ -20,7 +20,8 @@ EXPORTS = [
     'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
-    'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk',
+    'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk', 'gemb_cc_create', 'gemb_cc_info', 'gemb_cc_labels', 'gemb_cc_lcc',
+    'gemb_cc_times', 'gemb_cc_free',
 ]
 
 
@@ -129,6 +130,12 @@ def lib():
     L.gemb_nc_fit.argtypes = [vp, i64, ctypes.c_int, vp, vp, vp, ctypes.c_int, f64, f64, ctypes.c_int, vp, vp, vp,
                               ctypes.POINTER(NCStats)]
     L.gemb_nc_topk.argtypes = [vp, i64, ctypes.c_int, vp, ctypes.c_int, vp, vp, vp]
+    L.gemb_cc_create.argtypes = [vp, i64, vp, vp, ctypes.POINTER(vp)]
+    L.gemb_cc_info.argtypes = [vp] + [ctypes.POINTER(i64)] * 4
+    L.gemb_cc_labels.argtypes = [vp, vp]
+    L.gemb_cc_lcc.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.gemb_cc_times.argtypes = [vp, ctypes.POINTER(f64), ctypes.POINTER(f64)]
+    L.gemb_cc_free.argtypes = [vp]
     _lib = L
     return L
 
@@ -504,3 +511,48 @@ def nc_topk(ctx, X, W, koff):
     out = np.empty(max(int(koff[-1]), 1), dtype=np.int32)
     check(lib().gemb_nc_topk(ctx._h, m, d, _ptr(X), W.shape[0], _ptr(W), _ptr(koff), _ptr(out)))
     return out[:int(koff[-1])]
+
+
+class Components(_Handle):
+    """The weakly connected components of an n x n CSR resident on the device: gemb_cc_* (include/gemb200.h).
+    indptr int64 (n + 1), indices int32.  n_comp, lcc_root (smallest vertex id of the largest component, -1 when
+    n = 0), lcc_size and lcc_nnz are read once at creation."""
+    _destroy = 'gemb_cc_free'
+
+    def __init__(self, ctx, n, indptr, indices):
+        indptr = np.ascontiguousarray(indptr, dtype=np.int64)
+        indices = np.ascontiguousarray(indices, dtype=np.int32)
+        assert indptr.shape == (int(n) + 1,)
+        self.ctx = ctx
+        self.n = int(n)
+        self._h = ctypes.c_void_p()
+        check(lib().gemb_cc_create(ctx._h, self.n, _ptr(indptr), _ptr(indices), ctypes.byref(self._h)))
+        v = [ctypes.c_int64(0) for _ in range(4)]
+        check(lib().gemb_cc_info(self._h, *(ctypes.byref(x) for x in v)))
+        self.n_comp, self.lcc_root, self.lcc_size, self.lcc_nnz = (int(x.value) for x in v)
+
+    def labels(self):
+        """Component number of every vertex, 0..n_comp - 1 in the order of each component's smallest vertex."""
+        out = np.empty(self.n, dtype=np.int32)
+        check(lib().gemb_cc_labels(self._h, _ptr(out)))
+        return out
+
+    def lcc(self, data=None):
+        """The largest component as a CSR: (node_l int64 ascending old rows, indptr int64, indices int32, weights
+        fp64 or None).  data: the nnz fp64 weights of the graph, or None (unit)."""
+        data = None if data is None else np.ascontiguousarray(data, dtype=np.float64)
+        k, m = self.lcc_size, self.lcc_nnz
+        node_l = np.empty(k, dtype=np.int64)
+        indptr = np.empty(k + 1, dtype=np.int64)
+        indices = np.empty(max(m, 1), dtype=np.int32)
+        w = None if data is None else np.empty(max(m, 1), dtype=np.float64)
+        check(lib().gemb_cc_lcc(self._h, _ptr(data), _ptr(node_l), _ptr(indptr), _ptr(indices), _ptr(w)))
+        return node_l, indptr, indices[:m], (None if w is None else w[:m])
+
+    def times(self):
+        """(device ms of the labelling, device ms of the last lcc extraction)"""
+        a, b = ctypes.c_double(0.0), ctypes.c_double(0.0)
+        check(lib().gemb_cc_times(self._h, ctypes.byref(a), ctypes.byref(b)))
+        return float(a.value), float(b.value)
+
+    free = _Handle._release

@@ -3,6 +3,9 @@ edges among the node pairs that are not training edges.
 
 The task, in the reference's own functions (rng = one np.random.RandomState(seed), or the global np.random):
     train, test = split_di_graph_to_train_test(G, train_ratio, is_undirected)      evaluation_util.py:39-53
+    [lcc=True, only when train has more than one weak component -- upstream GEM's step:
+     train, nodeListMap = get_lcc(train)                                            graph_util.py:29-34
+     test = test.subgraph(nodeListMap) relabelled by nodeListMap (HostCSR: induced_graph(test, node_l))]
     test, node_l = sample_graph(test, n_sample_nodes)  (optional; the train graph    graph_util.py:42-58
                    is induced on the same node_l, relabelled the same way)
     X = model.learn_embedding(graph=train)[node_l]
@@ -17,7 +20,8 @@ sampled-pairs branch the few pairs are filtered on the host.  No CPU fallback: w
 
 digraph: a networkx DiGraph with nodes 0..n-1 or a gem_b200.graph.HostCSR (then the split and the sample stay in
 CSR form: no networkx at any size).  The embedding's rows are taken as node ids, as evaluateStaticGraphReconstruction
-does.  -> (MAP, prec_curv)
+does.  With lcc=True the embedding is learned on the largest component, and node ids are its 0..k-1.  The default
+lcc=False keeps every node; on a training graph that is one component both give the same bits.  -> (MAP, prec_curv)
 """
 import numpy as np
 
@@ -27,18 +31,39 @@ from gem_b200.evaluation import metrics
 from gem_b200.evaluation.evaluate_graph_reconstruction import _true_csr
 
 
-def split_and_sample(digraph, train_ratio=0.8, n_sample_nodes=None, is_undirected=True, rng=None):
+def split_and_sample(digraph, train_ratio=0.8, n_sample_nodes=None, is_undirected=True, rng=None, lcc=False,
+                     device=None):
     """The host steps 1-2: -> (train, test_sampled, train_sampled, node_l).  train is the whole training graph (what
-    the model learns on); the sampled graphs are induced on node_l (all nodes when no sample is drawn)."""
+    the model learns on); the sampled graphs are induced on node_l (all nodes when no sample is drawn).  lcc=True:
+    when the training graph has more than one weak component, train is its largest one (get_lcc, on the GPU `device`
+    for a HostCSR), the test graph is induced on the same nodes with the same relabelling, and node_l indexes them."""
     from gem_b200.utils import evaluation_util, graph_util
     train, test = evaluation_util.split_di_graph_to_train_test(digraph, train_ratio, is_undirected, rng)
+    if lcc:
+        train, test = _largest_component(train, test, device)
     test_s, node_l = graph_util.sample_graph(test, n_sample_nodes, rng)
     train_s = train if test_s is test else graph_util.induced_graph(train, node_l)
     return train, test_s, train_s, np.asarray(node_l, dtype=np.int64)
 
 
+def _largest_component(train, test, device):
+    """(train, test) cut to train's largest weak component, or unchanged when train is one component."""
+    from gem_b200.graph import HostCSR
+    from gem_b200.utils import graph_util
+    if isinstance(train, HostCSR):
+        train_l, node_l = graph_util.get_lcc(train, device)
+        if train_l.n == train.n:
+            return train, test
+        return train_l, graph_util.induced_graph(test, node_l)
+    import networkx as nx
+    train_l, node_map = graph_util.get_lcc(train)
+    if len(node_map) == len(train):
+        return train, test
+    return train_l, nx.relabel_nodes(test.subgraph(list(node_map)), node_map, copy=True)
+
+
 def evaluateStaticLinkPrediction(digraph, graph_embedding, train_ratio=0.8, n_sample_nodes=None, sample_ratio_e=None,
-                                 is_undirected=True, max_k=-1, seed=None, device=None):
+                                 is_undirected=True, max_k=-1, seed=None, device=None, lcc=False):
     from gem_b200.graph import HostCSR
     kind = recon_kind(graph_embedding)
     if kind is None:
@@ -46,8 +71,9 @@ def evaluateStaticLinkPrediction(digraph, graph_embedding, train_ratio=0.8, n_sa
                         "_recon_score ('gaussian': lap.py:39-42)" % type(graph_embedding).__name__)
     gauss = kind == _native.RECON_GAUSS
     rng = None if seed is None else np.random.RandomState(seed)
-    train, test_s, train_s, node_l = split_and_sample(digraph, train_ratio, n_sample_nodes, is_undirected, rng)
-    node_num = digraph.n if isinstance(digraph, HostCSR) else len(digraph.nodes)
+    dev = device if device is not None else getattr(graph_embedding, '_device', 0)
+    train, test_s, train_s, node_l = split_and_sample(digraph, train_ratio, n_sample_nodes, is_undirected, rng, lcc, dev)
+    node_num = train.n if isinstance(train, HostCSR) else len(train.nodes)
     X = np.asarray(graph_embedding.learn_embedding(graph=train))
     if X.shape[0] != node_num:
         raise ValueError('embedding has %d rows, graph has %d nodes' % (X.shape[0], node_num))
@@ -56,7 +82,6 @@ def evaluateStaticLinkPrediction(digraph, graph_embedding, train_ratio=0.8, n_sa
     te_indptr, te_indices = _true_csr(test_s, n)
     tr_indptr, tr_indices = _true_csr(train_s, n)
     in_test = metrics.csr_has_edge(n, te_indptr, te_indices)
-    dev = device if device is not None else getattr(graph_embedding, '_device', 0)
     with _native.Context(dev) as ctx, _native.Reconstruction(ctx, X, kind) as rec:
         if sample_ratio_e:
             # evaluation_util.py:5-18 + :25-28, then the pairs that are training edges dropped

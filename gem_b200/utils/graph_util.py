@@ -7,7 +7,8 @@ The functions with the reference's names keep its signatures (networkx graphs in
 saveEmbedding use the native parallel reader / writer of libgemb200.so -- host code, no GPU needed -- and fall back
 to the per-line loop only when the library has not been built).  loadEdgeListCSR / saveEdgeListCSR / saveCSR / loadCSR
 go straight between files and gem_b200.graph.HostCSR, which is what a 20 M-edge input needs: the reference's
-per-line Python loops take minutes there (SURVEY 8(f) rank 2)."""
+per-line Python loops take minutes there (SURVEY 8(f) rank 2).  get_lcc (:29-34) takes either form; on a HostCSR it
+runs on the GPU."""
 import os
 
 import numpy as np
@@ -177,6 +178,66 @@ def saveEmbedding(X, file_name, ids=None):
         f.write('%d %d\n' % X.shape)
         for i in ids:
             f.write('%d %s\n' % (i, ' '.join('%g' % v for v in X[i])))
+
+
+def get_lcc(di_graph, device=None):
+    """gem/utils/graph_util.py:29-34: the largest weakly connected component, relabelled 0..k-1.
+    networkx DiGraph: the reference's recipe with the helper networkx 2.4 removed written out --
+        c = max(nx.weakly_connected_components(G), key=len); H = G.subgraph(c).copy()
+        nodeListMap = dict(zip(list(H.nodes), range(len(H))))
+    -> (H relabelled by nodeListMap, nodeListMap).  The relabelling makes a copy, so H's nodes iterate as 0..k-1 (the
+    reference relabels in place: same nodes, edges and map, but a scrambled node order, and every embedding takes
+    list(graph.nodes) as its row order).  Plain networkx, no device.  An undirected nx.Graph raises, as in the
+    reference.  On a tie the component whose first node comes first in G's node order wins.  H's node order (and so
+    the map) is the order networkx's subgraph view yields: G's node order when the component holds at least half of
+    G's nodes, the component set's own iteration order otherwise.
+    gem_b200.graph.HostCSR: labelled and cut on the device (gemb_cc_*), every stored edge joining its two ends.
+    -> (HostCSR of the component, node_l): node_l (int64, ascending) maps new row -> old row, as sample_graph's does;
+    `nodes` and `symmetric` are carried over.  On a tie the component with the smallest row wins -- the networkx
+    rule over row order.  device: the CUDA device (default 0)."""
+    from gem_b200.graph import HostCSR
+    if isinstance(di_graph, HostCSR):
+        return _lcc_csr(di_graph, 0 if device is None else int(device))
+    import networkx as nx
+    c = max(nx.weakly_connected_components(di_graph), key=len)
+    H = di_graph.subgraph(c).copy()
+    nodeListMap = dict(zip(list(H.nodes), range(len(H))))
+    return nx.relabel_nodes(H, nodeListMap, copy=True), nodeListMap
+
+
+def _check_csr(csr):
+    """The input rules of gemb_cc_create, raised as ValueError before any device call."""
+    n = int(csr.n)
+    if not 0 <= n < 2 ** 31:
+        raise ValueError('get_lcc: n = %d; vertex ids are int32 (n < 2^31)' % n)
+    indptr = np.asarray(csr.indptr)
+    if indptr.shape != (n + 1,):
+        raise ValueError('get_lcc: indptr has %d entries, n + 1 = %d' % (indptr.size, n + 1))
+    if int(indptr[0]) != 0:
+        raise ValueError('get_lcc: indptr[0] = %d, not 0' % int(indptr[0]))
+    if n and np.any(indptr[1:] < indptr[:-1]):
+        raise ValueError('get_lcc: indptr is not non-decreasing')
+    nnz = int(indptr[-1])
+    if np.asarray(csr.indices).shape[0] < nnz:
+        raise ValueError('get_lcc: indptr ends at %d, indices holds %d' % (nnz, np.asarray(csr.indices).shape[0]))
+    ix = np.asarray(csr.indices)[:nnz]
+    if nnz and (int(ix.min()) < 0 or int(ix.max()) >= n):
+        raise ValueError('get_lcc: a column id lies outside [0, %d)' % n)
+    if csr.data is not None and np.asarray(csr.data).shape[0] < nnz:
+        raise ValueError('get_lcc: %d weights for %d stored edges' % (np.asarray(csr.data).shape[0], nnz))
+
+
+def _lcc_csr(csr, device):
+    from gem_b200 import _native
+    from gem_b200.graph import HostCSR
+    _check_csr(csr)
+    nnz = int(csr.indptr[-1])
+    with _native.Context(device) as ctx, _native.Components(ctx, csr.n, csr.indptr, csr.indices[:nnz]) as cc:
+        node_l, indptr, indices, w = cc.lcc(None if csr.data is None else csr.data[:nnz])
+    nodes = csr.nodes
+    if nodes is not None:
+        nodes = nodes[node_l] if isinstance(nodes, np.ndarray) else [nodes[i] for i in node_l.tolist()]
+    return HostCSR(node_l.size, indptr, indices, w, nodes=nodes, symmetric=csr.symmetric), node_l
 
 
 def sample_graph(di_graph, n_sampled_nodes=None, rng=None):

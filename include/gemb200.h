@@ -363,6 +363,32 @@ int gemb_nc_fit(gemb_ctx *ctx, int64_t n, int d, const float *X, const int64_t *
 int gemb_nc_topk(gemb_ctx *ctx, int64_t m, int d, const float *X, int L, const double *W, const int64_t *koff,
                  int32_t *pred_out);
 
+/* ---- weakly connected components and the largest one (get_lcc, graph_util.py:29-34: the largest weakly connected
+ * component, relabelled 0..k-1 in node order).  One handle, so the CSR is uploaded once.
+ * gemb_cc_create uploads the n x n CSR (host: indptr n + 1 int64 with indptr[0] = 0, non-decreasing; indices int32 in
+ * [0, n); 0 <= n < 2^31) and labels it: every stored edge joins its two ends whatever its direction (self loops,
+ * isolated vertices and one-way edges allowed).  Bad input is GEMB_ERR_ARG before any device work.  Two calls give the
+ * same bits.
+ * gemb_cc_info: the number of components; the LCC -- the largest, the one with the smallest vertex id on a tie
+ * (= max(nx.weakly_connected_components(G), key=len) over row order) -- by its smallest vertex id, its vertex count
+ * and its stored edges.  n = 0: 0 components, lcc_root -1, size 0.  Any output pointer may be NULL.
+ * gemb_cc_labels: comp_out (n int32) = component number of every vertex, 0..n_comp-1 in the order of each
+ * component's smallest vertex.
+ * gemb_cc_lcc: the LCC as a CSR.  node_l_out (lcc_size int64): old row of every new row, ascending (new id = rank of
+ * the old id among the LCC's vertices, so column ids stay sorted within each row); indptr_out (lcc_size + 1 int64);
+ * indices_out (lcc_nnz int32, new ids); data (nnz fp64, or NULL = unit weights): data_out (lcc_nnz) gets the weights
+ * of the kept edges (not written when data is NULL).
+ * gemb_cc_times: device time of the labelling in gemb_cc_create and of the last gemb_cc_lcc's extraction (events
+ * around the kernels; the host copies are outside). */
+typedef struct gemb_cc gemb_cc;
+int gemb_cc_create(gemb_ctx *ctx, int64_t n, const int64_t *indptr, const int32_t *indices, gemb_cc **out);
+int gemb_cc_info(gemb_cc *cc, int64_t *n_comp, int64_t *lcc_root, int64_t *lcc_size, int64_t *lcc_nnz);
+int gemb_cc_labels(gemb_cc *cc, int32_t *comp_out);
+int gemb_cc_lcc(gemb_cc *cc, const double *data, int64_t *node_l_out, int64_t *indptr_out, int32_t *indices_out,
+                double *data_out);
+int gemb_cc_times(gemb_cc *cc, double *label_ms, double *extract_ms);
+int gemb_cc_free(gemb_cc *cc);
+
 /* ---- wire formats (SURVEY 8(f) rank 2): the reference's text files, read and written natively and in parallel.
  * HOST code only -- these entry points need no GPU.
  * Edge list: every non-blank line "src dst [weight]" (loadGraphFromEdgeListTxt, graph_util.py:143-158: exactly three
