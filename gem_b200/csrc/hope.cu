@@ -10,8 +10,10 @@
 //     repeat
 //         U  = S V                       J SpMM sweeps
 //         T  = U^T U ;  (theta, Z) = eigh(T)                   Ritz values theta = sigma^2
-//         stop if the top-k theta moved by <= tol * theta_max  (or max_iters)
-//         U <- U Z Theta^-1/2 (orthonormal Ritz vectors);  W = S^T U ;  V <- CholQR2(W)
+//         stop_rule 0: stop if every top-k sigma moved by <= tol relative  (or max_iters)
+//         U <- U Z Theta^-1/2 (orthonormal Ritz vectors);  W = S^T U
+//         stop_rule 1: stop if max_j ||S^T u_j - sigma_j v_j|| = sqrt((W^T W)_jj - theta_j) <= tol * sigma_max
+//         V <- CholQR2(W)
 //     sigma = sqrt(theta) ascending over the top k;  X = [ U Z_k theta^-1/4 | V Z_k theta^1/4 ]
 //
 //  SYMMETRIC (A = A^T, which gemb_graph_upload knows; algorithm = 2, the default for symmetric
@@ -77,6 +79,7 @@ struct HopeResult {
     DeviceBuffer<float> Xalloc;
     float *sig_dev = nullptr;  // k floats
     double sigma_max = 0.0;
+    double norm = 0.0;         // symmetric solvers: the spectrum bound the map ended with (SpecMap::norm)
 };
 
 // host <-> device staging: the copy, then a stream synchronise (the host reads the result, or its buffer goes out of scope)
@@ -546,6 +549,13 @@ static double sigma_change(const double *theta, const double *theta_prev, int k,
     return change;
 }
 
+// the same measure on signed values s (spectral_mode 1: the eigenvalues themselves), floored at 1e-3 smax, smax = max |s_j|
+static double value_change(const double *s, const double *s_prev, int k, double smax) {
+    double change = 0.0;
+    for (int j = 0; j < k; j++) change = std::max(change, fabs(s[j] - s_prev[j]) / std::max(fabs(s[j]), 1e-3 * smax));
+    return change;
+}
+
 // ------------------------------------------------------------------------------------ general solver
 static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, HopeResult &R) {
     gemb_ctx *c = W.c;
@@ -556,7 +566,16 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
     GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, T1));
     GEMB_TRY(cholqr2(W, T1, T2, V));
 
-    std::vector<double> theta(b), theta_prev(b, 0.0);
+    // stop_rule 1 tests the round's residual after the S^T sweep, and extraction then needs this round's U: the sweep
+    // takes its Horner scratch from a block of its own instead of U
+    DeviceBuffer<float> Hs;
+    float *Hscr = U;
+    if (o.stop_rule == 1) {
+        GEMB_CUDA(Hs.alloc((size_t)W.shard * b));
+        GEMB_CUDA(cudaMemsetAsync(Hs.get(), 0, sizeof(float) * (size_t)W.shard * b, c->stream));
+        Hscr = Hs.get();
+    }
+    std::vector<double> theta(b), theta_prev(b, 0.0), wdiag(b);
     for (int it = 1; it <= o.max_iters; it++) {
         R.iters = it;
         GEMB_TRY(katz(W, false, beta, J, V, U, T1, T2));              // U = S V
@@ -570,8 +589,10 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         if (o.verbose)
             fprintf(stderr, "[gemb_hope/general] it %d  sigma_max %.6g sigma_k %.6g  ritz change %.3g\n", it,
                     sqrt(tmax), sqrt(std::max(theta[b - k], 0.0)), change);
-        if (it >= o.min_iters && change <= (double)o.tol) { R.converged = 1; break; }
-        if (it == o.max_iters) break;
+        if (o.stop_rule == 0) {
+            if (it >= o.min_iters && change <= (double)o.tol) { R.converged = 1; break; }
+            if (it == o.max_iters) break;
+        }
         // T1 = U Z Theta^-1/2: exactly orthonormal columns (Z diagonalises U^T U), ordered by sigma, so the
         // next block S^T T1 ~ V Z Sigma has nearly orthogonal columns whatever the spread of sigma is
         GEMB_TRY(c->t_dense.begin(c->stream));
@@ -580,8 +601,25 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         count_launch();
         GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), b, b, T1, b));
         GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_TRY(katz(W, true, beta, J, T1, Wk, U, T2));              // Wk = S^T T1   (U is scratch now)
-        GEMB_TRY(cholqr2(W, Wk, T1, V));                              // V = orth(S^T orth(S V))
+        GEMB_TRY(katz(W, true, beta, J, T1, Wk, Hscr, T2));           // Wk = S^T T1   (stop_rule 0: U is scratch now)
+        if (o.stop_rule == 0) { GEMB_TRY(cholqr2(W, Wk, T1, V)); continue; }   // V = orth(S^T orth(S V))
+        // residual of the Ritz triplets (sigma_j, u_j = T1_j, v_j = V Z_j): S^T u_j = S^T S V Z_j theta_j^-1/2, so
+        // v_j^T S^T u_j = theta_j^1/2 = sigma_j and ||S^T u_j - sigma_j v_j||^2 = (Wk^T Wk)_jj - theta_j.  That Gram is
+        // the first one CholeskyQR2 forms; its diagonal is read before the Cholesky overwrites it.  S v_j - sigma_j u_j
+        // is 0 by construction (U = S V).
+        GEMB_TRY(gram_full(W, Wk, Wk, W.G.get()));
+        GEMB_CUDA(cudaMemcpy2DAsync(wdiag.data(), sizeof(double), W.G.get(), sizeof(double) * (b + 1), sizeof(double), b,
+                                    cudaMemcpyDeviceToHost, c->stream));
+        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        double worst = 0.0;
+        for (int j = b - k; j < b; j++) worst = std::max(worst, sqrt(std::max(wdiag[j] - theta[j], 0.0)) / sqrt(tmax));
+        R.resid_est = (float)worst;
+        if (o.verbose) fprintf(stderr, "[gemb_hope/general] it %d  residual %.3g\n", it, worst);
+        if (it >= o.min_iters && worst <= (double)o.tol) { R.converged = 1; break; }
+        if (it == o.max_iters) break;
+        GEMB_TRY(cholqr_pass(W, W.G.get(), Wk, T1));                 // the rest of V = CholeskyQR2(Wk)
+        GEMB_TRY(gram_full(W, T1, T1, W.G.get()));
+        GEMB_TRY(cholqr_pass(W, W.G.get(), T1, V));
     }
     R.sigma_max = sqrt(std::max(theta[b - 1], 0.0));
 
@@ -686,7 +724,16 @@ struct SpecMap {
     bool katz;
     double norm;    // a priori bound on |l|: ||A||_inf, or the power-iteration ||A||_2
     double bound;   // current bound on |l|
+    bool estimated = false;   // norm is the power-iteration estimate, which can lie below ||A||_2 (a cluster of top values)
     SpecMap(double beta, bool katz, double norm) : beta(beta), katz(katz), norm(norm), bound(norm * 1.02 + 1e-30) {}
+    // an estimated norm is raised to max |l| over the Ritz values l[0..n) (all inside the spectrum), so that the clamp
+    // never moves a Ritz value; false when then beta * norm >= 1 (the Katz series diverges)
+    bool observe(const double *l, int n) {
+        if (!estimated) return true;
+        for (int i = 0; i < n; i++) norm = std::max(norm, fabs(l[i]));
+        bound = std::max(bound, norm * 1.02 + 1e-30);
+        return !katz || beta * norm < 1.0;
+    }
     // bound from the Ritz values l[0..n): growth * max |l|, never above the a priori one
     void tighten(const double *l, int n, double growth) {
         double amax = 0.0;
@@ -697,6 +744,9 @@ struct SpecMap {
     double f(double l) const { return beta * l / (1.0 - beta * l); }
     // rank key, largest wanted first: |f(l)| (= sigma), or l + bound
     double key(double l) const { l = clamp(l); return katz ? fabs(f(l)) : l + bound; }
+    // the value the stop measures are taken on and relative to: the key sigma (Katz), the eigenvalue l (mode 1; its
+    // key carries the shift `bound`, which would make both measures ~2x looser on D^-1/2 A D^-1/2)
+    double value(double l) const { return katz ? key(l) : clamp(l); }
     // |d key / dl|: maps an eigen-residual of A to the residual of the key's triplet (|f'(l)| = beta / (1 - beta l)^2)
     double slope(double l) const { l = clamp(l); return katz ? beta / ((1.0 - beta * l) * (1.0 - beta * l)) : 1.0; }
     // Chebyshev filter interval [c0 - e, c0 + e] over the damped set {l : key(l) < key(l_min)}, l_min the block's Ritz
@@ -726,6 +776,12 @@ struct SpecMap {
 };
 
 constexpr int GEMB_SWITCH_TO_LANCZOS = 1000;   // internal status of hope_symmetric (algorithm = 0 on a skewed spectrum)
+
+static int diverge_error(const SpecMap &map) {
+    set_error("beta * ||A||_2 >= %.4g (a Ritz value of magnitude %.4g): the Katz series (I - beta A)^-1 beta A does not "
+              "converge; choose beta < %.4g", map.beta * map.norm, map.norm, 1.0 / map.norm);
+    return GEMB_ERR_DIVERGE;
+}
 
 // ritz_bound: A is symmetric with non-negative weights and map.norm = ||A||_inf; then lambda_max = rho(A) >= |lambda_min|
 // (Perron-Frobenius), so 1.05 * (largest Ritz value) bounds the spectrum on both sides and the 2 x 16 narrow SpMM sweeps
@@ -768,6 +824,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     }
 
     std::vector<double> lam(2 * b), gval(b), th_sorted(b), th_prev(b, 0.0);   // lam[b..2b): z^T (AV)^T (AV) z (stop rule 1)
+    std::vector<double> vals(b), vals_prev(b, 0.0);                            // mode 1: the eigenvalues in rank order
     std::vector<int> order(b);
 
     // scaled three-term Chebyshev recurrence of degree deg on [c0 - e, c0 + e], normalised at the dominant end by
@@ -806,12 +863,22 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         // the eigen-decomposition therefore stays on the critical path.)
         GEMB_TRY(ritz_eigh(W, o.tol, true, lam, o.stop_rule == 1 ? AV : nullptr));
         if (ritz_bound) map.tighten(lam.data(), b, 1.05);
+        else if (!map.observe(lam.data(), b)) return diverge_error(map);
+        R.norm = map.norm;
         for (int i = 0; i < b; i++) gval[i] = map.key(lam[i]);
         std::iota(order.begin(), order.end(), 0);
         std::sort(order.begin(), order.end(), [&](int a, int c2) { return gval[a] > gval[c2]; });   // descending key
         for (int i = 0; i < b; i++) th_sorted[i] = gval[order[i]] * gval[order[i]];
         const double tmax = std::max(th_sorted[0], 1e-300);
-        const double change = sigma_change(th_sorted.data(), th_prev.data(), k, tmax);
+        // vmax: max |value| over the wanted pairs (Katz: sigma_max = gval[order[0]])
+        double vmax = 0.0;
+        for (int j = 0; j < k; j++) vmax = std::max(vmax, fabs(map.value(lam[order[j]])));
+        double change;
+        if (mode) {
+            for (int i = 0; i < b; i++) vals[i] = map.value(lam[order[i]]);
+            change = value_change(vals.data(), vals_prev.data(), k, vmax);
+            vals_prev = vals;
+        } else change = sigma_change(th_sorted.data(), th_prev.data(), k, tmax);
         R.change = change;
         th_prev = th_sorted;
         // algorithm = 0 (auto): a first Rayleigh-Ritz round whose wanted values already span more than 3x -- a
@@ -824,12 +891,13 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         if (o.stop_rule == 1) {
             // residual of the Ritz pairs from the Rayleigh-Ritz products alone: with V orthonormal and (l, z) an
             // eigenpair of V^T A V,  ||A V z - l V z||^2 = z^T (AV)^T (AV) z - l^2.  Mapped to the Katz operator
-            // through |f'(l)| = beta / (1 - beta l)^2 and measured against sigma_max, like compute_residual does.
+            // through |f'(l)| = beta / (1 - beta l)^2 and measured against sigma_max, like compute_residual does;
+            // mode 1: ||A v - l v|| against max |l| over the wanted pairs.
             double worst = 0.0;
             for (int j = 0; j < k; j++) {
                 const int col = order[j];
                 const double r2 = std::max(lam[b + col] - lam[col] * lam[col], 0.0);
-                worst = std::max(worst, map.slope(lam[col]) * sqrt(r2) / std::max(gval[order[0]], 1e-300));
+                worst = std::max(worst, map.slope(lam[col]) * sqrt(r2) / std::max(vmax, 1e-300));
             }
             stop_measure = worst;
             R.resid_est = (float)worst;
@@ -1405,9 +1473,11 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     const bool lanczos_fits = g->n >= 2048;
     // a priori spectrum bound: ||A||_inf for Lanczos; for Chebyshev see hope_symmetric
     const SpecMap lanczos_map(beta, true, hard_bound);
+    SpecMap sym_map(beta, o.spectral_mode == 0, ritz_bound ? hard_bound : nrm);
+    sym_map.estimated = !ritz_bound;                              // else ||A||_inf: a true bound
     if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, lanczos_map, R);
     else if (algo >= 2) {
-        s = hope_symmetric(W, o, d, SpecMap(beta, o.spectral_mode == 0, ritz_bound ? hard_bound : nrm), ritz_bound, R);
+        s = hope_symmetric(W, o, d, sym_map, ritz_bound, R);
         if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, lanczos_map, R); }
     } else s = hope_general(W, o, d, beta, J, R);
     if (s != GEMB_OK) return s;
@@ -1462,7 +1532,8 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         stats->total_ms = total_ms;
         stats->h2d_ms = 0.0;
         stats->d2h_ms = d2h_ms;
-        stats->norm2_A = (float)(ritz_bound ? hard_bound : nrm);   /* ||A||_inf when no power iteration ran */
+        /* ||A||_inf when no power iteration ran; else the power-iteration estimate, raised to the largest |Ritz value| */
+        stats->norm2_A = (float)(ritz_bound ? hard_bound : std::max(nrm, R.norm));
         stats->beta_used = beta;
         stats->ritz_change = (float)R.change;
         stats->resid_max = R.resid_max;

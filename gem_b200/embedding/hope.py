@@ -89,10 +89,12 @@ class HOPE(StaticGraphEmbedding):
                     print('SVD error (low rank): unavailable (%s)' % exc)
         self.stats = st
         self._sigma = sigma
-        self._check_converged(st, 'HOPE: the solver stopped at max_iters=%d without meeting tol=%g (singular values still '
-                              'moving by %.3g per round); the embedding is less accurate than requested -- raise max_iters / '
-                              'oversample or use algorithm=3 on power-law graphs'
-                              % (st['iters'], opts.get('tol', 1e-6), st['ritz_change']))
+        # the measure the solver stopped on: algorithm 3 always stops on its residual estimate
+        measure = ('residual estimate %.3g' % st['resid_est'] if opts.get('stop_rule', 0) == 1 or st.get('algorithm') == 3 else
+                   'singular values still moving by %.3g relative per round' % st['ritz_change'])
+        self._check_converged(st, 'HOPE: the solver stopped at max_iters=%d without meeting tol=%g (%s); the embedding is '
+                              'less accurate than requested -- raise max_iters / oversample or use algorithm=3 on power-law '
+                              'graphs' % (st['iters'], opts.get('tol', 1e-6), measure))
         self._result(X, csr.n)
         if getattr(self, '_verbose', 0):
             print('HOPE: algorithm %d, %d iterations, J=%d Katz terms, block %d, ritz change %.3g, converged %d' %

@@ -8,8 +8,9 @@ eigenvectors come from the d+1 LARGEST algebraic eigenpairs of A_hat = D^-1/2 W 
 that have edges), computed by the Chebyshev-filtered subspace iteration of libgemb200.so (gemb_hope with
 opts.spectral_mode = 1: the CSR SpMM, tensor-core Gram / apply and Rayleigh-Ritz kernels HOPE uses) -- no shift-invert, no CPU path.
 
-Extra, optional hyper-parameters: tol (default 1e-6: relative change of every wanted eigenvalue between two Rayleigh-Ritz rounds;
-stop_rule=1 switches to the residual estimate, which fp32 Gram matrices cannot certify below ~3e-4), max_iters, oversample,
+Extra, optional hyper-parameters: tol (default 1e-6: change of every wanted eigenvalue of A_hat between two Rayleigh-Ritz rounds,
+relative to itself and at least 1e-3 max|eigenvalue|; stop_rule=1 switches to the residual estimate
+max_j ||A_hat v_j - l_j v_j|| / max_j |l_j|, which fp32 Gram matrices cannot certify below ~6e-4), max_iters, oversample,
 cheb_degree, cheb_range_log2, seed, device, dtype, strict, verbose.
 `graph` may also be a scipy.sparse matrix or a gem_b200.graph.HostCSR (rows = 0..n-1)."""
 import numpy as np
@@ -77,8 +78,10 @@ def spectral_solve(model, op, d, name):
             _native.DeviceGraph(ctx, op.n, op.indptr, op.indices, op.data_f32()) as g:
         V, lam, st = g.hope(d + 1, 0.0, spectral_mode=1, **opts)
     model.stats = st
-    model._check_converged(st, '%s: the solver stopped at max_iters=%d without meeting tol=%g (eigenvalues still moving '
-                           'by %.3g per round)' % (name, st['iters'], opts['tol'], st['ritz_change']), stacklevel=4)
+    measure = ('residual estimate %.3g' % st.get('resid_est', -1.0) if opts.get('stop_rule', 0) == 1 else
+               'eigenvalues still moving by %.3g relative per round' % st['ritz_change'])
+    model._check_converged(st, '%s: the solver stopped at max_iters=%d without meeting tol=%g (%s)'
+                           % (name, st['iters'], opts['tol'], measure), stacklevel=4)
     return V, lam
 
 

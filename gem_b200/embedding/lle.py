@@ -11,7 +11,9 @@ tensor-core Gram / apply and Rayleigh-Ritz kernels HOPE and LaplacianEigenmaps r
 host (scipy.sparse product P^T P, sum_v deg(v)^2 entries -- fine for bounded degrees, not for power-law hubs); applying M and M^T as
 two fused sweeps inside the solver instead is the next step (DESIGN.md section 9).  No CPU path for the solve.
 
-Extra, optional hyper-parameters: tol (default 1e-6), max_iters, oversample, cheb_degree, cheb_range_log2, seed, device, dtype, strict."""
+Extra, optional hyper-parameters: tol (default 1e-6: change of every wanted eigenvalue of C between two Rayleigh-Ritz rounds,
+relative to itself and at least 1e-3 max|eigenvalue|, as in lap.py; stop_rule=1: the residual estimate
+max_j ||C v_j - l_j v_j|| / max_j |l_j|), max_iters, oversample, cheb_degree, cheb_range_log2, seed, device, dtype, strict."""
 import numpy as np
 
 from gem_b200 import graph as _graph

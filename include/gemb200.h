@@ -160,11 +160,20 @@ typedef struct {
     float cheb_range_log2; /* algorithm 2: the filter degree is lowered until the filtered block's column dynamic range
                               T_m(x_L) stays below 2^cheb_range_log2 (fp32 Gram-based orthonormalisation squares it);
                               0 = default (8) */
-    int32_t stop_rule;     /* 0 = relative change of every singular value <= tol (default);
-                              1 = residual: max_j ||S v_j - sigma_j u_j|| / sigma_max <= tol over the top k, estimated
-                                  from the Rayleigh-Ritz products (algorithm 2: |f'(l_j)| ||A v_j - l_j v_j||) */
+    int32_t stop_rule;     /* algorithms 1 and 2 (algorithm 3 always stops on its residual, whatever this says):
+                              0 = change: max_j |s_j - s_j'| / max(|s_j|, 1e-3 max|s|) <= tol between two rounds, s the k
+                                  singular values (spectral_mode 1: the d eigenvalues) (default);
+                              1 = residual <= tol over the top k, estimated from the products the round forms anyway:
+                                  algorithm 1: max_j ||S^T u_j - sigma_j v_j|| / sigma_max, from the diagonal of the
+                                  Gram of S^T U (S v_j - sigma_j u_j is 0 by construction); algorithm 2:
+                                  max_j |f'(l_j)| ||A v_j - l_j v_j|| / sigma_max, from z^T (AV)^T (AV) z - l^2
+                                  (||S v_j - sigma_j u_j|| is at most kappa_j = (1 - beta l_j) / (1 - beta l_max) >= 1
+                                  times its term); spectral_mode 1: max_j ||A v_j - l_j v_j|| / max_j |l_j|.
+                                  Both are differences of fp32-accurate Gram entries: they do not resolve residuals
+                                  below ~6e-4 */
     int32_t algorithm3_basis; /* algorithm 3 (thick-restart block Lanczos on A, symmetric A): maximum basis width,
-                              0 = default (max(2k + 64, 192) rounded to the block) */
+                              0 = default (max(2 k_keep, 160), k_keep = k + 16 rounded up to a multiple of 16);
+                              rounded up to a multiple of 16 */
     int32_t spectral_mode; /* 0 = HOPE (top d/2 singular triplets of the Katz operator).
                               1 = the d largest ALGEBRAIC eigenpairs of the uploaded symmetric matrix itself, on the same
                               Chebyshev-filtered subspace iteration (beta ignored): X_out = n x d eigenvectors in DESCENDING
@@ -188,9 +197,12 @@ typedef struct {
     double total_ms;       /* device time of the whole call (events), excluding H2D/D2H */
     double h2d_ms, d2h_ms;
     float norm2_A;         /* estimated ||A||_2 */
-    float ritz_change;     /* last max relative Ritz-value change */
-    float resid_max;       /* max_j ||S^T u_j - sigma_j v_j|| / sigma_max (compute_residual=1) */
-    float resid_est;       /* stop_rule = 1: the residual estimate the last round stopped on (else -1) */
+    float ritz_change;     /* algorithms 1 and 2: the last round's change measure (stop_rule 0 above), whichever rule
+                              stopped; algorithm 3: the last restart's residual estimate (= resid_est) */
+    float resid_max;       /* max_j ||S^T u_j - sigma_j v_j|| / sigma_max (compute_residual=1; spectral_mode 0) */
+    float resid_est;       /* the residual estimate of the last round (stop_rule 1 above; algorithm 3: max_j
+                              |f'(l_j)| ||A v_j - l_j v_j|| / sigma_max from the Lanczos coupling block, computed for
+                              either stop_rule), else -1 */
     int32_t mg_mode;       /* 0 = single GPU; 1 = all-gather of the block per sweep; 2 = needed-rows-only exchange over
                               NVLink peer memory (CUDA IPC): rows are stored into the peers' halo slots by the kernel
                               that produces them.  3 (fp16 halo copies) is no longer produced. */

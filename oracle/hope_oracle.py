@@ -258,6 +258,71 @@ def svd_error_probes(A, beta, X, n_probe, seed, S=None):
     return float(np.sqrt(np.sum(EZ * EZ) / n_probe))
 
 
+def katz_pairs(beta, X, sigma):
+    """The eigenpairs of a symmetric A behind an embedding of the symmetric solvers (algorithms 2 and 3), whose columns are
+    X = [v sign(f) sqrt(sigma) | v sqrt(sigma)] with f = f(l) = beta l / (1 - beta l):
+        v_q = X[:, k+q] / sqrt(sigma_q), normalised (norm_dev_q = | ||v_q|| - 1 | before that),
+        s_q = sign(X[:, q] . X[:, k+q]),  f_q = s_q sigma_q,  l_q = f_q / (beta (1 + f_q)).
+    Returns (V n x k, l, s, norm_dev), all fp64."""
+    X = np.asarray(X, dtype=np.float64)
+    k = X.shape[1] // 2
+    sig = np.asarray(sigma, dtype=np.float64)
+    V = X[:, k:] / np.sqrt(np.maximum(sig, 1e-300))[None, :]
+    nrm = np.linalg.norm(V, axis=0)
+    s = np.sign(np.sum(X[:, :k] * X[:, k:], axis=0))
+    s[s == 0] = 1.0
+    f = s * sig
+    return V / nrm[None, :], f / (beta * (1.0 + f)), s, np.abs(nrm - 1.0)
+
+
+def eig_residuals(A, V, l):
+    """||A v_q - l_q v_q|| per column, fp64."""
+    V = np.asarray(V, dtype=np.float64)
+    return np.linalg.norm(A @ V - V * np.asarray(l, dtype=np.float64)[None, :], axis=0)
+
+
+def katz_slope(beta, l):
+    """|f'(l)| = beta / (1 - beta l)^2: maps an eigen-residual of A to the residual of the Katz triplet."""
+    return beta / (1.0 - beta * np.asarray(l, dtype=np.float64)) ** 2
+
+
+def katz_kappa(beta, l, lmax):
+    """kappa_q = (1 - beta l_q) / (1 - beta lambda_max): with f(lam) - f(l) = beta (lam - l) / ((1 - beta lam)(1 - beta l)),
+    ||S v - f(l) v|| <= kappa_q slope(l_q) ||A v - l_q v||, with equality when v mixes only x(l_q) and x(lambda_max)."""
+    return (1.0 - beta * np.asarray(l, dtype=np.float64)) / (1.0 - beta * lmax)
+
+
+def katz_stop_residual(A, beta, X, sigma):
+    """What the symmetric solvers' stop_rule 1 documents, recomputed in fp64 at the returned vectors:
+    max_q slope(l_q) ||A v_q - l_q v_q|| / max sigma.  Returns (value, dict of the per-pair terms)."""
+    V, l, s, norm_dev = katz_pairs(beta, X, sigma)
+    r = eig_residuals(A, V, l)
+    sig = np.asarray(sigma, dtype=np.float64)
+    terms = katz_slope(beta, l) * r / max(sig.max(), 1e-300)
+    return float(terms.max()), dict(V=V, l=l, sign=s, norm_dev=norm_dev, r=r, terms=terms)
+
+
+def mode1_stop_residual(A, X, lam):
+    """spectral_mode 1 (Laplacian Eigenmaps / LLE): v_q = X[:, q], l_q = lam_q;  max_q ||A v_q - l_q v_q|| / max_q |l_q|.
+    Returns (value, per-pair residuals)."""
+    lam = np.asarray(lam, dtype=np.float64)
+    r = eig_residuals(A, np.asarray(X, dtype=np.float64), lam)
+    return float(r.max() / max(np.abs(lam).max(), 1e-300)), r
+
+
+def general_stop_residual(A, beta, X, terms, sigma):
+    """The general solver's (algorithm 1) stop_rule 1: max_q ||S^T u_q - sigma_q v_q|| / sigma_max (the second residual of
+    svd_residuals); also returns the first, max_q ||S v_q - sigma_q u_q|| / sigma_max, which is 0 by construction there."""
+    r1, r2, _, _ = svd_residuals(A, beta, X, terms, sigma=sigma)
+    return float(r2.max()), float(r1.max())
+
+
+def value_change(s, s_prev):
+    """The change measure of the solvers between two rounds' values: max_j |s_j - s_j'| / max(|s_j|, 1e-3 max|s|)."""
+    s, s_prev = np.asarray(s, dtype=np.float64), np.asarray(s_prev, dtype=np.float64)
+    return float(np.max(np.abs(s - s_prev) / np.maximum(np.abs(s), 1e-3 * np.abs(s).max())))
+
+
 def svd_residuals(A, beta, X, terms, sigma=None):
     """Size-independent property: for each triplet  ||S v - sigma u|| / sigma_max and
     ||S^T u - sigma v|| / sigma_max, with S applied matrix-free (fp64)."""
