@@ -17,7 +17,7 @@ UNIQUE_ID_BYTES = 128
 EXPORTS = [
     'gemb_version', 'gemb_last_error', 'gemb_device_count', 'gemb_launch_count', 'gemb_ctx_create', 'gemb_ctx_destroy',
     'gemb_host_alloc', 'gemb_host_free', 'gemb_mem_trim', 'gemb_mem_cached_bytes', 'gemb_mem_live_blocks', 'gemb_comm_unique_id', 'gemb_comm_init', 'gemb_graph_upload',
-    'gemb_graph_free', 'gemb_spmm', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
+    'gemb_graph_free', 'gemb_spmm', 'gemb_spmm4', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
     'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk', 'gemb_cc_create', 'gemb_cc_info', 'gemb_cc_labels', 'gemb_cc_lcc',
@@ -98,6 +98,7 @@ def lib():
     L.gemb_graph_upload.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, ctypes.POINTER(vp)]
     L.gemb_graph_free.argtypes = [vp]
     L.gemb_spmm.argtypes = [vp, ctypes.c_int, ctypes.c_int, f32, vp, f32, vp, f32, vp, vp]
+    L.gemb_spmm4.argtypes = [vp, ctypes.c_int, ctypes.c_int, f32, vp, f32, vp, f32, vp, f32, vp, vp]
     L.gemb_gram.argtypes = [vp, i64, vp, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp]
     L.gemb_apply.argtypes = [vp, i64, vp, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp]
     L.gemb_chol_inverse.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.POINTER(ctypes.c_int)]
@@ -344,6 +345,18 @@ class DeviceGraph(_Handle):
         Y = np.empty((self.n_local, b), dtype=np.float32)
         check(lib().gemb_spmm(self._h, int(bool(transpose)), b, float(alpha), _ptr(X), float(gamma), _ptr(Xself),
                               float(delta), _ptr(X0), _ptr(Y)))
+        return Y
+
+    def spmm4(self, X, alpha, gamma, Xself, delta, X0, eps, X1, transpose=False):
+        """Y = alpha op(A) X + gamma Xself + delta X0 + eps X1 (the composite operator's epilogue; test hook)."""
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        b = X.shape[1]
+        ops = [np.ascontiguousarray(a, dtype=np.float32) for a in (Xself, X0, X1)]
+        for a in ops:
+            assert a.shape == (self.n_local, b)
+        Y = np.empty((self.n_local, b), dtype=np.float32)
+        check(lib().gemb_spmm4(self._h, int(bool(transpose)), b, float(alpha), _ptr(X), float(gamma), _ptr(ops[0]),
+                               float(delta), _ptr(ops[1]), float(eps), _ptr(ops[2]), _ptr(Y)))
         return Y
 
     def hope(self, d, beta, out=None, want_output=True, **opts):

@@ -203,6 +203,10 @@ int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, flo
 int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
                  float gamma, const float *Xself, float delta, const float *X0, float *Y,
                  const HaloPushArgs *push = nullptr);
+// the same with a fourth epilogue operand: Y = alpha * A * X + gamma * Xself + delta * X0 + eps * X1 (single GPU, no
+// push; X1 needs Xself and X0).  The composite operator's Chebyshev step (hope.cu, spectral_mode 2) takes four rows.
+int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
+                 float gamma, const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y);
 
 // ---- halo.cu (multi-GPU)
 int halo_build(gemb_graph *g);                                   // collective; idempotent

@@ -56,6 +56,8 @@ struct HopeWork {
     DeviceBuffer<int> rank_dev;
     CallEvents<2> fork_join;    // c->stream -> c->side and back (ritz_eigh)
     int64_t spmm_wide = 0, spmm_all = 0;
+    int mode = 0;               // opts.spectral_mode
+    DeviceBuffer<float> opT;    // spectral_mode 2: T = X - A X between the two sweeps of one application (n x b)
     bool halo = false;       // multi-GPU: needed-rows-only exchange over peer memory (halo.cu); buf[] = g->halo.buf[]
     int64_t pushes = 0;      // blocks whose rows were pushed to the peers
     double push_bytes_per_row = 0.0;   // sum over the pushed blocks of (bytes per pushed row): NVLink bytes out = this * push_rows
@@ -186,6 +188,24 @@ static int dist_spmm3(HopeWork &W, bool transpose, int width, float alpha, const
 static int dist_spmm(HopeWork &W, bool transpose, int width, float alpha, const float *Xshard,
                      const float *X0, float *Y, bool timed) {
     return dist_spmm3(W, transpose, width, alpha, Xshard, 0.f, false, 1.f, X0, Y, timed);
+}
+
+// One application of the symmetric solver's operator Op:  Y = alpha * Op X + gamma * X (use_self) + delta * X0.
+// spectral_modes 0 and 1: Op = A, one sweep (dist_spmm3 as it stands).  spectral_mode 2 (single GPU): the composite
+// Op = -M^T M with M = I - A, uploaded as A and A^T and never formed -- sweep 1 T = X - A X, sweep 2
+// Y = alpha A^T T - alpha T + gamma X + delta X0, whose epilogue takes four rows (spmm4_launch).  One application
+// counts as two sweeps.
+static int op_apply(HopeWork &W, int width, float alpha, const float *X, float gamma, bool use_self, float delta,
+                    const float *X0, float *Y, bool timed, bool push_out = false) {
+    if (W.mode != 2) return dist_spmm3(W, false, width, alpha, X, gamma, use_self, delta, X0, Y, timed, push_out);
+    gemb_ctx *c = W.c;
+    float *T = W.opT.get();
+    if (timed) GEMB_TRY(c->t_spmm.begin(c->stream));
+    GEMB_TRY(spmm3_launch(c, W.g->A, W.rows, width, -1.f, X, 1.f, X, 0.f, nullptr, T));
+    GEMB_TRY(spmm4_launch(c, W.g->AT, W.rows, width, alpha, T, -alpha, T, gamma, use_self ? X : nullptr, delta, X0, Y));
+    if (timed) { GEMB_TRY(c->t_spmm.end(c->stream)); W.spmm_wide += 2; }
+    W.spmm_all += 2;
+    return GEMB_OK;
 }
 
 // out = sum_{j=1..J} (beta op(A))^j in   (Horner: W_m = in + beta op(A) W_{m-1}); t1,t2 scratch
@@ -407,6 +427,30 @@ static int estimate_norm2(HopeWork &W, uint64_t seed, float *x, float *y, float 
     return GEMB_OK;
 }
 
+// spectral_mode 2: ||M||_2^2 = ||M^T M||_2 by power iteration on the composite operator with a 4-column block.  From
+// below, like estimate_norm2: hope_symmetric raises it to the largest |Ritz value| (SpecMap::observe).
+static int estimate_composite_norm(HopeWork &W, uint64_t seed, float *x, float *y, double *out) {
+    gemb_ctx *c = W.c;
+    const int pw = 4;
+    GEMB_TRY(randn_launch(c, W.rows, pw, seed ^ 0x5bd1e995u, (uint64_t)W.g->row0, x));
+    double est = 0.0, prev = -1.0;
+    for (int it = 0; it < 32; it++) {
+        double h[2];
+        GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal.get()));
+        GEMB_TRY(op_apply(W, pw, 1.f, x, 0.f, false, 1.f, nullptr, y, false));
+        GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get() + 1));
+        GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
+        if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }   // M^T M x = 0 (M = 0: P = I)
+        est = sqrt(h[1] / h[0]);                                      // ||M^T M x|| / ||x|| -> ||M||_2^2
+        GEMB_TRY(scale_launch(c, W.rows * pw, (float)(1.0 / sqrt(h[1])), y));
+        std::swap(x, y);
+        if (prev > 0 && fabs(est - prev) <= 1e-3 * est && it >= 3) break;
+        prev = est;
+    }
+    *out = est;
+    return GEMB_OK;
+}
+
 // beta * ||A||_2 >= 1 does not mean the Katz series diverges: it converges iff beta * rho(A) < 1, and a directed graph
 // (a hub, a DAG: rho = 0) can have ||A||_2 far above rho(A).  Measure the series itself on a width-4 random probe:
 // t_j = (beta op(A))^j t_0; J = first j with ||t_j|| <= katz_tol * max_i ||t_i|| (for A and A^T), plus a margin.
@@ -447,7 +491,8 @@ struct Opts {
     int oversample = 16, max_iters = 30, min_iters = 2, katz_terms = 0, compute_residual = 0, verbose = 0;
     int algorithm = 0, cheb_degree = 8, stop_rule = 0, lanczos_basis = 0;
     int spectral_mode = 0;   // 0: top-k singular triplets of the Katz operator (HOPE); 1: the d largest ALGEBRAIC eigenpairs of the
-                             // uploaded symmetric matrix itself (Laplacian Eigenmaps: D^-1/2 A D^-1/2, lap.py:26-32)
+                             // uploaded symmetric matrix itself (Laplacian Eigenmaps: D^-1/2 A D^-1/2, lap.py:26-32);
+                             // 2: those of the composite -M^T M, M = I - A (LLE: A = D^-1 W, uploaded with A^T)
     float tol = 1e-6f, katz_tol = 1e-7f, range_log2 = 8.f;
     uint64_t seed = 1234;
 };
@@ -718,13 +763,16 @@ static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t 
 // ------------------------------------------------------------------------------------ symmetric solvers
 // The spectral map of the symmetric solvers.  Katz (spectral_mode 0): S = f(A), f(l) = beta l / (1 - beta l), so the
 // wanted values are the largest |f(l)| over A's eigenvalues l; spectral_mode 1: the largest algebraic l themselves.
-// Every Ritz value is clamped to [-bound, bound] (Ritz values lie inside the spectrum) before it is mapped.
+// spectral_mode 2 (negdef): the same on the composite -M^T M, whose spectrum is [-||M||_2^2, 0].
+// Every Ritz value is clamped to [-bound, bound] ([-bound, 0] when negdef: Ritz values lie inside the spectrum) before
+// it is mapped.
 struct SpecMap {
     double beta;
     bool katz;
     double norm;    // a priori bound on |l|: ||A||_inf, or the power-iteration ||A||_2
     double bound;   // current bound on |l|
     bool estimated = false;   // norm is the power-iteration estimate, which can lie below ||A||_2 (a cluster of top values)
+    bool negdef = false;      // spectral_mode 2: the operator is negative semi-definite; the wanted end is 0
     SpecMap(double beta, bool katz, double norm) : beta(beta), katz(katz), norm(norm), bound(norm * 1.02 + 1e-30) {}
     // an estimated norm is raised to max |l| over the Ritz values l[0..n) (all inside the spectrum), so that the clamp
     // never moves a Ritz value; false when then beta * norm >= 1 (the Katz series diverges)
@@ -740,7 +788,7 @@ struct SpecMap {
         for (int i = 0; i < n; i++) amax = std::max(amax, fabs(l[i]));
         bound = std::min(norm * 1.02, growth * amax) + 1e-30;
     }
-    double clamp(double l) const { return std::max(-bound, std::min(bound, l)); }
+    double clamp(double l) const { return std::max(-bound, std::min(negdef ? 0.0 : bound, l)); }
     double f(double l) const { return beta * l / (1.0 - beta * l); }
     // rank key, largest wanted first: |f(l)| (= sigma), or l + bound
     double key(double l) const { l = clamp(l); return katz ? fabs(f(l)) : l + bound; }
@@ -750,7 +798,8 @@ struct SpecMap {
     // |d key / dl|: maps an eigen-residual of A to the residual of the key's triplet (|f'(l)| = beta / (1 - beta l)^2)
     double slope(double l) const { l = clamp(l); return katz ? beta / ((1.0 - beta * l) * (1.0 - beta * l)) : 1.0; }
     // Chebyshev filter interval [c0 - e, c0 + e] over the damped set {l : key(l) < key(l_min)}, l_min the block's Ritz
-    // value of smallest key, and the end aL (+-bound) the filter is normalised at: the dominant end, the side of l_top
+    // value of smallest key, and the end aL (+-bound; negdef: 0) the filter is normalised at: the dominant end, the
+    // side of l_top
     struct Interval { double e, c0, aL; };
     Interval damped(double l_top, double l_min) const {
         const double tau = key(l_min);
@@ -760,7 +809,7 @@ struct SpecMap {
         hi = std::min(hi, bound);
         if (hi - lo < 2e-3 * bound) { const double mid = 0.5 * (hi + lo); lo = mid - 1e-3 * bound; hi = mid + 1e-3 * bound; }
         const double e = 0.5 * (hi - lo), c0 = 0.5 * (hi + lo);
-        return {e, c0, (!katz || l_top >= c0) ? bound : -bound};
+        return {e, c0, negdef ? 0.0 : ((!katz || l_top >= c0) ? bound : -bound)};
     }
     // the output of Ritz value l: sigma (|f(l)|, or l), the scale of its vector in X (sqrt(sigma), or 1), and whether
     // the left half of X takes the vector negated (f(l) < 0)
@@ -799,11 +848,15 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     // (round 1 orthonormalised after every step: 4 x CholeskyQR2 = 3.5 ms of the 58 ms solve at S, for nothing -- the
     // block's condition number after three steps is (lambda_1 / lambda_b)^3, a few units on a community graph).  Should
     // the first Cholesky drop columns (skewed spectrum, rank-deficient A), the careful form below takes over.
+    // spectral_mode 2: the wanted end of -M^T M is 0, its smallest |l|, which a power step would damp: the warm-up
+    // steps run on the shifted -M^T M + bound I instead, whose wanted end is its largest value.
+    const bool shift = mode == 2;
+    const float nu = shift ? (float)map.bound : 0.f;
     GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, pool[0]));
     GEMB_TRY(publish(W, pool[0], b));
-    GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[0], 0.f, false, 1.f, nullptr, pool[1], true, W.halo));
-    GEMB_TRY(dist_spmm3(W, false, b, 1.f, pool[1], 0.f, false, 1.f, nullptr, pool[2], true, W.halo));
-    GEMB_TRY(dist_spmm(W, false, b, 1.f, pool[2], nullptr, AV, true));
+    GEMB_TRY(op_apply(W, b, 1.f, pool[0], nu, shift, 1.f, nullptr, pool[1], true, W.halo));
+    GEMB_TRY(op_apply(W, b, 1.f, pool[1], nu, shift, 1.f, nullptr, pool[2], true, W.halo));
+    GEMB_TRY(op_apply(W, b, 1.f, pool[2], nu, shift, 1.f, nullptr, AV, true));
     GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
     GEMB_TRY(cholqr_pass(W, W.G.get(), AV, pool[0]));
     int rank1 = b;
@@ -817,7 +870,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         GEMB_TRY(cholqr2(W, pool[0], pool[1], V));
         GEMB_TRY(publish(W, V, b));
         for (int s = 0; s < 3; s++) {   // plain power steps V <- orth(A V)
-            GEMB_TRY(dist_spmm(W, false, b, 1.f, V, nullptr, AV, true));
+            GEMB_TRY(op_apply(W, b, 1.f, V, nu, shift, 1.f, nullptr, AV, true));
             GEMB_TRY(cholqr2(W, AV, pool[0], V));
             GEMB_TRY(publish(W, V, b));
         }
@@ -839,8 +892,8 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         for (int i = 2; i <= deg; i++) {
             const double sn = 1.0 / (tau2 - sigma);
             float *nxt = free_a;
-            GEMB_TRY(dist_spmm3(W, false, b, (float)(2.0 * sn / e), cur, (float)(-2.0 * sn * c0 / e), true,
-                                (float)(-sigma * sn), prev, nxt, true, /*push_out=*/i < deg));
+            GEMB_TRY(op_apply(W, b, (float)(2.0 * sn / e), cur, (float)(-2.0 * sn * c0 / e), true, (float)(-sigma * sn),
+                              prev, nxt, true, /*push_out=*/i < deg));
             sigma = sn;
             // rotate: the old `prev` becomes free unless it is V (V must survive until the new basis exists)
             float *old_prev = prev;
@@ -856,7 +909,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     for (int it = 1; it <= o.max_iters; it++) {
         R.iters = it;
         // Rayleigh-Ritz on A: T = V^T A V, (l, Z) = eigh(T)
-        GEMB_TRY(dist_spmm(W, false, b, 1.f, V, nullptr, AV, true));
+        GEMB_TRY(op_apply(W, b, 1.f, V, 0.f, false, 1.f, nullptr, AV, true));
         GEMB_TRY(gram_full(W, V, AV, W.G2.get()));
         // (Measured: running the single-CTA Jacobi on a side stream while the filter starts with the PREVIOUS
         // round's interval costs two extra rounds -- 75 instead of 56 SpMM sweeps -- and is slower overall;
@@ -870,13 +923,19 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         std::sort(order.begin(), order.end(), [&](int a, int c2) { return gval[a] > gval[c2]; });   // descending key
         for (int i = 0; i < b; i++) th_sorted[i] = gval[order[i]] * gval[order[i]];
         const double tmax = std::max(th_sorted[0], 1e-300);
-        // vmax: max |value| over the wanted pairs (Katz: sigma_max = gval[order[0]])
+        // vmax: max |value| over the wanted pairs (Katz: sigma_max = gval[order[0]]).  spectral_mode 2: the operator
+        // bound ||M||_2^2 -- the wanted eigenvalues -sigma^2 lie near 0, and both stop measures are taken relative to
+        // the operator, as the explicit form's are relative to its shift c >= ||M||_2^2
         double vmax = 0.0;
-        for (int j = 0; j < k; j++) vmax = std::max(vmax, fabs(map.value(lam[order[j]])));
+        if (mode == 2) vmax = map.norm;
+        else for (int j = 0; j < k; j++) vmax = std::max(vmax, fabs(map.value(lam[order[j]])));
         double change;
         if (mode) {
             for (int i = 0; i < b; i++) vals[i] = map.value(lam[order[i]]);
-            change = value_change(vals.data(), vals_prev.data(), k, vmax);
+            if (mode == 2) {        // round 1 has nothing to compare with (vals_prev = 0 would read as a tiny change)
+                change = it == 1 ? HUGE_VAL : 0.0;
+                for (int j = 0; j < k && it > 1; j++) change = std::max(change, fabs(vals[j] - vals_prev[j]) / std::max(vmax, 1e-300));
+            } else change = value_change(vals.data(), vals_prev.data(), k, vmax);
             vals_prev = vals;
         } else change = sigma_change(th_sorted.data(), th_prev.data(), k, tmax);
         R.change = change;
@@ -923,7 +982,10 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         if (growth > 1.0 + 1e-9) deg = std::min(deg, (int)floor(log(2.0 * exp2((double)o.range_log2)) / log(growth)));
 
         if (deg < 2) {                                          // A V is already there: one power step
-            GEMB_TRY(orth_rotated(W, AV, pool[0], V));
+            if (shift) {                                        // on -M^T M + bound I, as in the warm-up
+                GEMB_TRY(axpby_launch(W, 1.f, AV, nu, V, pool[1]));
+                GEMB_TRY(orth_rotated(W, pool[1], pool[0], V));
+            } else GEMB_TRY(orth_rotated(W, AV, pool[0], V));
             GEMB_TRY(refill_dropped(W, V, pool[0], pool[1], o.seed + 7919ull * (uint64_t)it));
             GEMB_TRY(publish(W, V, b));
             continue;
@@ -1343,10 +1405,13 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
                          float *sigma_out, gemb_hope_stats *stats) {
     GEMB_ARG(g != nullptr, "graph");
     GEMB_ARG(d >= 1, "d must be >= 1");
-    GEMB_ARG((uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode == 1) || d % 2 == 0, "d must be even (k = d/2 singular triplets)");
+    GEMB_ARG((uo && uo->struct_size == sizeof(gemb_hope_opts) && (uo->spectral_mode == 1 || uo->spectral_mode == 2)) || d % 2 == 0,
+             "d must be even (k = d/2 singular triplets)");
     GEMB_ARG(!stats || stats->struct_size == sizeof(gemb_hope_stats), "stats.struct_size");
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
+    GEMB_ARG(!(uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode == 2) || c->nranks == 1,
+             "spectral_mode 2 (the composite operator -M^T M) is single-GPU: use a context without a multi-GPU communicator");
     GEMB_ARG(!(c->nranks > 1 && g->replicated), "multi-GPU HOPE needs row shards (upload rows [rank*ceil(n/P), ...))");
     Opts o;
     if (uo) {
@@ -1367,7 +1432,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         GEMB_ARG(uo->stop_rule == 0 || uo->stop_rule == 1, "opts.stop_rule");
         o.stop_rule = uo->stop_rule;
         if (uo->algorithm3_basis > 0) o.lanczos_basis = uo->algorithm3_basis;
-        GEMB_ARG(uo->spectral_mode == 0 || uo->spectral_mode == 1, "opts.spectral_mode");
+        GEMB_ARG(uo->spectral_mode >= 0 && uo->spectral_mode <= 2, "opts.spectral_mode");
         o.spectral_mode = uo->spectral_mode;
     }
     if (o.spectral_mode == 1) {
@@ -1376,7 +1441,19 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         o.algorithm = 2;
         beta = 0.f;                 // unused: the ranking is by the eigenvalue itself
     }
-    if (o.algorithm >= 2 && !g->symmetric) {
+    if (o.spectral_mode == 2) {
+        // The wanted end of -M^T M (sigma^2 ~ 1e-2) is a sliver of a spectrum ||M||_2^2 wide (1246 on R-MAT 20's largest
+        // component): per degree the filter gains ~1 + (m a)^2 / 2 at low degree m, exponentially only at high degree.
+        // Degree 8 there stopped on the change rule with sigma^2 20x too large; degree 64 reaches an fp64 residual of
+        // 2e-5 (DESIGN 5f).  The dynamic-range cap below still bounds it.
+        if (!(uo->cheb_degree >= 2)) o.cheb_degree = 64;
+        GEMB_ARG(!g->symmetric, "spectral_mode 2 needs A = D^-1 W uploaded together with its transpose (indptr_t, "
+                                "indices_t, data_t): M^T M is applied as a sweep of A and a sweep of A^T");
+        GEMB_ARG(o.algorithm == 0 || o.algorithm == 2, "spectral_mode 2 runs on the Chebyshev-filtered subspace iteration (algorithm 0 or 2)");
+        o.algorithm = 2;
+        beta = 0.f;
+    }
+    if (o.algorithm >= 2 && !g->symmetric && o.spectral_mode != 2) {
         set_error("algorithm=%d (works on A itself, S = f(A)) needs a symmetric shard (upload with indptr_t = NULL)", o.algorithm);
         return GEMB_ERR_ARG;
     }
@@ -1392,6 +1469,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     const double t_enter = now();
     HopeWork W;
     W.g = g; W.c = c; W.b = b; W.rows = g->n_local; W.shard = g->n_shard;
+    W.mode = o.spectral_mode;
     // multi-GPU, symmetric shard: needed-rows-only exchange over peer memory (halo.cu) unless GEMB_MG=allgather or
     // CUDA IPC is not available on this box (then every rank falls back to the all-gather form together)
     static const bool mg_allgather = getenv("GEMB_MG") && !strcmp(getenv("GEMB_MG"), "allgather");
@@ -1428,6 +1506,10 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     GEMB_CUDA(W.M2.alloc(b * b));
     GEMB_CUDA(W.rank_dev.alloc(1));
     GEMB_CUDA(W.fork_join.create());
+    if (W.mode == 2) {                                     // the sixth n x b block: T between the two sweeps
+        GEMB_CUDA(W.opT.alloc((size_t)W.shard * b));
+        GEMB_CUDA(cudaMemsetAsync(W.opT.get(), 0, sizeof(float) * (size_t)W.shard * b, c->stream));
+    }
 
     c->t_spmm.reset(); c->t_dense.reset(); c->t_comm.reset(); c->t_misc.reset();
     const double t_alloc = now();
@@ -1448,7 +1530,12 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         GEMB_TRY(clear_scratch(W));
     }
     bool need_power = (J <= 0 && algo == 1) && !have_nrm;
-    if (algo >= 2) {
+    if (W.mode == 2) {
+        // the Perron-Frobenius shortcut (ritz_bound) does not apply to -M^T M: ||M||_2^2 by power iteration
+        GEMB_TRY(estimate_composite_norm(W, o.seed, W.buf[3], W.buf[4], &nrm));
+        if (!(nrm > 0.0)) nrm = 1.0;                       // M = 0: the spectrum is {0}, any positive bound holds it
+        GEMB_TRY(clear_scratch(W));
+    } else if (algo >= 2) {
         bool nonneg = false;
         GEMB_TRY(rowsum_bound(W, &hard_bound, &nonneg));
         if (nonneg && (double)beta * hard_bound * 1.02 < 1.0) ritz_bound = true;   // spectrum bounds from Ritz values
@@ -1475,6 +1562,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     const SpecMap lanczos_map(beta, true, hard_bound);
     SpecMap sym_map(beta, o.spectral_mode == 0, ritz_bound ? hard_bound : nrm);
     sym_map.estimated = !ritz_bound;                              // else ||A||_inf: a true bound
+    sym_map.negdef = o.spectral_mode == 2;
     if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, lanczos_map, R);
     else if (algo >= 2) {
         s = hope_symmetric(W, o, d, sym_map, ritz_bound, R);

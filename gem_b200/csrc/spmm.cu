@@ -17,7 +17,8 @@
 namespace gemb {
 
 int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, const float *X, float gamma,
-                      const float *Xself, float delta, const float *X0, float *Y, const HaloPushArgs *push);
+                      const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y,
+                      const HaloPushArgs *push);
 
 __device__ __forceinline__ void fma4(float4 &a, float v, const float4 &x) {
     a.x = fmaf(v, x.x, a.x);
@@ -79,12 +80,12 @@ spmm_heavy_partial_kernel(const int32_t *__restrict__ indptr, const int32_t *__r
     }
 }
 
-template <bool HAS_X0, bool HAS_SELF>
+template <bool HAS_X0, bool HAS_SELF, bool HAS_X1>
 __global__ void __launch_bounds__(256)
 spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, const int32_t *__restrict__ heavy_first,
                          int G, float alpha, float gamma, float delta, const float4 *__restrict__ partial,
                          const float4 *__restrict__ Xself, const float4 *__restrict__ X0, float4 *__restrict__ Y,
-                         bool has_push, HaloPushArgs P) {
+                         bool has_push, HaloPushArgs P, float eps, const float4 *__restrict__ X1) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int h = idx / G, c = idx - h * G;
     if (h >= n_heavy) return;
@@ -104,13 +105,19 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
         const float4 z = __ldg(X0 + row * G + c);
         r.x = fmaf(delta, z.x, r.x); r.y = fmaf(delta, z.y, r.y); r.z = fmaf(delta, z.z, r.z); r.w = fmaf(delta, z.w, r.w);
     }
+    if (HAS_X1) {
+        const float4 z = __ldg(X1 + row * G + c);
+        r.x = fmaf(eps, z.x, r.x); r.y = fmaf(eps, z.y, r.y); r.z = fmaf(eps, z.z, r.z); r.w = fmaf(eps, z.w, r.w);
+    }
     Y[row * G + c] = r;
     if (has_push) halo_push_row(P, row, G, c, r);
 }
 
-// Y[row] = alpha * (A X)[row] + gamma * Xself[row] + delta * X0[row]
+// Y[row] = alpha * (A X)[row] + gamma * Xself[row] + delta * X0[row] (+ eps * X1[row])
 //   Horner / Katz sweep:      gamma = 0, delta = 1, X0 = the sweep's input block
 //   Chebyshev three-term step: gamma = -2 s c0 / e (current block), delta = -s s' (previous block)
+//   the same step on the composite operator -M^T M, M = I - A (hope.cu, spectral_mode 2): the second sweep gathers
+//   T = X - A X through A^T and needs T, the current and the previous block: Xself = T, X0 = current, X1 = previous
 // One CTA per row TILE (SPMM_TILE_PASSES * rows_per_cta consecutive rows); the tile's slice of the column-id (and value)
 // arrays -- one contiguous range of the CSR -- is staged into shared memory by ONE TMA bulk copy (cp.async.bulk +
 // mbarrier complete_tx) issued by thread 0 while every row group fetches its row offsets; the other resident CTAs of the
@@ -123,13 +130,13 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
 // reference it -- 16-byte posted stores over NVLink, issued while the other row groups of the SM are still gathering.
 constexpr int BULK_CAP = 3072;                 // staged ids per tile (+ up to 3 of alignment slack + 4 of over-read)
 constexpr int SPMM_TILE_PASSES = 4;            // rows per tile = passes * (256 / G)
-template <bool HAS_VAL, bool HAS_PUSH, bool HAS_X0, bool HAS_SELF>
+template <bool HAS_VAL, bool HAS_PUSH, bool HAS_X0, bool HAS_SELF, bool HAS_X1>
 __global__ void __launch_bounds__(256)
 spmm_bulk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                  const float *__restrict__ vals, int64_t n_rows, int64_t nnz, int G, int rows_per_cta, int tile_rows,
                  float alpha, float gamma, float delta, const float4 *__restrict__ X,
                  const float4 *__restrict__ Xself, const float4 *__restrict__ X0, float4 *__restrict__ Y,
-                 int heavy_deg, HaloPushArgs P) {
+                 int heavy_deg, HaloPushArgs P, float eps, const float4 *__restrict__ X1) {
     __shared__ __align__(16) int32_t s_idx[BULK_CAP + 8];
     __shared__ __align__(16) float s_val[HAS_VAL ? BULK_CAP + 8 : 4];
     __shared__ __align__(8) uint64_t s_bar;
@@ -200,6 +207,10 @@ spmm_bulk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__
                 const float4 z = __ldg(X0 + row * G + c);
                 r.x = fmaf(delta, z.x, r.x); r.y = fmaf(delta, z.y, r.y); r.z = fmaf(delta, z.z, r.z); r.w = fmaf(delta, z.w, r.w);
             }
+            if (HAS_X1) {
+                const float4 z = __ldg(X1 + row * G + c);
+                r.x = fmaf(eps, z.x, r.x); r.y = fmaf(eps, z.y, r.y); r.z = fmaf(eps, z.z, r.z); r.w = fmaf(eps, z.w, r.w);
+            }
             Y[row * G + c] = r;
             if (HAS_PUSH) halo_push_row(P, row, G, c, r);
         }
@@ -230,9 +241,10 @@ int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, fl
     const float4 *X4 = (const float4 *)X, *X04 = (const float4 *)X0, *XS4 = (const float4 *)Xself;
     float4 *Y4 = (float4 *)Y;
 #define LAUNCH(V, PU, Z, S)                                                                                              \
-    spmm_bulk_kernel<V, PU, Z, S><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, n_rows, A.nnz, G, \
-                                                                              rows_per_cta, tile_rows, alpha, gamma, delta, \
-                                                                              X4, XS4, X04, Y4, hd, PA)
+    spmm_bulk_kernel<V, PU, Z, S, false><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, n_rows, \
+                                                                              A.nnz, G, rows_per_cta, tile_rows, alpha, \
+                                                                              gamma, delta, X4, XS4, X04, Y4, hd, PA, 0.f, \
+                                                                              nullptr)
 #define LAUNCHB(V, PU)                                                                                                   \
     do {                                                                                                                 \
         if (X0 && Xself) LAUNCH(V, PU, true, true); else if (X0) LAUNCH(V, PU, true, false);                             \
@@ -245,14 +257,44 @@ int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, fl
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     if (!heavy) return GEMB_OK;
-    return spmm_heavy_launch(ctx, A, b, alpha, X, gamma, Xself, delta, X0, Y, push);
+    return spmm_heavy_launch(ctx, A, b, alpha, X, gamma, Xself, delta, X0, 0.f, nullptr, Y, push);
+}
+
+int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
+                 float gamma, const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y) {
+    if (!X1) return spmm3_launch(ctx, A, n_rows, b, alpha, X, gamma, Xself, delta, X0, Y);
+    GEMB_ARG(Xself && X0, "the fourth epilogue operand needs Xself and X0");
+    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "block width must be a multiple of 4, <= 1024");
+    if (n_rows == 0) return GEMB_OK;
+    const int G = b / 4;
+    const int rows_per_cta = 256 / G;
+    const int tile_rows = rows_per_cta * SPMM_TILE_PASSES;
+    const int64_t n_tiles = (n_rows + tile_rows - 1) / tile_rows;
+    GEMB_ARG(n_tiles < (int64_t)2147483647, "grid too large");
+    const bool heavy = A.n_items > 0;
+    const int hd = heavy ? SPMM_HEAVY_DEG : 0;
+    HaloPushArgs PA;
+    memset(&PA, 0, sizeof PA);
+#define LAUNCH(V)                                                                                                        \
+    spmm_bulk_kernel<V, false, true, true, true><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(                            \
+        A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta, tile_rows, alpha, gamma, delta, (const float4 *)X, \
+        (const float4 *)Xself, (const float4 *)X0, (float4 *)Y, hd, PA, eps, (const float4 *)X1)
+    if (A.data) LAUNCH(true);
+    else LAUNCH(false);
+#undef LAUNCH
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    if (!heavy) return GEMB_OK;
+    return spmm_heavy_launch(ctx, A, b, alpha, X, gamma, Xself, delta, X0, eps, X1, Y, nullptr);
 }
 
 int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, const float *X, float gamma,
-                      const float *Xself, float delta, const float *X0, float *Y, const HaloPushArgs *push) {
+                      const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y,
+                      const HaloPushArgs *push) {
     const int G = b / 4;
     const int rows_per_cta = 256 / G;
     const float4 *X4 = (const float4 *)X, *X04 = (const float4 *)X0, *XS4 = (const float4 *)Xself;
+    const float4 *X14 = (const float4 *)X1;
     float4 *Y4 = (float4 *)Y;
     HaloPushArgs PA;
     memset(&PA, 0, sizeof PA);
@@ -273,12 +315,13 @@ int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, 
 #undef HP
         GEMB_CUDA(cudaGetLastError());
         const int fgrid = (int)(((int64_t)A.n_heavy * G + 255) / 256);
-#define FIN(Z, S) spmm_heavy_finish_kernel<Z, S><<<fgrid, 256, 0, ctx->stream>>>(A.n_heavy, A.heavy_row, A.heavy_first, G, alpha, gamma, \
-                                                                               delta, P4, XS4, X04, Y4, push != nullptr, PA)
-        if (X0 && Xself) FIN(true, true);
-        else if (X0) FIN(true, false);
-        else if (Xself) FIN(false, true);
-        else FIN(false, false);
+#define FIN(Z, S, X1P) spmm_heavy_finish_kernel<Z, S, X1P><<<fgrid, 256, 0, ctx->stream>>>(A.n_heavy, A.heavy_row, A.heavy_first, G, \
+                                                                    alpha, gamma, delta, P4, XS4, X04, Y4, push != nullptr, PA, eps, X14)
+        if (X1) FIN(true, true, true);                 // spmm4_launch: X1 comes with Xself and X0
+        else if (X0 && Xself) FIN(true, true, false);
+        else if (X0) FIN(true, false, false);
+        else if (Xself) FIN(false, true, false);
+        else FIN(false, false, false);
 #undef FIN
         GEMB_CUDA(cudaGetLastError());
         count_launch(2);
@@ -292,21 +335,30 @@ using namespace gemb;
 
 extern "C" int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma,
                          const float *Xself, float delta, const float *X0, float *Y) {
+    return gemb_spmm4(g, transpose, b, alpha, X, gamma, Xself, delta, X0, 0.f, nullptr, Y);
+}
+
+extern "C" int gemb_spmm4(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma,
+                          const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y) {
     GEMB_ARG(g && X && Y, "graph/X/Y");
     GEMB_ARG(b > 0 && b % 4 == 0, "b must be a positive multiple of 4");
+    GEMB_ARG(!X1 || (Xself && X0), "X1 needs Xself and X0");
+    GEMB_ARG(!X1 || g->n_local == g->n, "the fourth epilogue operand is single-GPU");
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
-    DeviceBuffer<float> dX, dY, dXs, dX0;
+    DeviceBuffer<float> dX, dY, dXs, dX0, dX1;
     const size_t full = (size_t)g->n * b, shard = (size_t)g->n_local * b;
     GEMB_CUDA(dX.alloc(full));
     GEMB_CUDA(dY.alloc(shard));
     if (Xself) GEMB_CUDA(dXs.alloc(shard));
     if (X0) GEMB_CUDA(dX0.alloc(shard));
+    if (X1) GEMB_CUDA(dX1.alloc(shard));
     GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * full, cudaMemcpyHostToDevice, c->stream));
     if (Xself) GEMB_CUDA(cudaMemcpyAsync(dXs.get(), Xself, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
     if (X0) GEMB_CUDA(cudaMemcpyAsync(dX0.get(), X0, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
-    GEMB_TRY(spmm3_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX.get(), gamma, dXs.get(), delta, dX0.get(),
-                          dY.get()));
+    if (X1) GEMB_CUDA(cudaMemcpyAsync(dX1.get(), X1, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
+    GEMB_TRY(spmm4_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX.get(), gamma, dXs.get(), delta, dX0.get(),
+                          eps, dX1.get(), dY.get()));
     GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * shard, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     return GEMB_OK;

@@ -67,16 +67,18 @@ def undirected_normalised(csr):
     return out, l_fro2
 
 
-def spectral_solve(model, op, d, name):
+def spectral_solve(model, op, d, name, op_t=None):
     """(V, lam): the d + 1 largest algebraic eigenpairs of the symmetric HostCSR `op` by the Chebyshev-filtered subspace
     iteration of gemb_hope (spectral_mode = 1), with the model's solver options; sets model.stats and warns (raises
-    under strict) when the solver stopped unconverged."""
+    under strict) when the solver stopped unconverged.  With op_t (the HostCSR of op's transpose) the eigenpairs are
+    those of the composite -(I - op)^T (I - op) instead, never formed (spectral_mode = 2)."""
     opts = {k: getattr(model, '_' + k) for k in _OPT_KEYS if hasattr(model, '_' + k)}
     opts.setdefault('tol', 1e-6)
     opts.setdefault('max_iters', 300)
+    tr = {} if op_t is None else {'indptr_t': op_t.indptr, 'indices_t': op_t.indices, 'data_t': op_t.data_f32()}
     with _native.Context(int(getattr(model, '_device', 0))) as ctx, \
-            _native.DeviceGraph(ctx, op.n, op.indptr, op.indices, op.data_f32()) as g:
-        V, lam, st = g.hope(d + 1, 0.0, spectral_mode=1, **opts)
+            _native.DeviceGraph(ctx, op.n, op.indptr, op.indices, op.data_f32(), **tr) as g:
+        V, lam, st = g.hope(d + 1, 0.0, spectral_mode=1 if op_t is None else 2, **opts)
     model.stats = st
     measure = ('residual estimate %.3g' % st.get('resid_est', -1.0) if opts.get('stop_rule', 0) == 1 else
                'eigenvalues still moving by %.3g relative per round' % st['ritz_change'])

@@ -112,6 +112,10 @@ int gemb_graph_free(gemb_graph *g);
  * all HOST, row-major fp32.  b must be a multiple of 4, <= 1024. */
 int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma, const float *Xself,
               float delta, const float *X0, float *Y);
+/* The same with the fourth epilogue operand of spectral_mode 2's Chebyshev step (single GPU):
+ * Y = alpha * op(A) * X + gamma * Xself + delta * X0 + eps * X1; X1 == NULL is gemb_spmm, else Xself and X0 are needed. */
+int gemb_spmm4(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma, const float *Xself,
+               float delta, const float *X0, float eps, const float *X1, float *Y);
 
 /* Test hook for the tensor-core contraction: G (b1 x b2, fp64, row-major) = P^T Q over n rows; P, Q host
  * fp32 row-major (Q == NULL means Q = P).  use_tensor_cores: 1 = wgmma kernel (GEMB_ERR_UNSUPPORTED if the
@@ -156,7 +160,7 @@ typedef struct {
                               spectrum; else 1); 1 = subspace iteration on S^T S through Katz sweeps (any A);
                               2 = Chebyshev-filtered subspace iteration on A itself, S = f(A) (symmetric A only);
                               3 = thick-restart block Lanczos on A (symmetric A only; power-law spectra) */
-    int32_t cheb_degree;   /* filter degree per outer iteration of algorithm 2, default 8 */
+    int32_t cheb_degree;   /* filter degree per outer iteration of algorithm 2, default 8 (spectral_mode 2: 64) */
     float cheb_range_log2; /* algorithm 2: the filter degree is lowered until the filtered block's column dynamic range
                               T_m(x_L) stays below 2^cheb_range_log2 (fp32 Gram-based orthonormalisation squares it);
                               0 = default (8) */
@@ -178,7 +182,19 @@ typedef struct {
                               1 = the d largest ALGEBRAIC eigenpairs of the uploaded symmetric matrix itself, on the same
                               Chebyshev-filtered subspace iteration (beta ignored): X_out = n x d eigenvectors in DESCENDING
                               eigenvalue order, sigma_out = the d eigenvalues.  Laplacian Eigenmaps (lap.py:26-32:
-                              eigs(normalized_laplacian, k = d+1, which='SM')) = this on D^-1/2 A D^-1/2 with d+1 pairs */
+                              eigs(normalized_laplacian, k = d+1, which='SM')) = this on D^-1/2 A D^-1/2 with d+1 pairs.
+                              2 = the d largest algebraic eigenpairs of the composite -M^T M, M = I - A, UNSHIFTED and never
+                              formed: the upload is A = P = D^-1 W (not symmetric) together with its transpose
+                              (indptr_t / indices_t / data_t; W symmetric: P^T has W's pattern with values w_ij / s_j), and
+                              one application of -M^T M is two SpMM sweeps, T = X - A X and A^T T - T.  X_out = n x d
+                              eigenvectors, sigma_out = the d eigenvalues l_j = -sigma_j^2 DESCENDING (sigma_j ascending: the
+                              smallest singular values of M and their right singular vectors; LLE, lle.py:25-32, is this with
+                              d+1 pairs).  Single GPU; algorithm 0 or 2 (beta ignored).  The spectrum bound is ||M||_2^2 by
+                              power iteration on -M^T M (stats->norm2_A), raised to the largest |Ritz value|.  Both stop
+                              measures are taken relative to that bound, not to each small eigenvalue:
+                              stop_rule 0: max_j |l_j - l_j'| / ||M||_2^2 (round 1: not converged);  stop_rule 1: max_j ||M^T M v_j - sigma_j^2 v_j||
+                              / ||M||_2^2.  Device memory: one n x b block more than modes 0 and 1 (T).  spmm_count counts
+                              two sweeps per application. */
 } gemb_hope_opts;
 
 typedef struct {
@@ -196,7 +212,7 @@ typedef struct {
     double comm_ms;        /* NCCL time (multi-GPU) */
     double total_ms;       /* device time of the whole call (events), excluding H2D/D2H */
     double h2d_ms, d2h_ms;
-    float norm2_A;         /* estimated ||A||_2 */
+    float norm2_A;         /* estimated ||A||_2 (spectral_mode 2: ||M||_2^2) */
     float ritz_change;     /* algorithms 1 and 2: the last round's change measure (stop_rule 0 above), whichever rule
                               stopped; algorithm 3: the last restart's residual estimate (= resid_est) */
     float resid_max;       /* max_j ||S^T u_j - sigma_j v_j|| / sigma_max (compute_residual=1; spectral_mode 0) */
