@@ -373,7 +373,7 @@ class DeviceGraph(_Handle):
         if want_output:
             X = out if out is not None else np.empty((self.n_local, d), dtype=np.float32)
             assert X.dtype == np.float32 and X.shape == (self.n_local, d) and X.flags.c_contiguous
-            sig = np.empty(d if o.spectral_mode else d // 2, dtype=np.float32)
+            sig = np.empty(d if o.spectral_mode in (1, 2) else d // 2, dtype=np.float32)
         check(lib().gemb_hope(self._h, int(d), float(beta), ctypes.byref(o), _ptr(X), _ptr(sig), ctypes.byref(st)))
         return X, sig, st.as_dict()
 

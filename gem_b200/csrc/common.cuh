@@ -207,6 +207,10 @@ int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, fl
 // push; X1 needs Xself and X0).  The composite operator's Chebyshev step (hope.cu, spectral_mode 2) takes four rows.
 int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
                  float gamma, const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y);
+// Y = alpha * diag(rscale) * A * X: every row's sum scaled by its entry of rscale (n_rows floats, device; single GPU, no
+// other epilogue operand).  Sweep 1 of the Adamic-Adar operator A D A (hope.cu, spectral_mode 4).
+int spmm_scaled_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
+                       const float *rscale, float *Y);
 
 // ---- halo.cu (multi-GPU)
 int halo_build(gemb_graph *g);                                   // collective; idempotent

@@ -58,6 +58,7 @@ struct HopeWork {
     int64_t spmm_wide = 0, spmm_all = 0;
     int mode = 0;               // opts.spectral_mode
     DeviceBuffer<float> opT;    // spectral_mode 2: T = X - A X between the two sweeps of one application (n x b)
+    DeviceBuffer<float> rscale; // spectral_mode 4: D_ii = 1 / (rowsum(A) + rowsum(A^T)), 0 for isolated rows (n floats)
     bool halo = false;       // multi-GPU: needed-rows-only exchange over peer memory (halo.cu); buf[] = g->halo.buf[]
     int64_t pushes = 0;      // blocks whose rows were pushed to the peers
     double push_bytes_per_row = 0.0;   // sum over the pushed blocks of (bytes per pushed row): NVLink bytes out = this * push_rows
@@ -208,7 +209,10 @@ static int op_apply(HopeWork &W, int width, float alpha, const float *X, float g
     return GEMB_OK;
 }
 
-// out = sum_{j=1..J} (beta op(A))^j in   (Horner: W_m = in + beta op(A) W_{m-1}); t1,t2 scratch
+// out = sum_{j=1..J} (beta op(A))^j in   (Horner: W_m = in + beta op(A) W_{m-1}); t1,t2 scratch.
+// spectral_mode 5 (rooted PageRank, beta = alpha, A = P): out = (1 - alpha) sum_{j=0..J} (alpha op(P))^j in -- the same
+// loop, with the j = 0 term and the factor (1 - alpha) folded into the last sweep's epilogue:
+// out = alpha (1 - alpha) op(P) W_{J-1} + (1 - alpha) in.
 static int katz(HopeWork &W, bool transpose, float beta, int J, const float *in, float *out,
                 float *t1, float *t2) {
     const float *cur = in;
@@ -217,10 +221,31 @@ static int katz(HopeWork &W, bool transpose, float beta, int J, const float *in,
             float *dst = (m & 1) ? t1 : t2;   // halo mode: `in` was published by the caller, dst feeds the next sweep
             GEMB_TRY(dist_spmm3(W, transpose, W.b, beta, cur, 0.f, false, 1.f, in, dst, true, W.halo));
             cur = dst;
+        } else if (W.mode == 5) {
+            const double a = beta;
+            GEMB_TRY(dist_spmm3(W, transpose, W.b, (float)(a * (1.0 - a)), cur, 0.f, false, (float)(1.0 - a), in, out, true));
         } else {
             GEMB_TRY(dist_spmm(W, transpose, W.b, beta, cur, nullptr, out, true));
         }
     }
+    return GEMB_OK;
+}
+
+// out = S in, or S^T in (transpose), for the proximity of the general solver (W.mode): Katz (0) and rooted PageRank (5)
+// by katz(); common neighbours (3) S = A A and Adamic-Adar (4) S = A D A by two sweeps, t1 = D op(A) in (D = I for mode
+// 3; the scale is applied in sweep 1's epilogue), then out = op(A) t1 -- S^T = A^T D A^T takes A^T in both.  Single GPU
+// for modes 3 and 4; one application counts as two sweeps.
+static int apply_S(HopeWork &W, bool transpose, float beta, int J, const float *in, float *out, float *t1, float *t2) {
+    if (W.mode != 3 && W.mode != 4) return katz(W, transpose, beta, J, in, out, t1, t2);
+    gemb_ctx *c = W.c;
+    const gemb_csr_dev &Op = transpose ? W.g->AT : W.g->A;
+    GEMB_TRY(c->t_spmm.begin(c->stream));
+    if (W.mode == 4) GEMB_TRY(spmm_scaled_launch(c, Op, W.rows, W.b, 1.f, in, W.rscale.get(), t1));
+    else GEMB_TRY(spmm_launch(c, Op, W.rows, W.b, 1.f, in, nullptr, t1));
+    GEMB_TRY(spmm_launch(c, Op, W.rows, W.b, 1.f, t1, nullptr, out));
+    GEMB_TRY(c->t_spmm.end(c->stream));
+    W.spmm_wide += 2;
+    W.spmm_all += 2;
     return GEMB_OK;
 }
 
@@ -374,6 +399,30 @@ __global__ void csr_rowsum_kernel(int64_t n, const int32_t *__restrict__ indptr,
     }
 }
 
+// s_i = 1 / (sum_j A_ij + sum_j AT_ij) accumulated in fp64, stored fp32; 0 where the sum is 0 (an isolated row).  AT is
+// the transpose's CSR, or A itself for a symmetric upload (then s_i = 1 / (2 rowsum_i(A))).
+__global__ void inv_degree_kernel(int64_t n, const int32_t *__restrict__ ip, const float *__restrict__ v,
+                                  const int32_t *__restrict__ ipt, const float *__restrict__ vt, float *__restrict__ s) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+        double acc = 0.0;
+        if (v) { for (int i = ip[r]; i < ip[r + 1]; i++) acc += (double)v[i]; } else acc += (double)(ip[r + 1] - ip[r]);
+        if (vt) { for (int i = ipt[r]; i < ipt[r + 1]; i++) acc += (double)vt[i]; } else acc += (double)(ipt[r + 1] - ipt[r]);
+        s[r] = acc > 0.0 ? (float)(1.0 / acc) : 0.f;
+    }
+}
+
+static int inv_degree(HopeWork &W) {
+    gemb_ctx *c = W.c;
+    GEMB_CUDA(W.rscale.alloc((size_t)std::max<int64_t>(W.rows, 1)));
+    if (W.rows == 0) return GEMB_OK;
+    const int grid = (int)std::min<int64_t>((W.rows + 255) / 256, (int64_t)c->sm_count * 8);
+    inv_degree_kernel<<<grid, 256, 0, c->stream>>>(W.rows, W.g->A.indptr, W.g->A.data, W.g->AT.indptr, W.g->AT.data,
+                                                   W.rscale.get());
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    return GEMB_OK;
+}
+
 static int comm_allreduce_max_f64(HopeWork &W, double *buf, size_t count) {
     if (W.c->nranks == 1) return GEMB_OK;
     NcclApi *api = nccl_api();
@@ -492,7 +541,8 @@ struct Opts {
     int algorithm = 0, cheb_degree = 8, stop_rule = 0, lanczos_basis = 0;
     int spectral_mode = 0;   // 0: top-k singular triplets of the Katz operator (HOPE); 1: the d largest ALGEBRAIC eigenpairs of the
                              // uploaded symmetric matrix itself (Laplacian Eigenmaps: D^-1/2 A D^-1/2, lap.py:26-32);
-                             // 2: those of the composite -M^T M, M = I - A (LLE: A = D^-1 W, uploaded with A^T)
+                             // 2: those of the composite -M^T M, M = I - A (LLE: A = D^-1 W, uploaded with A^T);
+                             // 3, 4, 5: HOPE on the common-neighbour, Adamic-Adar and rooted-PageRank proximities (apply_S)
     float tol = 1e-6f, katz_tol = 1e-7f, range_log2 = 8.f;
     uint64_t seed = 1234;
 };
@@ -535,7 +585,7 @@ static int residual_check(HopeWork &W, float beta, int J, const float *P, const 
                           float *scr2, const std::vector<int> &cols, double smax, float *out) {
     gemb_ctx *c = W.c;
     const int b = W.b;
-    GEMB_TRY(katz(W, true, beta, J, P, scr0, scr1, scr2));       // scr0 = S^T P
+    GEMB_TRY(apply_S(W, true, beta, J, P, scr0, scr1, scr2));    // scr0 = S^T P
     GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, sizeof(double) * b, c->stream));
     const int threads = (256 / b) * b > 0 ? (256 / b) * b : b;
     coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(W.rows, b, scr0, Qs, W.scal.get());
@@ -623,7 +673,7 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
     std::vector<double> theta(b), theta_prev(b, 0.0), wdiag(b);
     for (int it = 1; it <= o.max_iters; it++) {
         R.iters = it;
-        GEMB_TRY(katz(W, false, beta, J, V, U, T1, T2));              // U = S V
+        GEMB_TRY(apply_S(W, false, beta, J, V, U, T1, T2));           // U = S V
         GEMB_TRY(gram_full(W, U, U, W.G.get()));                            // T = U^T U
         GEMB_CUDA(cudaMemcpyAsync(W.G2.get(), W.G.get(), sizeof(double) * b * b, cudaMemcpyDeviceToDevice, c->stream));
         GEMB_TRY(ritz_eigh(W, o.tol, false, theta));
@@ -646,7 +696,7 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         count_launch();
         GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), b, b, T1, b));
         GEMB_TRY(c->t_dense.end(c->stream));
-        GEMB_TRY(katz(W, true, beta, J, T1, Wk, Hscr, T2));           // Wk = S^T T1   (stop_rule 0: U is scratch now)
+        GEMB_TRY(apply_S(W, true, beta, J, T1, Wk, Hscr, T2));        // Wk = S^T T1   (stop_rule 0: U is scratch now)
         if (o.stop_rule == 0) { GEMB_TRY(cholqr2(W, Wk, T1, V)); continue; }   // V = orth(S^T orth(S V))
         // residual of the Ritz triplets (sigma_j, u_j = T1_j, v_j = V Z_j): S^T u_j = S^T S V Z_j theta_j^-1/2, so
         // v_j^T S^T u_j = theta_j^1/2 = sigma_j and ||S^T u_j - sigma_j v_j||^2 = (Wk^T Wk)_jj - theta_j.  That Gram is
@@ -1412,6 +1462,10 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     GEMB_CUDA(cudaSetDevice(c->device));
     GEMB_ARG(!(uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode == 2) || c->nranks == 1,
              "spectral_mode 2 (the composite operator -M^T M) is single-GPU: use a context without a multi-GPU communicator");
+    GEMB_ARG(!(uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode >= 3 && uo->spectral_mode <= 5) ||
+                 c->nranks == 1,
+             "spectral_modes 3-5 (common neighbours, Adamic-Adar, rooted PageRank) are single-GPU: use a context without a "
+             "multi-GPU communicator");
     GEMB_ARG(!(c->nranks > 1 && g->replicated), "multi-GPU HOPE needs row shards (upload rows [rank*ceil(n/P), ...))");
     Opts o;
     if (uo) {
@@ -1432,7 +1486,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         GEMB_ARG(uo->stop_rule == 0 || uo->stop_rule == 1, "opts.stop_rule");
         o.stop_rule = uo->stop_rule;
         if (uo->algorithm3_basis > 0) o.lanczos_basis = uo->algorithm3_basis;
-        GEMB_ARG(uo->spectral_mode >= 0 && uo->spectral_mode <= 2, "opts.spectral_mode");
+        GEMB_ARG(uo->spectral_mode >= 0 && uo->spectral_mode <= 5, "opts.spectral_mode");
         o.spectral_mode = uo->spectral_mode;
     }
     if (o.spectral_mode == 1) {
@@ -1453,12 +1507,19 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         o.algorithm = 2;
         beta = 0.f;
     }
+    if (o.spectral_mode >= 3) {
+        GEMB_ARG(o.algorithm <= 1, "spectral_modes 3-5 run on the general solver (algorithm 0 or 1): S is not a function "
+                                   "of a symmetric A");
+        o.algorithm = 1;
+        if (o.spectral_mode == 5) GEMB_ARG(beta > 0.f && beta < 1.f, "spectral_mode 5 takes alpha in beta: 0 < alpha < 1");
+        else beta = 0.f;            // unused: S = A A or A D A has no coefficient
+    }
     if (o.algorithm >= 2 && !g->symmetric && o.spectral_mode != 2) {
         set_error("algorithm=%d (works on A itself, S = f(A)) needs a symmetric shard (upload with indptr_t = NULL)", o.algorithm);
         return GEMB_ERR_ARG;
     }
     const int algo = o.algorithm ? o.algorithm : (g->symmetric ? 2 : 1);
-    const int k = o.spectral_mode ? d : d / 2;
+    const int k = (o.spectral_mode == 1 || o.spectral_mode == 2) ? d : d / 2;
     GEMB_ARG((int64_t)k <= g->n, "d/2 must not exceed the number of nodes");
     int64_t bb = std::min<int64_t>(g->n, (int64_t)k + o.oversample);
     int b = (int)((bb + 3) / 4 * 4);
@@ -1529,8 +1590,23 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         have_nrm = true;
         GEMB_TRY(clear_scratch(W));
     }
-    bool need_power = (J <= 0 && algo == 1) && !have_nrm;
-    if (W.mode == 2) {
+    bool need_power = (J <= 0 && algo == 1) && !have_nrm && W.mode < 3;
+    if (W.mode >= 3) {
+        // no norm estimate: modes 3 and 4 are two sweeps per application, and ||alpha P||_inf <= alpha bounds the rooted
+        // PageRank series a priori
+        bool nonneg = true;
+        double pinf = 0.0;
+        if (W.mode >= 4) {
+            GEMB_TRY(rowsum_bound(W, &pinf, &nonneg));
+            GEMB_ARG(nonneg, "spectral_modes 4 and 5 (Adamic-Adar, rooted PageRank) need non-negative weights");
+        }
+        if (W.mode == 4) GEMB_TRY(inv_degree(W));
+        if (W.mode != 5) J = 0;     // no series: katz_terms is ignored and reported as 0
+        if (W.mode == 5) {
+            GEMB_ARG(pinf <= 1.0 + 1e-5, "spectral_mode 5 needs P = D_out^-1 A (every row sum <= 1)");
+            if (J <= 0) J = std::max(1, std::min(4096, (int)ceil(log((double)o.katz_tol) / log((double)beta))));
+        }
+    } else if (W.mode == 2) {
         // the Perron-Frobenius shortcut (ritz_bound) does not apply to -M^T M: ||M||_2^2 by power iteration
         GEMB_TRY(estimate_composite_norm(W, o.seed, W.buf[3], W.buf[4], &nrm));
         if (!(nrm > 0.0)) nrm = 1.0;                       // M = 0: the spectrum is {0}, any positive bound holds it

@@ -18,7 +18,7 @@ namespace gemb {
 
 int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, const float *X, float gamma,
                       const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y,
-                      const HaloPushArgs *push);
+                      const HaloPushArgs *push, const float *rscale = nullptr);
 
 __device__ __forceinline__ void fma4(float4 &a, float v, const float4 &x) {
     a.x = fmaf(v, x.x, a.x);
@@ -80,12 +80,13 @@ spmm_heavy_partial_kernel(const int32_t *__restrict__ indptr, const int32_t *__r
     }
 }
 
-template <bool HAS_X0, bool HAS_SELF, bool HAS_X1>
+template <bool HAS_X0, bool HAS_SELF, bool HAS_X1, bool HAS_SCALE>
 __global__ void __launch_bounds__(256)
 spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, const int32_t *__restrict__ heavy_first,
                          int G, float alpha, float gamma, float delta, const float4 *__restrict__ partial,
                          const float4 *__restrict__ Xself, const float4 *__restrict__ X0, float4 *__restrict__ Y,
-                         bool has_push, HaloPushArgs P, float eps, const float4 *__restrict__ X1) {
+                         bool has_push, HaloPushArgs P, float eps, const float4 *__restrict__ X1,
+                         const float *__restrict__ rscale) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int h = idx / G, c = idx - h * G;
     if (h >= n_heavy) return;
@@ -96,7 +97,8 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
         const float4 t = partial[(size_t)it * G + c];
         acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
     }
-    float4 r = make_float4(alpha * acc.x, alpha * acc.y, alpha * acc.z, alpha * acc.w);
+    const float a = HAS_SCALE ? alpha * __ldg(rscale + row) : alpha;
+    float4 r = make_float4(a * acc.x, a * acc.y, a * acc.z, a * acc.w);
     if (HAS_SELF) {
         const float4 z = __ldg(Xself + row * G + c);
         r.x = fmaf(gamma, z.x, r.x); r.y = fmaf(gamma, z.y, r.y); r.z = fmaf(gamma, z.z, r.z); r.w = fmaf(gamma, z.w, r.w);
@@ -114,6 +116,8 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
 }
 
 // Y[row] = alpha * (A X)[row] + gamma * Xself[row] + delta * X0[row] (+ eps * X1[row])
+//   HAS_SCALE: alpha * rscale[row] multiplies the row's sum instead of alpha (Y = alpha diag(s) A X; the first sweep of
+//   the Adamic-Adar operator A D A, hope.cu, spectral_mode 4)
 //   Horner / Katz sweep:      gamma = 0, delta = 1, X0 = the sweep's input block
 //   Chebyshev three-term step: gamma = -2 s c0 / e (current block), delta = -s s' (previous block)
 //   the same step on the composite operator -M^T M, M = I - A (hope.cu, spectral_mode 2): the second sweep gathers
@@ -130,13 +134,14 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
 // reference it -- 16-byte posted stores over NVLink, issued while the other row groups of the SM are still gathering.
 constexpr int BULK_CAP = 3072;                 // staged ids per tile (+ up to 3 of alignment slack + 4 of over-read)
 constexpr int SPMM_TILE_PASSES = 4;            // rows per tile = passes * (256 / G)
-template <bool HAS_VAL, bool HAS_PUSH, bool HAS_X0, bool HAS_SELF, bool HAS_X1>
+template <bool HAS_VAL, bool HAS_PUSH, bool HAS_X0, bool HAS_SELF, bool HAS_X1, bool HAS_SCALE = false>
 __global__ void __launch_bounds__(256)
 spmm_bulk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                  const float *__restrict__ vals, int64_t n_rows, int64_t nnz, int G, int rows_per_cta, int tile_rows,
                  float alpha, float gamma, float delta, const float4 *__restrict__ X,
                  const float4 *__restrict__ Xself, const float4 *__restrict__ X0, float4 *__restrict__ Y,
-                 int heavy_deg, HaloPushArgs P, float eps, const float4 *__restrict__ X1) {
+                 int heavy_deg, HaloPushArgs P, float eps, const float4 *__restrict__ X1,
+                 const float *__restrict__ rscale) {
     __shared__ __align__(16) int32_t s_idx[BULK_CAP + 8];
     __shared__ __align__(16) float s_val[HAS_VAL ? BULK_CAP + 8 : 4];
     __shared__ __align__(8) uint64_t s_bar;
@@ -198,7 +203,8 @@ spmm_bulk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__
                 }
                 for (; i < e; i++) fma4(acc, HAS_VAL ? __ldg(vals + i) : 1.f, __ldg(X + (int64_t)__ldg(indices + i) * G + c));
             }
-            float4 r = make_float4(alpha * acc.x, alpha * acc.y, alpha * acc.z, alpha * acc.w);
+            const float a = HAS_SCALE ? alpha * __ldg(rscale + row) : alpha;
+            float4 r = make_float4(a * acc.x, a * acc.y, a * acc.z, a * acc.w);
             if (HAS_SELF) {
                 const float4 z = __ldg(Xself + row * G + c);
                 r.x = fmaf(gamma, z.x, r.x); r.y = fmaf(gamma, z.y, r.y); r.z = fmaf(gamma, z.z, r.z); r.w = fmaf(gamma, z.w, r.w);
@@ -244,7 +250,7 @@ int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, fl
     spmm_bulk_kernel<V, PU, Z, S, false><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, n_rows, \
                                                                               A.nnz, G, rows_per_cta, tile_rows, alpha, \
                                                                               gamma, delta, X4, XS4, X04, Y4, hd, PA, 0.f, \
-                                                                              nullptr)
+                                                                              nullptr, nullptr)
 #define LAUNCHB(V, PU)                                                                                                   \
     do {                                                                                                                 \
         if (X0 && Xself) LAUNCH(V, PU, true, true); else if (X0) LAUNCH(V, PU, true, false);                             \
@@ -278,7 +284,7 @@ int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, fl
 #define LAUNCH(V)                                                                                                        \
     spmm_bulk_kernel<V, false, true, true, true><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(                            \
         A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta, tile_rows, alpha, gamma, delta, (const float4 *)X, \
-        (const float4 *)Xself, (const float4 *)X0, (float4 *)Y, hd, PA, eps, (const float4 *)X1)
+        (const float4 *)Xself, (const float4 *)X0, (float4 *)Y, hd, PA, eps, (const float4 *)X1, nullptr)
     if (A.data) LAUNCH(true);
     else LAUNCH(false);
 #undef LAUNCH
@@ -288,9 +294,36 @@ int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, fl
     return spmm_heavy_launch(ctx, A, b, alpha, X, gamma, Xself, delta, X0, eps, X1, Y, nullptr);
 }
 
+int spmm_scaled_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
+                       const float *rscale, float *Y) {
+    GEMB_ARG(rscale, "spmm_scaled_launch: rscale");
+    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "block width must be a multiple of 4, <= 1024");
+    if (n_rows == 0) return GEMB_OK;
+    const int G = b / 4;
+    const int rows_per_cta = 256 / G;
+    const int tile_rows = rows_per_cta * SPMM_TILE_PASSES;
+    const int64_t n_tiles = (n_rows + tile_rows - 1) / tile_rows;
+    GEMB_ARG(n_tiles < (int64_t)2147483647, "grid too large");
+    const bool heavy = A.n_items > 0;
+    const int hd = heavy ? SPMM_HEAVY_DEG : 0;
+    HaloPushArgs PA;
+    memset(&PA, 0, sizeof PA);
+#define LAUNCH(V)                                                                                                        \
+    spmm_bulk_kernel<V, false, false, false, false, true><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(                   \
+        A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta, tile_rows, alpha, 0.f, 0.f, (const float4 *)X,     \
+        nullptr, nullptr, (float4 *)Y, hd, PA, 0.f, nullptr, rscale)
+    if (A.data) LAUNCH(true);
+    else LAUNCH(false);
+#undef LAUNCH
+    GEMB_CUDA(cudaGetLastError());
+    count_launch();
+    if (!heavy) return GEMB_OK;
+    return spmm_heavy_launch(ctx, A, b, alpha, X, 0.f, nullptr, 0.f, nullptr, 0.f, nullptr, Y, nullptr, rscale);
+}
+
 int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, const float *X, float gamma,
                       const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y,
-                      const HaloPushArgs *push) {
+                      const HaloPushArgs *push, const float *rscale) {
     const int G = b / 4;
     const int rows_per_cta = 256 / G;
     const float4 *X4 = (const float4 *)X, *X04 = (const float4 *)X0, *XS4 = (const float4 *)Xself;
@@ -315,13 +348,14 @@ int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, 
 #undef HP
         GEMB_CUDA(cudaGetLastError());
         const int fgrid = (int)(((int64_t)A.n_heavy * G + 255) / 256);
-#define FIN(Z, S, X1P) spmm_heavy_finish_kernel<Z, S, X1P><<<fgrid, 256, 0, ctx->stream>>>(A.n_heavy, A.heavy_row, A.heavy_first, G, \
-                                                                    alpha, gamma, delta, P4, XS4, X04, Y4, push != nullptr, PA, eps, X14)
-        if (X1) FIN(true, true, true);                 // spmm4_launch: X1 comes with Xself and X0
-        else if (X0 && Xself) FIN(true, true, false);
-        else if (X0) FIN(true, false, false);
-        else if (Xself) FIN(false, true, false);
-        else FIN(false, false, false);
+#define FIN(Z, S, X1P, SC) spmm_heavy_finish_kernel<Z, S, X1P, SC><<<fgrid, 256, 0, ctx->stream>>>(A.n_heavy, A.heavy_row,  \
+                                         A.heavy_first, G, alpha, gamma, delta, P4, XS4, X04, Y4, push != nullptr, PA, eps, X14, rscale)
+        if (rscale) FIN(false, false, false, true);    // spmm_scaled_launch: no other epilogue operand
+        else if (X1) FIN(true, true, true, false);     // spmm4_launch: X1 comes with Xself and X0
+        else if (X0 && Xself) FIN(true, true, false, false);
+        else if (X0) FIN(true, false, false, false);
+        else if (Xself) FIN(false, true, false, false);
+        else FIN(false, false, false, false);
 #undef FIN
         GEMB_CUDA(cudaGetLastError());
         count_launch(2);

@@ -138,7 +138,7 @@ int gemb_apply(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const float *M,
 int gemb_chol_inverse(gemb_ctx *ctx, int b, const double *G, double *Minv64_out, float *Minv32_out, int *rank_out);
 int gemb_eigh(gemb_ctx *ctx, int b, const double *G, double rel_tol, double *w_out, double *Z_out);
 
-/* ---- HOPE.  Replaces hope.py:29-36: S = (I - beta A)^-1 beta A is never formed; its top
+/* ---- HOPE.  Replaces hope.py:29-36: S = (I - beta A)^-1 beta A (or, by spectral_mode, another proximity) is never formed; its top
  * k = d/2 singular triplets come from a block subspace iteration with Rayleigh-Ritz whose
  * operator applications are CSR SpMM sweeps (Katz/Horner sweeps of S and S^T in general; a Chebyshev
  * filter in A itself when A is symmetric, since then S = f(A)).  Output convention = the reference:
@@ -194,13 +194,27 @@ typedef struct {
                               measures are taken relative to that bound, not to each small eigenvalue:
                               stop_rule 0: max_j |l_j - l_j'| / ||M||_2^2 (round 1: not converged);  stop_rule 1: max_j ||M^T M v_j - sigma_j^2 v_j||
                               / ||M||_2^2.  Device memory: one n x b block more than modes 0 and 1 (T).  spmm_count counts
-                              two sweeps per application. */
+                              two sweeps per application.
+                              3, 4, 5 = HOPE on another proximity S (Ou et al., KDD 2016, Table 1), same output as mode 0
+                              (k = d/2 triplets of S, d even; X_out = [U sqrt(Sigma) | V sqrt(Sigma)], sigma ascending):
+                              3 = common neighbours S = A A;  4 = Adamic-Adar S = A D A, D_ii = 1 / (sum_j A_ij + sum_j A_ji),
+                              0 where that sum is 0 (computed on the device from A and A^T: n floats);  5 = rooted PageRank
+                              S = (1 - alpha) sum_{j=0..J} (alpha P)^j ~ (1 - alpha) (I - alpha P)^-1, the upload being
+                              P = D_out^-1 A and its transpose, normalised by the caller (row sums <= 1, else GEMB_ERR_ARG),
+                              alpha passed in `beta`, 0 < alpha < 1.  J = ceil(log(katz_tol) / log(alpha)) (||alpha P||_inf
+                              <= alpha; no power iteration), or katz_terms when given.  Modes 4 and 5 refuse negative
+                              weights.  S and S^T are applied matrix-free by the general solver: algorithm 0 resolves to 1;
+                              algorithms 2 and 3, a multi-GPU communicator and (mode 5) alpha outside (0, 1) are
+                              GEMB_ERR_ARG before any work.  compute_residual and both stop_rules work on this S.  Modes 3
+                              and 4 apply S as two sweeps (T = D op(A) X, then op(A) T; S^T takes A^T), mode 5 as J sweeps.
+                              Stats: katz_terms = J (mode 5) or 0; norm2_A = 0 (no norm estimate is made); beta_used =
+                              alpha (mode 5) or 0; spmm_count counts every sweep. */
 } gemb_hope_opts;
 
 typedef struct {
     uint32_t struct_size;
     int32_t iters;         /* subspace iterations performed */
-    int32_t katz_terms;    /* J actually used */
+    int32_t katz_terms;    /* J actually used (spectral_mode 5: the rooted-PageRank series' J; 3, 4: 0) */
     int32_t block;         /* b */
     int32_t converged;
     int32_t algorithm;     /* 1 or 2: the solver that ran */
@@ -212,10 +226,10 @@ typedef struct {
     double comm_ms;        /* NCCL time (multi-GPU) */
     double total_ms;       /* device time of the whole call (events), excluding H2D/D2H */
     double h2d_ms, d2h_ms;
-    float norm2_A;         /* estimated ||A||_2 (spectral_mode 2: ||M||_2^2) */
+    float norm2_A;         /* estimated ||A||_2 (spectral_mode 2: ||M||_2^2; spectral_modes 3-5: 0, not estimated) */
     float ritz_change;     /* algorithms 1 and 2: the last round's change measure (stop_rule 0 above), whichever rule
                               stopped; algorithm 3: the last restart's residual estimate (= resid_est) */
-    float resid_max;       /* max_j ||S^T u_j - sigma_j v_j|| / sigma_max (compute_residual=1; spectral_mode 0) */
+    float resid_max;       /* max_j ||S^T u_j - sigma_j v_j|| / sigma_max (compute_residual=1; spectral_modes 0, 3-5) */
     float resid_est;       /* the residual estimate of the last round (stop_rule 1 above; algorithm 3: max_j
                               |f'(l_j)| ||A v_j - l_j v_j|| / sigma_max from the Lanczos coupling block, computed for
                               either stop_rule), else -1 */
@@ -225,7 +239,8 @@ typedef struct {
     int64_t halo_rows;     /* mg_mode 2: distinct remote rows this shard references */
     int64_t push_rows;     /* mg_mode 2: (row, peer) pairs this rank stores per exchanged block */
     int64_t pushes;        /* mg_mode 2: blocks exchanged in this call (NVLink bytes out = pushes*push_rows*4*block) */
-    float beta_used;       /* the beta the solve ran with (differs from the argument when that was negative) */
+    float beta_used;       /* the beta the solve ran with (differs from the argument when that was negative;
+                              spectral_mode 5: alpha; 1-4: 0) */
     double push_bytes;     /* mg_mode 2: bytes this rank stored into its peers over NVLink in this call */
 } gemb_hope_stats;
 
