@@ -17,7 +17,8 @@ UNIQUE_ID_BYTES = 128
 EXPORTS = [
     'gemb_version', 'gemb_last_error', 'gemb_device_count', 'gemb_launch_count', 'gemb_ctx_create', 'gemb_ctx_destroy',
     'gemb_host_alloc', 'gemb_host_free', 'gemb_mem_trim', 'gemb_mem_cached_bytes', 'gemb_mem_live_blocks', 'gemb_comm_unique_id', 'gemb_comm_init', 'gemb_graph_upload',
-    'gemb_graph_free', 'gemb_spmm', 'gemb_spmm4', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
+    'gemb_graph_free', 'gemb_spmm', 'gemb_spmm4', 'gemb_spmm_scaled', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope',
+    'gemb_hope_apply', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
     'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk', 'gemb_cc_create', 'gemb_cc_info', 'gemb_cc_labels', 'gemb_cc_lcc',
@@ -103,7 +104,10 @@ def lib():
     L.gemb_apply.argtypes = [vp, i64, vp, ctypes.c_int, vp, ctypes.c_int, ctypes.c_int, vp]
     L.gemb_chol_inverse.argtypes = [vp, ctypes.c_int, vp, vp, vp, ctypes.POINTER(ctypes.c_int)]
     L.gemb_eigh.argtypes = [vp, ctypes.c_int, vp, f64, vp, vp]
+    L.gemb_spmm_scaled.argtypes = [vp, ctypes.c_int, ctypes.c_int, f32, vp, vp, vp]
     L.gemb_hope.argtypes = [vp, ctypes.c_int, f32, ctypes.POINTER(HopeOpts), vp, vp, ctypes.POINTER(HopeStats)]
+    L.gemb_hope_apply.argtypes = [vp, ctypes.POINTER(HopeOpts), f32, ctypes.c_int, ctypes.c_int, vp, vp,
+                                  ctypes.POINTER(ctypes.c_int)]
     L.gemb_hope_svd_error.argtypes = [vp, ctypes.c_int, f32, vp, ctypes.c_int, ctypes.c_uint64, ctypes.POINTER(f64)]
     L.gemb_n2v_alias.argtypes = [vp, vp, vp, vp]
     L.gemb_n2v_walks.argtypes = [vp, vp, vp, i64, ctypes.c_int, ctypes.c_int, f64, f64, i32, i64, i64, vp,
@@ -359,15 +363,42 @@ class DeviceGraph(_Handle):
                                float(delta), _ptr(ops[1]), float(eps), _ptr(ops[2]), _ptr(Y)))
         return Y
 
+    def spmm_scaled(self, X, rscale, alpha=1.0, transpose=False):
+        """Y = alpha diag(rscale) op(A) X (the row-scaled sweep of the Adamic-Adar operator; single GPU; test hook)."""
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        rscale = np.ascontiguousarray(rscale, dtype=np.float32)
+        assert X.shape[0] == self.n and rscale.shape == (self.n,)
+        Y = np.empty_like(X)
+        check(lib().gemb_spmm_scaled(self._h, int(bool(transpose)), X.shape[1], float(alpha), _ptr(X), _ptr(rscale),
+                                     _ptr(Y)))
+        return Y
+
+    @staticmethod
+    def _hope_opts(opts):
+        return HopeOpts(struct_size=ctypes.sizeof(HopeOpts), oversample=int(opts.get('oversample', -1)),
+                        max_iters=int(opts.get('max_iters', 0)), min_iters=int(opts.get('min_iters', 0)),
+                        tol=float(opts.get('tol', 0.0)), katz_terms=int(opts.get('katz_terms', 0)),
+                        katz_tol=float(opts.get('katz_tol', 0.0)), seed=int(opts.get('seed', 0)),
+                        compute_residual=int(opts.get('compute_residual', 0)), verbose=int(opts.get('verbose', 0)),
+                        algorithm=int(opts.get('algorithm', 0)), cheb_degree=int(opts.get('cheb_degree', 0)),
+                        cheb_range_log2=float(opts.get('cheb_range_log2', 0.0)), stop_rule=int(opts.get('stop_rule', 0)),
+                        algorithm3_basis=int(opts.get('algorithm3_basis', 0)),
+                        spectral_mode=int(opts.get('spectral_mode', 0)))
+
+    def hope_apply(self, X, beta, transpose=False, **opts):
+        """(Y, J): one application of the operator gemb_hope uses for opts['spectral_mode'] -- S X or S^T X (modes 0,
+        3-5), the symmetric solver's Op X (modes 1, 2) -- and the series' terms J (gemb_hope_apply; test hook)."""
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        assert X.ndim == 2 and X.shape[0] == self.n
+        o = self._hope_opts(opts)
+        Y = np.empty_like(X)
+        J = ctypes.c_int(-1)
+        check(lib().gemb_hope_apply(self._h, ctypes.byref(o), float(beta), int(bool(transpose)), X.shape[1], _ptr(X),
+                                    _ptr(Y), ctypes.byref(J)))
+        return Y, int(J.value)
+
     def hope(self, d, beta, out=None, want_output=True, **opts):
-        o = HopeOpts(struct_size=ctypes.sizeof(HopeOpts), oversample=int(opts.get('oversample', -1)),
-                     max_iters=int(opts.get('max_iters', 0)), min_iters=int(opts.get('min_iters', 0)),
-                     tol=float(opts.get('tol', 0.0)), katz_terms=int(opts.get('katz_terms', 0)),
-                     katz_tol=float(opts.get('katz_tol', 0.0)), seed=int(opts.get('seed', 0)),
-                     compute_residual=int(opts.get('compute_residual', 0)), verbose=int(opts.get('verbose', 0)),
-                     algorithm=int(opts.get('algorithm', 0)), cheb_degree=int(opts.get('cheb_degree', 0)),
-                     cheb_range_log2=float(opts.get('cheb_range_log2', 0.0)), stop_rule=int(opts.get('stop_rule', 0)),
-                     algorithm3_basis=int(opts.get('algorithm3_basis', 0)), spectral_mode=int(opts.get('spectral_mode', 0)))
+        o = self._hope_opts(opts)
         st = HopeStats(struct_size=ctypes.sizeof(HopeStats))
         X = sig = None
         if want_output:

@@ -1451,13 +1451,11 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
     return GEMB_OK;
 }
 
-extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts *uo, float *X_out,
-                         float *sigma_out, gemb_hope_stats *stats) {
-    GEMB_ARG(g != nullptr, "graph");
-    GEMB_ARG(d >= 1, "d must be >= 1");
-    GEMB_ARG((uo && uo->struct_size == sizeof(gemb_hope_opts) && (uo->spectral_mode == 1 || uo->spectral_mode == 2)) || d % 2 == 0,
-             "d must be even (k = d/2 singular triplets)");
-    GEMB_ARG(!stats || stats->struct_size == sizeof(gemb_hope_stats), "stats.struct_size");
+namespace gemb {
+
+// The option parsing and argument checks of gemb_hope and gemb_hope_apply (nothing is launched): the user's options
+// over the defaults into *po, and each spectral_mode's coefficient into *beta (0 where the mode has none).
+static int hope_options(gemb_graph *g, float *beta, const gemb_hope_opts *uo, Opts *po) {
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
     GEMB_ARG(!(uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode == 2) || c->nranks == 1,
@@ -1493,7 +1491,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         GEMB_ARG(g->symmetric, "spectral_mode 1 (largest algebraic eigenpairs) needs a symmetric upload");
         GEMB_ARG(o.algorithm == 0 || o.algorithm == 2, "spectral_mode 1 runs on the Chebyshev-filtered subspace iteration (algorithm 0 or 2)");
         o.algorithm = 2;
-        beta = 0.f;                 // unused: the ranking is by the eigenvalue itself
+        *beta = 0.f;                // unused: the ranking is by the eigenvalue itself
     }
     if (o.spectral_mode == 2) {
         // The wanted end of -M^T M (sigma^2 ~ 1e-2) is a sliver of a spectrum ||M||_2^2 wide (1246 on R-MAT 20's largest
@@ -1505,19 +1503,56 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
                                 "indices_t, data_t): M^T M is applied as a sweep of A and a sweep of A^T");
         GEMB_ARG(o.algorithm == 0 || o.algorithm == 2, "spectral_mode 2 runs on the Chebyshev-filtered subspace iteration (algorithm 0 or 2)");
         o.algorithm = 2;
-        beta = 0.f;
+        *beta = 0.f;
     }
     if (o.spectral_mode >= 3) {
         GEMB_ARG(o.algorithm <= 1, "spectral_modes 3-5 run on the general solver (algorithm 0 or 1): S is not a function "
                                    "of a symmetric A");
         o.algorithm = 1;
-        if (o.spectral_mode == 5) GEMB_ARG(beta > 0.f && beta < 1.f, "spectral_mode 5 takes alpha in beta: 0 < alpha < 1");
-        else beta = 0.f;            // unused: S = A A or A D A has no coefficient
+        if (o.spectral_mode == 5) GEMB_ARG(*beta > 0.f && *beta < 1.f, "spectral_mode 5 takes alpha in beta: 0 < alpha < 1");
+        else *beta = 0.f;           // unused: S = A A or A D A has no coefficient
     }
     if (o.algorithm >= 2 && !g->symmetric && o.spectral_mode != 2) {
         set_error("algorithm=%d (works on A itself, S = f(A)) needs a symmetric shard (upload with indptr_t = NULL)", o.algorithm);
         return GEMB_ERR_ARG;
     }
+    *po = o;
+    return GEMB_OK;
+}
+
+// The set-up of spectral_modes 3-5 on the device, before the first application of S (W's scalars allocated):
+// modes 4 and 5 refuse negative weights and mode 5 a row sum of P above 1 (one pass over the CSR, csr_rowsum_kernel),
+// mode 4 builds D (inv_degree), mode 5 takes J = ceil(log katz_tol / log alpha) unless katz_terms gave one.  *J: in,
+// opts.katz_terms (0: not given); out, the series' terms (0 for modes 3 and 4).  No norm estimate: modes 3 and 4 are
+// two sweeps per application, and ||alpha P||_inf <= alpha bounds the rooted PageRank series a priori.
+static int proximity_setup(HopeWork &W, const Opts &o, float beta, int *J) {
+    bool nonneg = true;
+    double pinf = 0.0;
+    if (W.mode >= 4) {
+        GEMB_TRY(rowsum_bound(W, &pinf, &nonneg));
+        GEMB_ARG(nonneg, "spectral_modes 4 and 5 (Adamic-Adar, rooted PageRank) need non-negative weights");
+    }
+    if (W.mode == 4) GEMB_TRY(inv_degree(W));
+    if (W.mode != 5) *J = 0;    // no series: katz_terms is ignored and reported as 0
+    if (W.mode == 5) {
+        GEMB_ARG(pinf <= 1.0 + 1e-5, "spectral_mode 5 needs P = D_out^-1 A (every row sum <= 1)");
+        if (*J <= 0) *J = std::max(1, std::min(4096, (int)ceil(log((double)o.katz_tol) / log((double)beta))));
+    }
+    return GEMB_OK;
+}
+
+}  // namespace gemb
+
+extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts *uo, float *X_out,
+                         float *sigma_out, gemb_hope_stats *stats) {
+    GEMB_ARG(g != nullptr, "graph");
+    GEMB_ARG(d >= 1, "d must be >= 1");
+    GEMB_ARG((uo && uo->struct_size == sizeof(gemb_hope_opts) && (uo->spectral_mode == 1 || uo->spectral_mode == 2)) || d % 2 == 0,
+             "d must be even (k = d/2 singular triplets)");
+    GEMB_ARG(!stats || stats->struct_size == sizeof(gemb_hope_stats), "stats.struct_size");
+    gemb_ctx *c = g->ctx;
+    Opts o;
+    GEMB_TRY(hope_options(g, &beta, uo, &o));
     const int algo = o.algorithm ? o.algorithm : (g->symmetric ? 2 : 1);
     const int k = (o.spectral_mode == 1 || o.spectral_mode == 2) ? d : d / 2;
     GEMB_ARG((int64_t)k <= g->n, "d/2 must not exceed the number of nodes");
@@ -1592,20 +1627,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     }
     bool need_power = (J <= 0 && algo == 1) && !have_nrm && W.mode < 3;
     if (W.mode >= 3) {
-        // no norm estimate: modes 3 and 4 are two sweeps per application, and ||alpha P||_inf <= alpha bounds the rooted
-        // PageRank series a priori
-        bool nonneg = true;
-        double pinf = 0.0;
-        if (W.mode >= 4) {
-            GEMB_TRY(rowsum_bound(W, &pinf, &nonneg));
-            GEMB_ARG(nonneg, "spectral_modes 4 and 5 (Adamic-Adar, rooted PageRank) need non-negative weights");
-        }
-        if (W.mode == 4) GEMB_TRY(inv_degree(W));
-        if (W.mode != 5) J = 0;     // no series: katz_terms is ignored and reported as 0
-        if (W.mode == 5) {
-            GEMB_ARG(pinf <= 1.0 + 1e-5, "spectral_mode 5 needs P = D_out^-1 A (every row sum <= 1)");
-            if (J <= 0) J = std::max(1, std::min(4096, (int)ceil(log((double)o.katz_tol) / log((double)beta))));
-        }
+        GEMB_TRY(proximity_setup(W, o, beta, &J));
     } else if (W.mode == 2) {
         // the Perron-Frobenius shortcut (ritz_bound) does not apply to -M^T M: ||M||_2^2 by power iteration
         GEMB_TRY(estimate_composite_norm(W, o.seed, W.buf[3], W.buf[4], &nrm));
@@ -1702,5 +1724,35 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         stats->ritz_change = (float)R.change;
         stats->resid_max = R.resid_max;
     }
+    return GEMB_OK;
+}
+
+extern "C" int gemb_hope_apply(gemb_graph *g, const gemb_hope_opts *uo, float beta, int transpose, int b, const float *X,
+                               float *Y, int *J_out) {
+    GEMB_ARG(g && uo && X && Y, "graph/opts/X/Y");
+    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "b must be a positive multiple of 4, <= 1024");
+    gemb_ctx *c = g->ctx;
+    GEMB_ARG(c->nranks == 1 && g->n_local == g->n, "gemb_hope_apply is single-GPU");
+    Opts o;
+    GEMB_TRY(hope_options(g, &beta, uo, &o));
+    GEMB_ARG(o.spectral_mode != 0 || (o.katz_terms > 0 && beta >= 0.f),
+             "spectral_mode 0 needs opts.katz_terms > 0 and beta >= 0 (no norm estimate is made)");
+    const int64_t n = g->n;
+    const size_t blk = (size_t)n * b;
+    HopeWork W;
+    W.g = g; W.c = c; W.b = b; W.rows = n; W.shard = n;
+    W.mode = o.spectral_mode;
+    GEMB_TRY(W.alloc_blocks(blk));
+    GEMB_CUDA(W.scal.alloc(2));
+    if (W.mode == 2) GEMB_CUDA(W.opT.alloc(blk));
+    int J = o.katz_terms;
+    if (W.mode >= 3) GEMB_TRY(proximity_setup(W, o, beta, &J));
+    else if (W.mode != 0) J = 0;
+    float *in = W.buf[0], *out = W.buf[1];
+    GEMB_CUDA(cudaMemcpyAsync(in, X, sizeof(float) * blk, cudaMemcpyHostToDevice, c->stream));
+    if (W.mode == 1 || W.mode == 2) GEMB_TRY(op_apply(W, b, 1.f, in, 0.f, false, 1.f, nullptr, out, false));
+    else GEMB_TRY(apply_S(W, transpose != 0, beta, J, in, out, W.buf[2], W.buf[3]));
+    GEMB_TRY(copy_sync(c, Y, out, sizeof(float) * blk, cudaMemcpyDeviceToHost));
+    if (J_out) *J_out = J;
     return GEMB_OK;
 }

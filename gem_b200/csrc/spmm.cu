@@ -397,3 +397,23 @@ extern "C" int gemb_spmm4(gemb_graph *g, int transpose, int b, float alpha, cons
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     return GEMB_OK;
 }
+
+extern "C" int gemb_spmm_scaled(gemb_graph *g, int transpose, int b, float alpha, const float *X, const float *rscale,
+                                float *Y) {
+    GEMB_ARG(g && X && rscale && Y, "graph/X/rscale/Y");
+    GEMB_ARG(b > 0 && b % 4 == 0, "b must be a positive multiple of 4");
+    gemb_ctx *c = g->ctx;
+    GEMB_ARG(c->nranks == 1 && g->n_local == g->n, "gemb_spmm_scaled is single-GPU");
+    GEMB_CUDA(cudaSetDevice(c->device));
+    DeviceBuffer<float> dX, dS, dY;
+    const size_t full = (size_t)g->n * b;
+    GEMB_CUDA(dX.alloc(full));
+    GEMB_CUDA(dS.alloc((size_t)std::max<int64_t>(g->n, 1)));
+    GEMB_CUDA(dY.alloc(full));
+    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * full, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(cudaMemcpyAsync(dS.get(), rscale, sizeof(float) * g->n, cudaMemcpyHostToDevice, c->stream));
+    GEMB_TRY(spmm_scaled_launch(c, transpose ? g->AT : g->A, g->n, b, alpha, dX.get(), dS.get(), dY.get()));
+    GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * full, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    return GEMB_OK;
+}

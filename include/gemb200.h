@@ -116,6 +116,10 @@ int gemb_spmm(gemb_graph *g, int transpose, int b, float alpha, const float *X, 
  * Y = alpha * op(A) * X + gamma * Xself + delta * X0 + eps * X1; X1 == NULL is gemb_spmm, else Xself and X0 are needed. */
 int gemb_spmm4(gemb_graph *g, int transpose, int b, float alpha, const float *X, float gamma, const float *Xself,
                float delta, const float *X0, float eps, const float *X1, float *Y);
+/* The sweep with a per-row scale, as the first sweep of spectral_mode 4 (Adamic-Adar) runs it, on light and heavy rows:
+ * Y = alpha * diag(rscale) * op(A) * X.  X and Y are n x b, rscale n floats; all HOST.  Single GPU (row0 = 0,
+ * n_local = n, no communicator).  b must be a multiple of 4, <= 1024. */
+int gemb_spmm_scaled(gemb_graph *g, int transpose, int b, float alpha, const float *X, const float *rscale, float *Y);
 
 /* Test hook for the tensor-core contraction: G (b1 x b2, fp64, row-major) = P^T Q over n rows; P, Q host
  * fp32 row-major (Q == NULL means Q = P).  use_tensor_cores: 1 = wgmma kernel (GEMB_ERR_UNSUPPORTED if the
@@ -250,6 +254,17 @@ typedef struct {
  * iteration inside the call -- BASELINE.json configs[3] prescribes beta = 0.5 / rho_hat(A); stats->beta_used reports it. */
 int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts *opts, float *X_out,
               float *sigma_out, gemb_hope_stats *stats);
+
+/* Test hook: one application of the operator gemb_hope solves for opts->spectral_mode, through the same option checks
+ * and device set-up (negative-weight and row-sum refusals, D, the rooted-PageRank J):
+ *   modes 0, 3, 4, 5: Y = S X, or S^T X (transpose), S as spectral_mode describes it -- mode 0 the Katz series
+ *                     sum_{j=1..J} (beta A)^j with J = opts->katz_terms, which must be > 0 (no norm estimate is made),
+ *                     and beta >= 0;
+ *   modes 1, 2:       Y = Op X, the symmetric solver's operator (A, or the composite -M^T M); transpose is ignored.
+ * X and Y are n x b, b a multiple of 4, <= 1024; all HOST.  *J_out (may be NULL): the series' terms used (modes 0 and 5),
+ * else 0.  Single GPU (row0 = 0, n_local = n, no communicator). */
+int gemb_hope_apply(gemb_graph *g, const gemb_hope_opts *opts, float beta, int transpose, int b, const float *X,
+                    float *Y, int *J_out);
 
 /* The diagnostic hope.py:38-40 prints: || U diag(s) V^T - S ||_F = || X1 X2^T - S ||_F with S = (I - beta A)^-1 beta A.
  * X: host, n x d row-major fp32 (the embedding gemb_hope returned).  S is never stored whole:

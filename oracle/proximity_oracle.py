@@ -118,6 +118,58 @@ def embedding(A, proximity, d, alpha=None, dense_max=3000, tol=1e-12, seed=0, te
     return np.concatenate((u * np.sqrt(s)[None, :], vt.T * np.sqrt(s)[None, :]), axis=1), s
 
 
+def _apply(A, mode, X, transpose, coef, terms, absolute):
+    A = sp.csr_matrix(A, dtype=np.float64)
+    X = np.asarray(X, dtype=np.float64)
+    d = inv_degree(A) if mode == 4 else None
+    if absolute:
+        A, X, d = abs(A), np.abs(X), (None if d is None else np.abs(d))
+        coef = None if coef is None else abs(float(coef))
+    M = A.T.tocsr() if transpose and mode not in (1, 2) else A
+    if mode in (0, 5):
+        if terms is None or terms < 1:
+            raise ValueError('modes 0 and 5 need terms >= 1')
+        W = X
+        for _ in range(terms - 1 if mode == 0 else terms):
+            W = X + coef * (M @ W)
+        return coef * (M @ W) if mode == 0 else (1.0 - coef) * W
+    if mode == 1:
+        return M @ X
+    if mode == 2:
+        if absolute:
+            T = X + M @ X
+            return M.T @ T + T
+        T = X - M @ X
+        return M.T @ T - T
+    if mode in (3, 4):
+        Y = M @ X
+        if mode == 4:
+            Y = d[:, None] * Y
+        return M @ Y
+    raise ValueError(mode)
+
+
+def operator_apply(A, mode, X, transpose=False, coef=None, terms=None):
+    """Y = S X, or S^T X (transpose), in fp64 for gemb_hope's operator of spectral_mode `mode` on the matrix A AS
+    UPLOADED (never formed; X an n x b block):
+        0  Katz:                 S = sum_{j=1..terms} (coef A)^j               (coef = beta)
+        1  the matrix itself:    S = A                                          (transpose ignored: A symmetric)
+        2  LLE composite:        S = -M^T M, M = I - A, A = P = D^-1 W          (transpose ignored: S symmetric)
+        3  common neighbours:    S = A A
+        4  Adamic-Adar:          S = A D A, D = inv_degree(A)
+        5  rooted PageRank:      S = (1 - coef) sum_{j=0..terms} (coef A)^j     (coef = alpha, A = P as uploaded: not
+                                                                                 renormalised, unlike proximity_dense)
+    S^T takes A^T wherever A appears (A^T D A^T for mode 4)."""
+    return _apply(A, mode, X, transpose, coef, terms, False)
+
+
+def operator_abs(A, mode, X, transpose=False, coef=None, terms=None):
+    """The same products on |A|, |D|, |X| and |coef| (mode 2: (I + |A|^T)(I + |A|) |X|): the sum of the magnitudes of
+    every term, the scale of the per-entry forward error of any summation order.  Equal to operator_apply when A >= 0
+    and X >= 0, except for mode 2, whose S has negative entries."""
+    return _apply(A, mode, X, transpose, coef, terms, True)
+
+
 def residuals(A, proximity, X, sigma, alpha=None, S=None):
     """Per triplet of an embedding X = [U sqrt(sigma) | V sqrt(sigma)]: ||S v - sigma u|| / sigma_max and
     ||S^T u - sigma v|| / sigma_max, in fp64 with u = X1_j / sqrt(sigma_j), v = X2_j / sqrt(sigma_j).  S: a matrix or

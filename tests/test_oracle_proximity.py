@@ -114,3 +114,100 @@ def test_embedding_layout_and_residuals(proximity):
     Xm, sm = po.embedding(A, proximity, 8, alpha=alpha, dense_max=0)
     assert np.allclose(sm, s, rtol=1e-10)
     assert np.linalg.norm(Xm[:, :4] @ Xm[:, 4:].T - X1 @ X2.T) < 1e-9 * np.linalg.norm(X1 @ X2.T)
+
+
+# ----------------------------------------------------------------- operator_apply / operator_abs (gemb_hope_apply's oracle)
+def _dense_operator(A, mode, transpose, coef, terms, absolute=False):
+    """The dense matrix operator_apply (absolute: operator_abs) multiplies by, built independently of it."""
+    Ad = A.toarray()
+    n = Ad.shape[0]
+    if absolute:
+        Ad, coef = np.abs(Ad), (None if coef is None else abs(coef))
+    if mode == 0:
+        S, T = np.zeros((n, n)), np.eye(n)
+        for _ in range(terms):
+            T = coef * Ad @ T
+            S += T
+    elif mode == 1:
+        S = Ad
+    elif mode == 2:
+        M = np.eye(n) + Ad if absolute else np.eye(n) - Ad
+        S = M.T @ M if absolute else -(M.T @ M)
+    elif mode in (3, 4):
+        if absolute:
+            D = np.abs(po.inv_degree(A)) if mode == 4 else np.ones(n)
+            S = Ad @ np.diag(D) @ Ad
+        else:
+            S = po.proximity_dense(A, 'common_neighbors' if mode == 3 else 'adamic_adar')
+    else:
+        S, T = np.eye(n), np.eye(n)
+        for _ in range(terms):
+            T = coef * Ad @ T
+            S += T
+        S = (1.0 - coef) * S
+    return S.T if transpose and mode not in (1, 2) else S
+
+
+def _signed_digraph():
+    A = po.random_digraph(n=60, seed=5, p=0.12)
+    A.data = A.data * np.random.default_rng(1).choice([-1.0, 1.0], A.nnz)
+    return A
+
+
+@pytest.mark.parametrize('transpose', [False, True])
+@pytest.mark.parametrize('mode,coef,terms', [(0, 0.07, 1), (0, 0.07, 6), (1, None, None), (2, None, None),
+                                             (3, None, None), (4, None, None), (5, 0.6, 1), (5, 0.6, 9)])
+def test_operator_apply_equals_dense(mode, coef, terms, transpose):
+    """operator_apply and operator_abs against dense matrices on a directed graph with an isolated node and a row
+    without out-edges (signed for operator_abs, so that |.| matters), and the mode-5 series against proximity_dense's on
+    P = transition(A)."""
+    A = po.random_digraph(n=60, seed=5, p=0.12)
+    if mode == 1:
+        A = (A + A.T).tocsr()
+    if mode == 2:
+        A = po.transition(A)
+    X = np.random.default_rng(2).standard_normal((A.shape[0], 7))
+    for absolute, B in ((False, A), (True, _signed_digraph() if mode != 1 else (_signed_digraph() + _signed_digraph().T))):
+        fn = po.operator_abs if absolute else po.operator_apply
+        Y = fn(B, mode, X, transpose=transpose, coef=coef, terms=terms)
+        S = _dense_operator(B, mode, transpose, coef, terms, absolute)
+        ref = S @ (np.abs(X) if absolute else X)
+        assert np.abs(Y - ref).max() <= 1e-13 * max(1.0, np.abs(ref).max())
+    if mode == 5:
+        S = po.proximity_dense(po.random_digraph(n=60, seed=5, p=0.12), 'rooted_pagerank', alpha=coef, terms=terms)
+        Y = po.operator_apply(po.transition(po.random_digraph(n=60, seed=5, p=0.12)), 5, X, transpose, coef, terms)
+        assert np.abs(Y - (S.T if transpose else S) @ X).max() <= 1e-13
+
+
+@pytest.mark.parametrize('transpose', [False, True])
+@pytest.mark.parametrize('mode,coef,terms', [(0, 0.05, 4), (1, None, None), (2, None, None), (3, None, None),
+                                             (4, None, None), (5, 0.5, 7)])
+def test_operator_abs_bounds_operator(mode, coef, terms, transpose):
+    """A >= 0 and X >= 0: operator_abs is operator_apply (mode 2, whose S is signed: it bounds it).  Signed: it bounds
+    |operator_apply| entry by entry."""
+    A = po.random_digraph(n=80, seed=4, p=0.08)
+    if mode == 1:
+        A = (A + A.T).tocsr()
+    if mode in (2, 5):
+        A = po.transition(A)
+    rng = np.random.default_rng(3)
+    Xp = rng.random((A.shape[0], 5))
+    Y, B = (f(A, mode, Xp, transpose, coef, terms) for f in (po.operator_apply, po.operator_abs))
+    if mode == 2:
+        assert np.all(np.abs(Y) <= B * (1 + 1e-14)) and not np.allclose(np.abs(Y), B)
+    else:
+        assert np.abs(Y - B).max() <= 1e-14 * np.abs(B).max()
+    Xs = rng.standard_normal((A.shape[0], 5))
+    Y, B = (f(A, mode, Xs, transpose, coef, terms) for f in (po.operator_apply, po.operator_abs))
+    assert np.all(np.abs(Y) <= B * (1 + 1e-14))
+
+
+def test_operator_apply_empty_graph():
+    """No edges: S = 0 (modes 0, 1, 3, 4), -I (mode 2), (1 - alpha) I (mode 5)."""
+    A = sp.csr_matrix((50, 50))
+    X = np.random.default_rng(4).standard_normal((50, 4))
+    for mode in (0, 1, 3, 4):
+        assert not np.any(po.operator_apply(A, mode, X, coef=0.1, terms=3))
+    assert np.array_equal(po.operator_apply(A, 2, X), -X)
+    assert np.array_equal(po.operator_apply(A, 5, X, coef=0.25, terms=5), 0.75 * X)
+    assert not np.any(po.inv_degree(A))
