@@ -195,22 +195,26 @@ struct gemb_graph {
 namespace gemb {
 
 // ---- spmm.cu
-// Y[n_rows x b] = X0 + alpha * A * X ; X has leading dimension ldx (>= b), rows indexed by the
-// global column ids in A.  X0/Y are row shards (ld = b).  All device pointers.
-int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha,
-                const float *X, const float *X0, float *Y);
-// Y = alpha * A * X + gamma * Xself + delta * X0   (Xself / X0: row shards, may be null)
-int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
-                 float gamma, const float *Xself, float delta, const float *X0, float *Y,
-                 const HaloPushArgs *push = nullptr);
-// the same with a fourth epilogue operand: Y = alpha * A * X + gamma * Xself + delta * X0 + eps * X1 (single GPU, no
-// push; X1 needs Xself and X0).  The composite operator's Chebyshev step (hope.cu, spectral_mode 2) takes four rows.
-int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
-                 float gamma, const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y);
-// Y = alpha * diag(rscale) * A * X: every row's sum scaled by its entry of rscale (n_rows floats, device; single GPU, no
-// other epilogue operand).  Sweep 1 of the Adamic-Adar operator A D A (hope.cu, spectral_mode 4).
-int spmm_scaled_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
-                       const float *rscale, float *Y);
+// The fused epilogue of one sweep:  Y = alpha * diag(rscale) * A * X + gamma * Xself + delta * X0 + eps * X1, and with
+// `push` each finished row of Y is also stored into the peers' halo slots (halo.cu).  A null pointer leaves its term out;
+// the defaults give the plain sweep Y = A X.  Xself, X0, X1: row shards; rscale: one float per row.  The instantiated
+// operand sets: any of {Xself, X0}, with or without push; X1 with Xself and X0 (the Chebyshev step on the composite
+// operator, hope.cu); rscale alone (the first sweep of Adamic-Adar, hope.cu).  Callers name the fields they set.
+struct SpmmEpilogue {
+    float alpha = 1.f;
+    float gamma = 0.f;
+    const float *Xself = nullptr;
+    float delta = 1.f;
+    const float *X0 = nullptr;
+    float eps = 0.f;
+    const float *X1 = nullptr;
+    const float *rscale = nullptr;
+    const HaloPushArgs *push = nullptr;
+};
+// Y[n_rows x b] = the epilogue over A X; X's rows are indexed by the global column ids in A.  All device pointers.
+// GEMB_ERR_ARG for an operand set that is not instantiated.
+int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, const float *X, float *Y,
+                const SpmmEpilogue &e);
 
 // ---- halo.cu (multi-GPU)
 int halo_build(gemb_graph *g);                                   // collective; idempotent
@@ -220,8 +224,7 @@ int halo_barrier(gemb_graph *g);                                 // all ranks' p
 void halo_push_args(const gemb_graph *g, int buf_index, HaloPushArgs *out);
 int halo_free(gemb_graph *g);
 void halo_pool_release(gemb_ctx *c);                              // at context destruction (not collective)
-// Y = a P + c Q over the local rows of halo blocks, pushing Y's rows to the peers (Chebyshev first step)
-int halo_check_timeout(gemb_graph *g);
+int halo_check_timeout(gemb_graph *g);                           // GEMB_ERR_NCCL when a barrier wait gave up
 
 // ---- dense.cu
 // G[b1 x b2] (fp64, row-major, OVERWRITTEN) = P^T Q over n rows (P: n x b1, Q: n x b2, fp32).

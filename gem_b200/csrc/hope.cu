@@ -42,6 +42,18 @@
 
 namespace gemb {
 
+// opts.spectral_mode, converted once by hope_options.  katz: top-k singular triplets of the Katz operator (HOPE); eigen:
+// the d largest ALGEBRAIC eigenpairs of the uploaded symmetric matrix itself (Laplacian Eigenmaps: D^-1/2 A D^-1/2,
+// lap.py:26-32); composite: those of -M^T M, M = I - A (LLE: A = D^-1 W, uploaded with A^T); common_neighbours,
+// adamic_adar, rooted_pagerank: HOPE on those proximities (apply_S)
+enum class Mode { katz, eigen, composite, common_neighbours, adamic_adar, rooted_pagerank };
+// the output is d eigenpairs (k = d, d may be odd), not d/2 singular triplets
+static bool eigen_output(Mode m) { return m == Mode::eigen || m == Mode::composite; }
+// S is not a function of a symmetric A: the general solver only (single GPU)
+static bool general_only(Mode m) {
+    return m == Mode::common_neighbours || m == Mode::adamic_adar || m == Mode::rooted_pagerank;
+}
+
 struct HopeWork {
     gemb_graph *g;
     gemb_ctx *c;
@@ -56,9 +68,9 @@ struct HopeWork {
     DeviceBuffer<int> rank_dev;
     CallEvents<2> fork_join;    // c->stream -> c->side and back (ritz_eigh)
     int64_t spmm_wide = 0, spmm_all = 0;
-    int mode = 0;               // opts.spectral_mode
-    DeviceBuffer<float> opT;    // spectral_mode 2: T = X - A X between the two sweeps of one application (n x b)
-    DeviceBuffer<float> rscale; // spectral_mode 4: D_ii = 1 / (rowsum(A) + rowsum(A^T)), 0 for isolated rows (n floats)
+    Mode mode = Mode::katz;
+    DeviceBuffer<float> opT;    // composite: T = X - A X between the two sweeps of one application (n x b)
+    DeviceBuffer<float> rscale; // adamic_adar: D_ii = 1 / (rowsum(A) + rowsum(A^T)), 0 for isolated rows (n floats)
     bool halo = false;       // multi-GPU: needed-rows-only exchange over peer memory (halo.cu); buf[] = g->halo.buf[]
     int64_t pushes = 0;      // blocks whose rows were pushed to the peers
     double push_bytes_per_row = 0.0;   // sum over the pushed blocks of (bytes per pushed row): NVLink bytes out = this * push_rows
@@ -153,57 +165,49 @@ static int publish(HopeWork &W, const float *buf, int width) {
     return end_push(W, width, bi);
 }
 
-// Y(shard) = alpha * op(A) * X + gamma * X(shard) + delta * X0(shard).  Sharded: halo mode gathers from the block's own
+// Y(shard) = the epilogue e over op(A) X (e.Xself, e.X0: row shards).  Sharded: halo mode gathers from the block's own
 // [local | halo] rows and (push_out) stores Y's rows into the peers' halo slots from the epilogue; otherwise X is
-// all-gathered first.
-static int dist_spmm3(HopeWork &W, bool transpose, int width, float alpha, const float *Xshard, float gamma,
-                      bool use_self, float delta, const float *X0, float *Y, bool timed, bool push_out = false) {
+// all-gathered first.  timed: a block-width sweep (t_spmm, spmm_wide).
+static int dist_spmm(HopeWork &W, bool transpose, int width, const float *Xshard, SpmmEpilogue e, float *Y, bool timed,
+                     bool push_out = false) {
+    gemb_csr_dev A = transpose && !W.halo ? W.g->AT : W.g->A;   // halo mode: a symmetric shard
+    const float *X = Xshard;
+    HaloPushArgs P;
     if (W.halo) {
-        gemb_csr_dev A = W.g->A;
         A.indices = W.g->halo.indices_ext;
-        HaloPushArgs P;
         const int bo = W.buf_index(Y), bin = W.buf_index(Xshard);
         GEMB_ARG(bin >= 0, "spmm input is not a work block");
-        if (push_out) { GEMB_ARG(bo >= 0, "spmm output is not a work block"); halo_push_args(W.g, bo, &P); }
-        if (timed) GEMB_TRY(W.c->t_spmm.begin(W.c->stream));
-        GEMB_TRY(spmm3_launch(W.c, A, W.rows, width, alpha, Xshard, gamma, use_self ? Xshard : nullptr, delta, X0, Y,
-                              push_out ? &P : nullptr));
-        if (timed) { GEMB_TRY(W.c->t_spmm.end(W.c->stream)); W.spmm_wide++; }
-        W.spmm_all++;
-        if (push_out) return end_push(W, width);
-        return GEMB_OK;
-    }
-    const float *Xfull = Xshard;
-    if (W.c->nranks > 1) {
+        if (push_out) {
+            GEMB_ARG(bo >= 0, "spmm output is not a work block");
+            halo_push_args(W.g, bo, &P);
+            e.push = &P;
+        }
+    } else if (W.c->nranks > 1) {
         GEMB_TRY(comm_allgather(W, Xshard, width));
-        Xfull = W.full.get();
+        X = W.full.get();
     }
     if (timed) GEMB_TRY(W.c->t_spmm.begin(W.c->stream));
-    GEMB_TRY(spmm3_launch(W.c, transpose ? W.g->AT : W.g->A, W.rows, width, alpha, Xfull, gamma,
-                          use_self ? Xshard : nullptr, delta, X0, Y));
+    GEMB_TRY(spmm_launch(W.c, A, W.rows, width, X, Y, e));
     if (timed) { GEMB_TRY(W.c->t_spmm.end(W.c->stream)); W.spmm_wide++; }
     W.spmm_all++;
+    if (e.push) return end_push(W, width);
     return GEMB_OK;
 }
 
-static int dist_spmm(HopeWork &W, bool transpose, int width, float alpha, const float *Xshard,
-                     const float *X0, float *Y, bool timed) {
-    return dist_spmm3(W, transpose, width, alpha, Xshard, 0.f, false, 1.f, X0, Y, timed);
-}
-
-// One application of the symmetric solver's operator Op:  Y = alpha * Op X + gamma * X (use_self) + delta * X0.
-// spectral_modes 0 and 1: Op = A, one sweep (dist_spmm3 as it stands).  spectral_mode 2 (single GPU): the composite
-// Op = -M^T M with M = I - A, uploaded as A and A^T and never formed -- sweep 1 T = X - A X, sweep 2
-// Y = alpha A^T T - alpha T + gamma X + delta X0, whose epilogue takes four rows (spmm4_launch).  One application
-// counts as two sweeps.
-static int op_apply(HopeWork &W, int width, float alpha, const float *X, float gamma, bool use_self, float delta,
-                    const float *X0, float *Y, bool timed, bool push_out = false) {
-    if (W.mode != 2) return dist_spmm3(W, false, width, alpha, X, gamma, use_self, delta, X0, Y, timed, push_out);
+// One application of the symmetric solver's operator Op:  Y = the epilogue e over Op X (e.Xself: X or null).  Modes
+// katz and eigen: Op = A, one sweep (dist_spmm).  composite (single GPU): Op = -M^T M with M = I - A, uploaded as A and
+// A^T and never formed -- sweep 1 T = X - A X, sweep 2 Y = alpha A^T T - alpha T + gamma X + delta X0, whose epilogue
+// takes e's operands one slot later.  One application counts as two sweeps.
+static int op_apply(HopeWork &W, int width, const float *X, const SpmmEpilogue &e, float *Y, bool timed,
+                    bool push_out = false) {
+    if (W.mode != Mode::composite) return dist_spmm(W, false, width, X, e, Y, timed, push_out);
     gemb_ctx *c = W.c;
     float *T = W.opT.get();
     if (timed) GEMB_TRY(c->t_spmm.begin(c->stream));
-    GEMB_TRY(spmm3_launch(c, W.g->A, W.rows, width, -1.f, X, 1.f, X, 0.f, nullptr, T));
-    GEMB_TRY(spmm4_launch(c, W.g->AT, W.rows, width, alpha, T, -alpha, T, gamma, use_self ? X : nullptr, delta, X0, Y));
+    GEMB_TRY(spmm_launch(c, W.g->A, W.rows, width, X, T, {.alpha = -1.f, .gamma = 1.f, .Xself = X, .delta = 0.f}));
+    GEMB_TRY(spmm_launch(c, W.g->AT, W.rows, width, T, Y,
+                         {.alpha = e.alpha, .gamma = -e.alpha, .Xself = T, .delta = e.gamma, .X0 = e.Xself,
+                          .eps = e.delta, .X1 = e.X0}));
     if (timed) { GEMB_TRY(c->t_spmm.end(c->stream)); W.spmm_wide += 2; }
     W.spmm_all += 2;
     return GEMB_OK;
@@ -219,13 +223,14 @@ static int katz(HopeWork &W, bool transpose, float beta, int J, const float *in,
     for (int m = 1; m <= J; m++) {
         if (m < J) {
             float *dst = (m & 1) ? t1 : t2;   // halo mode: `in` was published by the caller, dst feeds the next sweep
-            GEMB_TRY(dist_spmm3(W, transpose, W.b, beta, cur, 0.f, false, 1.f, in, dst, true, W.halo));
+            GEMB_TRY(dist_spmm(W, transpose, W.b, cur, {.alpha = beta, .X0 = in}, dst, true, W.halo));
             cur = dst;
-        } else if (W.mode == 5) {
+        } else if (W.mode == Mode::rooted_pagerank) {
             const double a = beta;
-            GEMB_TRY(dist_spmm3(W, transpose, W.b, (float)(a * (1.0 - a)), cur, 0.f, false, (float)(1.0 - a), in, out, true));
+            GEMB_TRY(dist_spmm(W, transpose, W.b, cur,
+                               {.alpha = (float)(a * (1.0 - a)), .delta = (float)(1.0 - a), .X0 = in}, out, true));
         } else {
-            GEMB_TRY(dist_spmm(W, transpose, W.b, beta, cur, nullptr, out, true));
+            GEMB_TRY(dist_spmm(W, transpose, W.b, cur, {.alpha = beta}, out, true));
         }
     }
     return GEMB_OK;
@@ -236,13 +241,13 @@ static int katz(HopeWork &W, bool transpose, float beta, int J, const float *in,
 // 3; the scale is applied in sweep 1's epilogue), then out = op(A) t1 -- S^T = A^T D A^T takes A^T in both.  Single GPU
 // for modes 3 and 4; one application counts as two sweeps.
 static int apply_S(HopeWork &W, bool transpose, float beta, int J, const float *in, float *out, float *t1, float *t2) {
-    if (W.mode != 3 && W.mode != 4) return katz(W, transpose, beta, J, in, out, t1, t2);
+    if (W.mode != Mode::common_neighbours && W.mode != Mode::adamic_adar)
+        return katz(W, transpose, beta, J, in, out, t1, t2);
     gemb_ctx *c = W.c;
     const gemb_csr_dev &Op = transpose ? W.g->AT : W.g->A;
     GEMB_TRY(c->t_spmm.begin(c->stream));
-    if (W.mode == 4) GEMB_TRY(spmm_scaled_launch(c, Op, W.rows, W.b, 1.f, in, W.rscale.get(), t1));
-    else GEMB_TRY(spmm_launch(c, Op, W.rows, W.b, 1.f, in, nullptr, t1));
-    GEMB_TRY(spmm_launch(c, Op, W.rows, W.b, 1.f, t1, nullptr, out));
+    GEMB_TRY(spmm_launch(c, Op, W.rows, W.b, in, t1, {.rscale = W.mode == Mode::adamic_adar ? W.rscale.get() : nullptr}));
+    GEMB_TRY(spmm_launch(c, Op, W.rows, W.b, t1, out, {}));
     GEMB_TRY(c->t_spmm.end(c->stream));
     W.spmm_wide += 2;
     W.spmm_all += 2;
@@ -460,8 +465,8 @@ static int estimate_norm2(HopeWork &W, uint64_t seed, float *x, float *y, float 
         double h[2];
         GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal.get()));
         GEMB_TRY(publish(W, x, pw));
-        GEMB_TRY(dist_spmm3(W, false, pw, 1.f, x, 0.f, false, 1.f, nullptr, y, false, true));
-        GEMB_TRY(dist_spmm(W, true, pw, 1.f, y, nullptr, z, false));
+        GEMB_TRY(dist_spmm(W, false, pw, x, {}, y, false, true));
+        GEMB_TRY(dist_spmm(W, true, pw, y, {}, z, false));
         GEMB_TRY(sumsq_launch(c, W.rows * pw, z, W.scal.get() + 1));
         GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 2));
         GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
@@ -486,7 +491,7 @@ static int estimate_composite_norm(HopeWork &W, uint64_t seed, float *x, float *
     for (int it = 0; it < 32; it++) {
         double h[2];
         GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal.get()));
-        GEMB_TRY(op_apply(W, pw, 1.f, x, 0.f, false, 1.f, nullptr, y, false));
+        GEMB_TRY(op_apply(W, pw, x, {}, y, false));
         GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get() + 1));
         GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
         if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }   // M^T M x = 0 (M = 0: P = I)
@@ -517,7 +522,7 @@ static int probe_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t s
         bool done = false;
         for (j = 1; j <= Jmax; j++) {
             double h = 0.0;
-            GEMB_TRY(dist_spmm(W, tr == 1, pw, beta, x, nullptr, y, false));
+            GEMB_TRY(dist_spmm(W, tr == 1, pw, x, {.alpha = beta}, y, false));
             GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get()));
             GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 1));
             GEMB_TRY(copy_sync(c, &h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
@@ -539,10 +544,7 @@ static int probe_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t s
 struct Opts {
     int oversample = 16, max_iters = 30, min_iters = 2, katz_terms = 0, compute_residual = 0, verbose = 0;
     int algorithm = 0, cheb_degree = 8, stop_rule = 0, lanczos_basis = 0;
-    int spectral_mode = 0;   // 0: top-k singular triplets of the Katz operator (HOPE); 1: the d largest ALGEBRAIC eigenpairs of the
-                             // uploaded symmetric matrix itself (Laplacian Eigenmaps: D^-1/2 A D^-1/2, lap.py:26-32);
-                             // 2: those of the composite -M^T M, M = I - A (LLE: A = D^-1 W, uploaded with A^T);
-                             // 3, 4, 5: HOPE on the common-neighbour, Adamic-Adar and rooted-PageRank proximities (apply_S)
+    Mode mode = Mode::katz;
     float tol = 1e-6f, katz_tol = 1e-7f, range_log2 = 8.f;
     uint64_t seed = 1234;
 };
@@ -885,10 +887,10 @@ static int diverge_error(const SpecMap &map) {
 // ritz_bound: A is symmetric with non-negative weights and map.norm = ||A||_inf; then lambda_max = rho(A) >= |lambda_min|
 // (Perron-Frobenius), so 1.05 * (largest Ritz value) bounds the spectrum on both sides and the 2 x 16 narrow SpMM sweeps
 // of the power iteration are not needed.  Otherwise map.norm is a tight estimate of ||A||_2 (power iteration).
-static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool ritz_bound, HopeResult &R) {
+static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map, bool ritz_bound, HopeResult &R) {
     gemb_ctx *c = W.c;
-    const int mode = o.spectral_mode;
-    const int b = W.b, k = mode ? d : d / 2;
+    const bool eigen = eigen_output(o.mode);
+    const int b = W.b;
     R.algorithm = 2;
     R.katz_terms = 0;
     float *V = W.buf[0], *AV = W.buf[1];
@@ -900,13 +902,14 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     // the first Cholesky drop columns (skewed spectrum, rank-deficient A), the careful form below takes over.
     // spectral_mode 2: the wanted end of -M^T M is 0, its smallest |l|, which a power step would damp: the warm-up
     // steps run on the shifted -M^T M + bound I instead, whose wanted end is its largest value.
-    const bool shift = mode == 2;
-    const float nu = shift ? (float)map.bound : 0.f;
+    const bool composite = o.mode == Mode::composite;
+    const float nu = composite ? (float)map.bound : 0.f;
+    auto power = [&](const float *x) { return SpmmEpilogue{.gamma = nu, .Xself = composite ? x : nullptr}; };
     GEMB_TRY(randn_launch(c, W.rows, b, o.seed, (uint64_t)W.g->row0, pool[0]));
     GEMB_TRY(publish(W, pool[0], b));
-    GEMB_TRY(op_apply(W, b, 1.f, pool[0], nu, shift, 1.f, nullptr, pool[1], true, W.halo));
-    GEMB_TRY(op_apply(W, b, 1.f, pool[1], nu, shift, 1.f, nullptr, pool[2], true, W.halo));
-    GEMB_TRY(op_apply(W, b, 1.f, pool[2], nu, shift, 1.f, nullptr, AV, true));
+    GEMB_TRY(op_apply(W, b, pool[0], power(pool[0]), pool[1], true, W.halo));
+    GEMB_TRY(op_apply(W, b, pool[1], power(pool[1]), pool[2], true, W.halo));
+    GEMB_TRY(op_apply(W, b, pool[2], power(pool[2]), AV, true));
     GEMB_TRY(gram_full(W, AV, AV, W.G.get()));
     GEMB_TRY(cholqr_pass(W, W.G.get(), AV, pool[0]));
     int rank1 = b;
@@ -920,7 +923,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         GEMB_TRY(cholqr2(W, pool[0], pool[1], V));
         GEMB_TRY(publish(W, V, b));
         for (int s = 0; s < 3; s++) {   // plain power steps V <- orth(A V)
-            GEMB_TRY(op_apply(W, b, 1.f, V, nu, shift, 1.f, nullptr, AV, true));
+            GEMB_TRY(op_apply(W, b, V, power(V), AV, true));
             GEMB_TRY(cholqr2(W, AV, pool[0], V));
             GEMB_TRY(publish(W, V, b));
         }
@@ -942,8 +945,10 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         for (int i = 2; i <= deg; i++) {
             const double sn = 1.0 / (tau2 - sigma);
             float *nxt = free_a;
-            GEMB_TRY(op_apply(W, b, (float)(2.0 * sn / e), cur, (float)(-2.0 * sn * c0 / e), true, (float)(-sigma * sn),
-                              prev, nxt, true, /*push_out=*/i < deg));
+            GEMB_TRY(op_apply(W, b, cur,
+                              {.alpha = (float)(2.0 * sn / e), .gamma = (float)(-2.0 * sn * c0 / e), .Xself = cur,
+                               .delta = (float)(-sigma * sn), .X0 = prev},
+                              nxt, true, /*push_out=*/i < deg));
             sigma = sn;
             // rotate: the old `prev` becomes free unless it is V (V must survive until the new basis exists)
             float *old_prev = prev;
@@ -959,7 +964,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     for (int it = 1; it <= o.max_iters; it++) {
         R.iters = it;
         // Rayleigh-Ritz on A: T = V^T A V, (l, Z) = eigh(T)
-        GEMB_TRY(op_apply(W, b, 1.f, V, 0.f, false, 1.f, nullptr, AV, true));
+        GEMB_TRY(op_apply(W, b, V, {}, AV, true));
         GEMB_TRY(gram_full(W, V, AV, W.G2.get()));
         // (Measured: running the single-CTA Jacobi on a side stream while the filter starts with the PREVIOUS
         // round's interval costs two extra rounds -- 75 instead of 56 SpMM sweeps -- and is slower overall;
@@ -973,16 +978,16 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         std::sort(order.begin(), order.end(), [&](int a, int c2) { return gval[a] > gval[c2]; });   // descending key
         for (int i = 0; i < b; i++) th_sorted[i] = gval[order[i]] * gval[order[i]];
         const double tmax = std::max(th_sorted[0], 1e-300);
-        // vmax: max |value| over the wanted pairs (Katz: sigma_max = gval[order[0]]).  spectral_mode 2: the operator
+        // vmax: max |value| over the wanted pairs (Katz: sigma_max = gval[order[0]]).  composite: the operator
         // bound ||M||_2^2 -- the wanted eigenvalues -sigma^2 lie near 0, and both stop measures are taken relative to
         // the operator, as the explicit form's are relative to its shift c >= ||M||_2^2
         double vmax = 0.0;
-        if (mode == 2) vmax = map.norm;
+        if (composite) vmax = map.norm;
         else for (int j = 0; j < k; j++) vmax = std::max(vmax, fabs(map.value(lam[order[j]])));
         double change;
-        if (mode) {
+        if (eigen) {
             for (int i = 0; i < b; i++) vals[i] = map.value(lam[order[i]]);
-            if (mode == 2) {        // round 1 has nothing to compare with (vals_prev = 0 would read as a tiny change)
+            if (composite) {    // round 1 has nothing to compare with (vals_prev = 0 would read as a tiny change)
                 change = it == 1 ? HUGE_VAL : 0.0;
                 for (int j = 0; j < k && it > 1; j++) change = std::max(change, fabs(vals[j] - vals_prev[j]) / std::max(vmax, 1e-300));
             } else change = value_change(vals.data(), vals_prev.data(), k, vmax);
@@ -993,8 +998,8 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         // algorithm = 0 (auto): a first Rayleigh-Ritz round whose wanted values already span more than 3x -- a
         // power-law spectrum -- is a case for restarted Lanczos: a filter that damps everything below the k-th value
         // spreads the wanted columns over g^m and degenerates to power steps (DESIGN section 5)
-        if (it == 1 && !mode && o.algorithm == 0 && W.g->n >= 2048 && gval[order[k - 1]] < 0.33 * gval[order[0]] &&
-            gval[order[std::min(b - 1, 3)]] < 0.7 * gval[order[0]])
+        if (it == 1 && o.mode == Mode::katz && o.algorithm == 0 && W.g->n >= 2048 &&
+            gval[order[k - 1]] < 0.33 * gval[order[0]] && gval[order[std::min(b - 1, 3)]] < 0.7 * gval[order[0]])
             return GEMB_SWITCH_TO_LANCZOS;
         double stop_measure = change;
         if (o.stop_rule == 1) {
@@ -1032,7 +1037,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         if (growth > 1.0 + 1e-9) deg = std::min(deg, (int)floor(log(2.0 * exp2((double)o.range_log2)) / log(growth)));
 
         if (deg < 2) {                                          // A V is already there: one power step
-            if (shift) {                                        // on -M^T M + bound I, as in the warm-up
+            if (composite) {                                    // on -M^T M + bound I, as in the warm-up
                 GEMB_TRY(axpby_launch(W, 1.f, AV, nu, V, pool[1]));
                 GEMB_TRY(orth_rotated(W, pool[1], pool[0], V));
             } else GEMB_TRY(orth_rotated(W, AV, pool[0], V));
@@ -1057,7 +1062,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     std::vector<double> Zh((size_t)b * b);
     GEMB_TRY(copy_sync(c, Zh.data(), W.Z.get(), sizeof(double) * b * b, cudaMemcpyDeviceToHost));
     // M = [M1 | M2] (b x d; LE / LLE: M1 alone, b x k): one apply writes whole rows of X
-    const int xw = mode ? k : 2 * k;
+    const int xw = eigen ? k : 2 * k;
     std::vector<float> M((size_t)b * xw), sig(k);
     std::vector<int> sel(k);
     for (int j = 0; j < k; j++) {
@@ -1068,7 +1073,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
         for (int i = 0; i < b; i++) {
             const double z = Zh[(size_t)i * b + col];
             M[(size_t)i * xw + q] = (float)((t.neg ? -z : z) * t.scale);
-            if (!mode) M[(size_t)i * xw + k + q] = (float)(z * t.scale);
+            if (!eigen) M[(size_t)i * xw + k + q] = (float)(z * t.scale);
         }
     }
     R.sigma_max = gval[order[0]];
@@ -1078,7 +1083,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, SpecMap map, bool r
     GEMB_TRY(c->t_dense.begin(c->stream));
     GEMB_TRY(apply_launch(c, W.rows, V, b, W.M1.get(), xw, xw, R.Xd, d));
     GEMB_TRY(c->t_dense.end(c->stream));
-    if (mode || !o.compute_residual) return GEMB_OK;
+    if (eigen || !o.compute_residual) return GEMB_OK;
 
     // check the triplets against the Katz operator itself: || S^T u - sigma v || / sigma_max
     const int J = katz_terms_for(map.beta, ritz_bound ? map.bound / 1.02 : map.norm, o.katz_tol);
@@ -1237,7 +1242,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
         m += p;
         steps++;
         GEMB_TRY(publish(W, Vcur, p));
-        GEMB_TRY(dist_spmm3(W, false, p, 1.f, Vcur, 0.f, false, 1.f, nullptr, Wb, true, false));
+        GEMB_TRY(dist_spmm(W, false, p, Vcur, {}, Wb, true));
         std::fill(Hcol.begin(), Hcol.end(), 0.0);
         const int nc_live = (m + cw - 1) / cw;
         for (int pass = 0; pass < 2; pass++) {
@@ -1458,13 +1463,6 @@ namespace gemb {
 static int hope_options(gemb_graph *g, float *beta, const gemb_hope_opts *uo, Opts *po) {
     gemb_ctx *c = g->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
-    GEMB_ARG(!(uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode == 2) || c->nranks == 1,
-             "spectral_mode 2 (the composite operator -M^T M) is single-GPU: use a context without a multi-GPU communicator");
-    GEMB_ARG(!(uo && uo->struct_size == sizeof(gemb_hope_opts) && uo->spectral_mode >= 3 && uo->spectral_mode <= 5) ||
-                 c->nranks == 1,
-             "spectral_modes 3-5 (common neighbours, Adamic-Adar, rooted PageRank) are single-GPU: use a context without a "
-             "multi-GPU communicator");
-    GEMB_ARG(!(c->nranks > 1 && g->replicated), "multi-GPU HOPE needs row shards (upload rows [rank*ceil(n/P), ...))");
     Opts o;
     if (uo) {
         GEMB_ARG(uo->struct_size == sizeof(gemb_hope_opts), "opts.struct_size");
@@ -1485,15 +1483,21 @@ static int hope_options(gemb_graph *g, float *beta, const gemb_hope_opts *uo, Op
         o.stop_rule = uo->stop_rule;
         if (uo->algorithm3_basis > 0) o.lanczos_basis = uo->algorithm3_basis;
         GEMB_ARG(uo->spectral_mode >= 0 && uo->spectral_mode <= 5, "opts.spectral_mode");
-        o.spectral_mode = uo->spectral_mode;
+        o.mode = (Mode)uo->spectral_mode;
     }
-    if (o.spectral_mode == 1) {
+    GEMB_ARG(o.mode != Mode::composite || c->nranks == 1,
+             "spectral_mode 2 (the composite operator -M^T M) is single-GPU: use a context without a multi-GPU communicator");
+    GEMB_ARG(!general_only(o.mode) || c->nranks == 1,
+             "spectral_modes 3-5 (common neighbours, Adamic-Adar, rooted PageRank) are single-GPU: use a context without a "
+             "multi-GPU communicator");
+    GEMB_ARG(!(c->nranks > 1 && g->replicated), "multi-GPU HOPE needs row shards (upload rows [rank*ceil(n/P), ...))");
+    if (o.mode == Mode::eigen) {
         GEMB_ARG(g->symmetric, "spectral_mode 1 (largest algebraic eigenpairs) needs a symmetric upload");
         GEMB_ARG(o.algorithm == 0 || o.algorithm == 2, "spectral_mode 1 runs on the Chebyshev-filtered subspace iteration (algorithm 0 or 2)");
         o.algorithm = 2;
         *beta = 0.f;                // unused: the ranking is by the eigenvalue itself
     }
-    if (o.spectral_mode == 2) {
+    if (o.mode == Mode::composite) {
         // The wanted end of -M^T M (sigma^2 ~ 1e-2) is a sliver of a spectrum ||M||_2^2 wide (1246 on R-MAT 20's largest
         // component): per degree the filter gains ~1 + (m a)^2 / 2 at low degree m, exponentially only at high degree.
         // Degree 8 there stopped on the change rule with sigma^2 20x too large; degree 64 reaches an fp64 residual of
@@ -1505,14 +1509,14 @@ static int hope_options(gemb_graph *g, float *beta, const gemb_hope_opts *uo, Op
         o.algorithm = 2;
         *beta = 0.f;
     }
-    if (o.spectral_mode >= 3) {
+    if (general_only(o.mode)) {
         GEMB_ARG(o.algorithm <= 1, "spectral_modes 3-5 run on the general solver (algorithm 0 or 1): S is not a function "
                                    "of a symmetric A");
         o.algorithm = 1;
-        if (o.spectral_mode == 5) GEMB_ARG(*beta > 0.f && *beta < 1.f, "spectral_mode 5 takes alpha in beta: 0 < alpha < 1");
+        if (o.mode == Mode::rooted_pagerank) GEMB_ARG(*beta > 0.f && *beta < 1.f, "spectral_mode 5 takes alpha in beta: 0 < alpha < 1");
         else *beta = 0.f;           // unused: S = A A or A D A has no coefficient
     }
-    if (o.algorithm >= 2 && !g->symmetric && o.spectral_mode != 2) {
+    if (o.algorithm >= 2 && !g->symmetric && o.mode != Mode::composite) {
         set_error("algorithm=%d (works on A itself, S = f(A)) needs a symmetric shard (upload with indptr_t = NULL)", o.algorithm);
         return GEMB_ERR_ARG;
     }
@@ -1528,16 +1532,17 @@ static int hope_options(gemb_graph *g, float *beta, const gemb_hope_opts *uo, Op
 static int proximity_setup(HopeWork &W, const Opts &o, float beta, int *J) {
     bool nonneg = true;
     double pinf = 0.0;
-    if (W.mode >= 4) {
+    if (W.mode != Mode::common_neighbours) {
         GEMB_TRY(rowsum_bound(W, &pinf, &nonneg));
         GEMB_ARG(nonneg, "spectral_modes 4 and 5 (Adamic-Adar, rooted PageRank) need non-negative weights");
     }
-    if (W.mode == 4) GEMB_TRY(inv_degree(W));
-    if (W.mode != 5) *J = 0;    // no series: katz_terms is ignored and reported as 0
-    if (W.mode == 5) {
-        GEMB_ARG(pinf <= 1.0 + 1e-5, "spectral_mode 5 needs P = D_out^-1 A (every row sum <= 1)");
-        if (*J <= 0) *J = std::max(1, std::min(4096, (int)ceil(log((double)o.katz_tol) / log((double)beta))));
+    if (W.mode == Mode::adamic_adar) GEMB_TRY(inv_degree(W));
+    if (W.mode != Mode::rooted_pagerank) {
+        *J = 0;                 // no series: katz_terms is ignored and reported as 0
+        return GEMB_OK;
     }
+    GEMB_ARG(pinf <= 1.0 + 1e-5, "spectral_mode 5 needs P = D_out^-1 A (every row sum <= 1)");
+    if (*J <= 0) *J = std::max(1, std::min(4096, (int)ceil(log((double)o.katz_tol) / log((double)beta))));
     return GEMB_OK;
 }
 
@@ -1547,14 +1552,13 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
                          float *sigma_out, gemb_hope_stats *stats) {
     GEMB_ARG(g != nullptr, "graph");
     GEMB_ARG(d >= 1, "d must be >= 1");
-    GEMB_ARG((uo && uo->struct_size == sizeof(gemb_hope_opts) && (uo->spectral_mode == 1 || uo->spectral_mode == 2)) || d % 2 == 0,
-             "d must be even (k = d/2 singular triplets)");
     GEMB_ARG(!stats || stats->struct_size == sizeof(gemb_hope_stats), "stats.struct_size");
     gemb_ctx *c = g->ctx;
     Opts o;
     GEMB_TRY(hope_options(g, &beta, uo, &o));
+    GEMB_ARG(eigen_output(o.mode) || d % 2 == 0, "d must be even (k = d/2 singular triplets)");
     const int algo = o.algorithm ? o.algorithm : (g->symmetric ? 2 : 1);
-    const int k = (o.spectral_mode == 1 || o.spectral_mode == 2) ? d : d / 2;
+    const int k = eigen_output(o.mode) ? d : d / 2;
     GEMB_ARG((int64_t)k <= g->n, "d/2 must not exceed the number of nodes");
     int64_t bb = std::min<int64_t>(g->n, (int64_t)k + o.oversample);
     int b = (int)((bb + 3) / 4 * 4);
@@ -1565,7 +1569,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     const double t_enter = now();
     HopeWork W;
     W.g = g; W.c = c; W.b = b; W.rows = g->n_local; W.shard = g->n_shard;
-    W.mode = o.spectral_mode;
+    W.mode = o.mode;
     // multi-GPU, symmetric shard: needed-rows-only exchange over peer memory (halo.cu) unless GEMB_MG=allgather or
     // CUDA IPC is not available on this box (then every rank falls back to the all-gather form together)
     static const bool mg_allgather = getenv("GEMB_MG") && !strcmp(getenv("GEMB_MG"), "allgather");
@@ -1602,7 +1606,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     GEMB_CUDA(W.M2.alloc(b * b));
     GEMB_CUDA(W.rank_dev.alloc(1));
     GEMB_CUDA(W.fork_join.create());
-    if (W.mode == 2) {                                     // the sixth n x b block: T between the two sweeps
+    if (W.mode == Mode::composite) {                       // the sixth n x b block: T between the two sweeps
         GEMB_CUDA(W.opT.alloc((size_t)W.shard * b));
         GEMB_CUDA(cudaMemsetAsync(W.opT.get(), 0, sizeof(float) * (size_t)W.shard * b, c->stream));
     }
@@ -1625,10 +1629,10 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         have_nrm = true;
         GEMB_TRY(clear_scratch(W));
     }
-    bool need_power = (J <= 0 && algo == 1) && !have_nrm && W.mode < 3;
-    if (W.mode >= 3) {
+    bool need_power = (J <= 0 && algo == 1) && !have_nrm && !general_only(W.mode);
+    if (general_only(W.mode)) {
         GEMB_TRY(proximity_setup(W, o, beta, &J));
-    } else if (W.mode == 2) {
+    } else if (W.mode == Mode::composite) {
         // the Perron-Frobenius shortcut (ritz_bound) does not apply to -M^T M: ||M||_2^2 by power iteration
         GEMB_TRY(estimate_composite_norm(W, o.seed, W.buf[3], W.buf[4], &nrm));
         if (!(nrm > 0.0)) nrm = 1.0;                       // M = 0: the spectrum is {0}, any positive bound holds it
@@ -1658,12 +1662,12 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     const bool lanczos_fits = g->n >= 2048;
     // a priori spectrum bound: ||A||_inf for Lanczos; for Chebyshev see hope_symmetric
     const SpecMap lanczos_map(beta, true, hard_bound);
-    SpecMap sym_map(beta, o.spectral_mode == 0, ritz_bound ? hard_bound : nrm);
+    SpecMap sym_map(beta, o.mode == Mode::katz, ritz_bound ? hard_bound : nrm);
     sym_map.estimated = !ritz_bound;                              // else ||A||_inf: a true bound
-    sym_map.negdef = o.spectral_mode == 2;
+    sym_map.negdef = o.mode == Mode::composite;
     if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, lanczos_map, R);
     else if (algo >= 2) {
-        s = hope_symmetric(W, o, d, sym_map, ritz_bound, R);
+        s = hope_symmetric(W, o, d, k, sym_map, ritz_bound, R);
         if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, lanczos_map, R); }
     } else s = hope_general(W, o, d, beta, J, R);
     if (s != GEMB_OK) return s;
@@ -1735,22 +1739,22 @@ extern "C" int gemb_hope_apply(gemb_graph *g, const gemb_hope_opts *uo, float be
     GEMB_ARG(c->nranks == 1 && g->n_local == g->n, "gemb_hope_apply is single-GPU");
     Opts o;
     GEMB_TRY(hope_options(g, &beta, uo, &o));
-    GEMB_ARG(o.spectral_mode != 0 || (o.katz_terms > 0 && beta >= 0.f),
+    GEMB_ARG(o.mode != Mode::katz || (o.katz_terms > 0 && beta >= 0.f),
              "spectral_mode 0 needs opts.katz_terms > 0 and beta >= 0 (no norm estimate is made)");
     const int64_t n = g->n;
     const size_t blk = (size_t)n * b;
     HopeWork W;
     W.g = g; W.c = c; W.b = b; W.rows = n; W.shard = n;
-    W.mode = o.spectral_mode;
+    W.mode = o.mode;
     GEMB_TRY(W.alloc_blocks(blk));
     GEMB_CUDA(W.scal.alloc(2));
-    if (W.mode == 2) GEMB_CUDA(W.opT.alloc(blk));
+    if (W.mode == Mode::composite) GEMB_CUDA(W.opT.alloc(blk));
     int J = o.katz_terms;
-    if (W.mode >= 3) GEMB_TRY(proximity_setup(W, o, beta, &J));
-    else if (W.mode != 0) J = 0;
+    if (general_only(W.mode)) GEMB_TRY(proximity_setup(W, o, beta, &J));
+    else if (W.mode != Mode::katz) J = 0;
     float *in = W.buf[0], *out = W.buf[1];
     GEMB_CUDA(cudaMemcpyAsync(in, X, sizeof(float) * blk, cudaMemcpyHostToDevice, c->stream));
-    if (W.mode == 1 || W.mode == 2) GEMB_TRY(op_apply(W, b, 1.f, in, 0.f, false, 1.f, nullptr, out, false));
+    if (eigen_output(W.mode)) GEMB_TRY(op_apply(W, b, in, {}, out, false));
     else GEMB_TRY(apply_S(W, transpose != 0, beta, J, in, out, W.buf[2], W.buf[3]));
     GEMB_TRY(copy_sync(c, Y, out, sizeof(float) * blk, cudaMemcpyDeviceToHost));
     if (J_out) *J_out = J;

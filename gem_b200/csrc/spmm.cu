@@ -1,4 +1,5 @@
-// gem_b200/csrc/spmm.cu -- CSR SpMM  Y = X0 + alpha * A * X  over an fp32 row-major block.
+// gem_b200/csrc/spmm.cu -- CSR SpMM  Y = alpha * A * X  over an fp32 row-major block, with a fused epilogue that adds up
+// to three more row blocks (SpmmEpilogue, common.cuh).
 //
 // Replaces the dense products hidden in hope.py:31 (inv(I - beta A) . beta A) and inside
 // scipy's svds matvecs (hope.py:33): S is never formed, every S.x is a Horner sweep of this kernel.
@@ -7,8 +8,8 @@
 // c of the group owns columns [4c, 4c+4) of the block, so one nonzero = one coalesced 16*G-byte
 // read of X[col, :] (320 B for b = 80) and the accumulators never leave registers.  Column ids and
 // values of a row tile are staged in shared memory (spmm_bulk_kernel below).  The nonzero loop is
-// unrolled by 4 so that each thread keeps 4 independent 16-byte gathers in flight.  The Horner
-// epilogue (X0 + alpha * acc) is fused: one extra coalesced read.
+// unrolled by 4 so that each thread keeps 4 independent 16-byte gathers in flight.  The epilogue
+// (the Horner step: X0 + alpha * acc) is fused: one extra coalesced read per operand.
 #include "common.cuh"
 #include <string.h>
 #include <algorithm>
@@ -16,15 +17,26 @@
 
 namespace gemb {
 
-int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, const float *X, float gamma,
-                      const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y,
-                      const HaloPushArgs *push, const float *rscale = nullptr);
-
 __device__ __forceinline__ void fma4(float4 &a, float v, const float4 &x) {
     a.x = fmaf(v, x.x, a.x);
     a.y = fmaf(v, x.y, a.y);
     a.z = fmaf(v, x.z, a.z);
     a.w = fmaf(v, x.w, a.w);
+}
+
+// The epilogue of one finished row chunk (SpmmEpilogue): a * acc with a = alpha (HAS_SCALE: alpha * rscale[row]), then
+// gamma * Xself, delta * X0 and eps * X1 added in this order by one fmaf each -- the order fixes the rounding.
+template <bool HAS_X0, bool HAS_SELF, bool HAS_X1, bool HAS_SCALE>
+__device__ __forceinline__ float4 spmm_epilogue(const float4 &acc, int64_t row, int G, int c, float alpha, float gamma,
+                                                float delta, float eps, const float4 *__restrict__ Xself,
+                                                const float4 *__restrict__ X0, const float4 *__restrict__ X1,
+                                                const float *__restrict__ rscale) {
+    const float a = HAS_SCALE ? alpha * __ldg(rscale + row) : alpha;
+    float4 r = make_float4(a * acc.x, a * acc.y, a * acc.z, a * acc.w);
+    if (HAS_SELF) fma4(r, gamma, __ldg(Xself + row * G + c));
+    if (HAS_X0) fma4(r, delta, __ldg(X0 + row * G + c));
+    if (HAS_X1) fma4(r, eps, __ldg(X1 + row * G + c));
+    return r;
 }
 
 // ---- heavy rows (degree > SPMM_HEAVY_DEG; the hubs of a power-law graph -- R-MAT scale 21 has a 61 814-neighbour
@@ -97,20 +109,8 @@ spmm_heavy_finish_kernel(int n_heavy, const int32_t *__restrict__ heavy_row, con
         const float4 t = partial[(size_t)it * G + c];
         acc.x += t.x; acc.y += t.y; acc.z += t.z; acc.w += t.w;
     }
-    const float a = HAS_SCALE ? alpha * __ldg(rscale + row) : alpha;
-    float4 r = make_float4(a * acc.x, a * acc.y, a * acc.z, a * acc.w);
-    if (HAS_SELF) {
-        const float4 z = __ldg(Xself + row * G + c);
-        r.x = fmaf(gamma, z.x, r.x); r.y = fmaf(gamma, z.y, r.y); r.z = fmaf(gamma, z.z, r.z); r.w = fmaf(gamma, z.w, r.w);
-    }
-    if (HAS_X0) {
-        const float4 z = __ldg(X0 + row * G + c);
-        r.x = fmaf(delta, z.x, r.x); r.y = fmaf(delta, z.y, r.y); r.z = fmaf(delta, z.z, r.z); r.w = fmaf(delta, z.w, r.w);
-    }
-    if (HAS_X1) {
-        const float4 z = __ldg(X1 + row * G + c);
-        r.x = fmaf(eps, z.x, r.x); r.y = fmaf(eps, z.y, r.y); r.z = fmaf(eps, z.z, r.z); r.w = fmaf(eps, z.w, r.w);
-    }
+    const float4 r =
+        spmm_epilogue<HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>(acc, row, G, c, alpha, gamma, delta, eps, Xself, X0, X1, rscale);
     Y[row * G + c] = r;
     if (has_push) halo_push_row(P, row, G, c, r);
 }
@@ -203,20 +203,8 @@ spmm_bulk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__
                 }
                 for (; i < e; i++) fma4(acc, HAS_VAL ? __ldg(vals + i) : 1.f, __ldg(X + (int64_t)__ldg(indices + i) * G + c));
             }
-            const float a = HAS_SCALE ? alpha * __ldg(rscale + row) : alpha;
-            float4 r = make_float4(a * acc.x, a * acc.y, a * acc.z, a * acc.w);
-            if (HAS_SELF) {
-                const float4 z = __ldg(Xself + row * G + c);
-                r.x = fmaf(gamma, z.x, r.x); r.y = fmaf(gamma, z.y, r.y); r.z = fmaf(gamma, z.z, r.z); r.w = fmaf(gamma, z.w, r.w);
-            }
-            if (HAS_X0) {
-                const float4 z = __ldg(X0 + row * G + c);
-                r.x = fmaf(delta, z.x, r.x); r.y = fmaf(delta, z.y, r.y); r.z = fmaf(delta, z.z, r.z); r.w = fmaf(delta, z.w, r.w);
-            }
-            if (HAS_X1) {
-                const float4 z = __ldg(X1 + row * G + c);
-                r.x = fmaf(eps, z.x, r.x); r.y = fmaf(eps, z.y, r.y); r.z = fmaf(eps, z.z, r.z); r.w = fmaf(eps, z.w, r.w);
-            }
+            const float4 r = spmm_epilogue<HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>(acc, row, G, c, alpha, gamma, delta, eps,
+                                                                                Xself, X0, X1, rscale);
             Y[row * G + c] = r;
             if (HAS_PUSH) halo_push_row(P, row, G, c, r);
         }
@@ -225,141 +213,99 @@ spmm_bulk_kernel(const int32_t *__restrict__ indptr, const int32_t *__restrict__
     }
 }
 
-int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha,
-                const float *X, const float *X0, float *Y) {
-    return spmm3_launch(ctx, A, n_rows, b, alpha, X, 0.f, nullptr, 1.f, X0, Y, nullptr);
-}
-
-int spmm3_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
-                 float gamma, const float *Xself, float delta, const float *X0, float *Y, const HaloPushArgs *push) {
-    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "block width must be a multiple of 4, <= 1024");
-    if (n_rows == 0) return GEMB_OK;
+// One sweep with the epilogue's operand set fixed at compile time: the bulk kernel over every row tile, then, when A has
+// heavy rows, their chunk sums (into ctx->spmm_scratch, grown on demand) and the finish kernel with the same epilogue.
+template <bool HAS_PUSH, bool HAS_X0, bool HAS_SELF, bool HAS_X1, bool HAS_SCALE>
+static int spmm_sweep(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, const float *X, float *Y,
+                      const SpmmEpilogue &e) {
     const int G = b / 4;
     const int rows_per_cta = 256 / G;
     const int tile_rows = rows_per_cta * SPMM_TILE_PASSES;
     const int64_t n_tiles = (n_rows + tile_rows - 1) / tile_rows;
     GEMB_ARG(n_tiles < (int64_t)2147483647, "grid too large");
     const bool heavy = A.n_items > 0;
-    const int hd = heavy ? SPMM_HEAVY_DEG : 0;
     HaloPushArgs PA;
     memset(&PA, 0, sizeof PA);
-    if (push) PA = *push;
-    const float4 *X4 = (const float4 *)X, *X04 = (const float4 *)X0, *XS4 = (const float4 *)Xself;
+    if (HAS_PUSH) PA = *e.push;
+    const float4 *X4 = (const float4 *)X, *XS4 = (const float4 *)e.Xself, *X04 = (const float4 *)e.X0;
+    const float4 *X14 = (const float4 *)e.X1;
     float4 *Y4 = (float4 *)Y;
-#define LAUNCH(V, PU, Z, S)                                                                                              \
-    spmm_bulk_kernel<V, PU, Z, S, false><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, n_rows, \
-                                                                              A.nnz, G, rows_per_cta, tile_rows, alpha, \
-                                                                              gamma, delta, X4, XS4, X04, Y4, hd, PA, 0.f, \
-                                                                              nullptr, nullptr)
-#define LAUNCHB(V, PU)                                                                                                   \
-    do {                                                                                                                 \
-        if (X0 && Xself) LAUNCH(V, PU, true, true); else if (X0) LAUNCH(V, PU, true, false);                             \
-        else if (Xself) LAUNCH(V, PU, false, true); else LAUNCH(V, PU, false, false);                                    \
-    } while (0)
-    if (A.data) { if (push) LAUNCHB(true, true); else LAUNCHB(true, false); }
-    else { if (push) LAUNCHB(false, true); else LAUNCHB(false, false); }
-#undef LAUNCHB
-#undef LAUNCH
+    auto bulk = A.data ? spmm_bulk_kernel<true, HAS_PUSH, HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>
+                       : spmm_bulk_kernel<false, HAS_PUSH, HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>;
+    bulk<<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta,
+                                                    tile_rows, e.alpha, e.gamma, e.delta, X4, XS4, X04, Y4,
+                                                    heavy ? SPMM_HEAVY_DEG : 0, PA, e.eps, X14, e.rscale);
     GEMB_CUDA(cudaGetLastError());
     count_launch();
     if (!heavy) return GEMB_OK;
-    return spmm_heavy_launch(ctx, A, b, alpha, X, gamma, Xself, delta, X0, 0.f, nullptr, Y, push);
-}
-
-int spmm4_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
-                 float gamma, const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y) {
-    if (!X1) return spmm3_launch(ctx, A, n_rows, b, alpha, X, gamma, Xself, delta, X0, Y);
-    GEMB_ARG(Xself && X0, "the fourth epilogue operand needs Xself and X0");
-    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "block width must be a multiple of 4, <= 1024");
-    if (n_rows == 0) return GEMB_OK;
-    const int G = b / 4;
-    const int rows_per_cta = 256 / G;
-    const int tile_rows = rows_per_cta * SPMM_TILE_PASSES;
-    const int64_t n_tiles = (n_rows + tile_rows - 1) / tile_rows;
-    GEMB_ARG(n_tiles < (int64_t)2147483647, "grid too large");
-    const bool heavy = A.n_items > 0;
-    const int hd = heavy ? SPMM_HEAVY_DEG : 0;
-    HaloPushArgs PA;
-    memset(&PA, 0, sizeof PA);
-#define LAUNCH(V)                                                                                                        \
-    spmm_bulk_kernel<V, false, true, true, true><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(                            \
-        A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta, tile_rows, alpha, gamma, delta, (const float4 *)X, \
-        (const float4 *)Xself, (const float4 *)X0, (float4 *)Y, hd, PA, eps, (const float4 *)X1, nullptr)
-    if (A.data) LAUNCH(true);
-    else LAUNCH(false);
-#undef LAUNCH
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    if (!heavy) return GEMB_OK;
-    return spmm_heavy_launch(ctx, A, b, alpha, X, gamma, Xself, delta, X0, eps, X1, Y, nullptr);
-}
-
-int spmm_scaled_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, float alpha, const float *X,
-                       const float *rscale, float *Y) {
-    GEMB_ARG(rscale, "spmm_scaled_launch: rscale");
-    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "block width must be a multiple of 4, <= 1024");
-    if (n_rows == 0) return GEMB_OK;
-    const int G = b / 4;
-    const int rows_per_cta = 256 / G;
-    const int tile_rows = rows_per_cta * SPMM_TILE_PASSES;
-    const int64_t n_tiles = (n_rows + tile_rows - 1) / tile_rows;
-    GEMB_ARG(n_tiles < (int64_t)2147483647, "grid too large");
-    const bool heavy = A.n_items > 0;
-    const int hd = heavy ? SPMM_HEAVY_DEG : 0;
-    HaloPushArgs PA;
-    memset(&PA, 0, sizeof PA);
-#define LAUNCH(V)                                                                                                        \
-    spmm_bulk_kernel<V, false, false, false, false, true><<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(                   \
-        A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta, tile_rows, alpha, 0.f, 0.f, (const float4 *)X,     \
-        nullptr, nullptr, (float4 *)Y, hd, PA, 0.f, nullptr, rscale)
-    if (A.data) LAUNCH(true);
-    else LAUNCH(false);
-#undef LAUNCH
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    if (!heavy) return GEMB_OK;
-    return spmm_heavy_launch(ctx, A, b, alpha, X, 0.f, nullptr, 0.f, nullptr, 0.f, nullptr, Y, nullptr, rscale);
-}
-
-int spmm_heavy_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int b, float alpha, const float *X, float gamma,
-                      const float *Xself, float delta, const float *X0, float eps, const float *X1, float *Y,
-                      const HaloPushArgs *push, const float *rscale) {
-    const int G = b / 4;
-    const int rows_per_cta = 256 / G;
-    const float4 *X4 = (const float4 *)X, *X04 = (const float4 *)X0, *XS4 = (const float4 *)Xself;
-    const float4 *X14 = (const float4 *)X1;
-    float4 *Y4 = (float4 *)Y;
-    HaloPushArgs PA;
-    memset(&PA, 0, sizeof PA);
-    if (push) PA = *push;
-    {
-        const size_t need = sizeof(float) * (size_t)A.n_items * b;
-        if (ctx->spmm_scratch_bytes < need) {
-            GEMB_CUDA(dfree(ctx->spmm_scratch));
-            ctx->spmm_scratch = nullptr; ctx->spmm_scratch_bytes = 0;
-            GEMB_CUDA(dmalloc(&ctx->spmm_scratch, need));
-            ctx->spmm_scratch_bytes = need;
-        }
-        float4 *P4 = (float4 *)ctx->spmm_scratch;
-#define HP(V) spmm_heavy_partial_kernel<V><<<A.n_items, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, A.item_row, A.item_beg, \
-                                                                            G, rows_per_cta, SPMM_HEAVY_CHUNK, X4, P4)
-        if (A.data) HP(true);
-        else HP(false);
-#undef HP
-        GEMB_CUDA(cudaGetLastError());
-        const int fgrid = (int)(((int64_t)A.n_heavy * G + 255) / 256);
-#define FIN(Z, S, X1P, SC) spmm_heavy_finish_kernel<Z, S, X1P, SC><<<fgrid, 256, 0, ctx->stream>>>(A.n_heavy, A.heavy_row,  \
-                                         A.heavy_first, G, alpha, gamma, delta, P4, XS4, X04, Y4, push != nullptr, PA, eps, X14, rscale)
-        if (rscale) FIN(false, false, false, true);    // spmm_scaled_launch: no other epilogue operand
-        else if (X1) FIN(true, true, true, false);     // spmm4_launch: X1 comes with Xself and X0
-        else if (X0 && Xself) FIN(true, true, false, false);
-        else if (X0) FIN(true, false, false, false);
-        else if (Xself) FIN(false, true, false, false);
-        else FIN(false, false, false, false);
-#undef FIN
-        GEMB_CUDA(cudaGetLastError());
-        count_launch(2);
+    const size_t need = sizeof(float) * (size_t)A.n_items * b;
+    if (ctx->spmm_scratch_bytes < need) {
+        GEMB_CUDA(dfree(ctx->spmm_scratch));
+        ctx->spmm_scratch = nullptr; ctx->spmm_scratch_bytes = 0;
+        GEMB_CUDA(dmalloc(&ctx->spmm_scratch, need));
+        ctx->spmm_scratch_bytes = need;
     }
+    float4 *P4 = (float4 *)ctx->spmm_scratch;
+    auto partial = A.data ? spmm_heavy_partial_kernel<true> : spmm_heavy_partial_kernel<false>;
+    partial<<<A.n_items, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, A.item_row, A.item_beg, G, rows_per_cta,
+                                               SPMM_HEAVY_CHUNK, X4, P4);
+    GEMB_CUDA(cudaGetLastError());
+    const int fgrid = (int)(((int64_t)A.n_heavy * G + 255) / 256);
+    spmm_heavy_finish_kernel<HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE><<<fgrid, 256, 0, ctx->stream>>>(
+        A.n_heavy, A.heavy_row, A.heavy_first, G, e.alpha, e.gamma, e.delta, P4, XS4, X04, Y4, HAS_PUSH, PA, e.eps, X14,
+        e.rscale);
+    GEMB_CUDA(cudaGetLastError());
+    count_launch(2);
+    return GEMB_OK;
+}
+
+int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, const float *X, float *Y,
+                const SpmmEpilogue &e) {
+    GEMB_ARG(!e.X1 || (e.Xself && e.X0), "the fourth epilogue operand needs Xself and X0");
+    GEMB_ARG(!e.X1 || !e.push, "the fourth epilogue operand is single-GPU");
+    GEMB_ARG(!e.rscale || (!e.Xself && !e.X0 && !e.X1 && !e.push), "the row scale takes no other epilogue operand");
+    GEMB_ARG(b > 0 && b % 4 == 0 && b <= 1024, "block width must be a multiple of 4, <= 1024");
+    if (n_rows == 0) return GEMB_OK;
+    //                                    PUSH   X0     SELF   X1     SCALE
+    if (e.rscale) return spmm_sweep<false, false, false, false, true>(ctx, A, n_rows, b, X, Y, e);
+    if (e.X1) return spmm_sweep<false, true, true, true, false>(ctx, A, n_rows, b, X, Y, e);
+    if (e.push) {
+        if (e.X0 && e.Xself) return spmm_sweep<true, true, true, false, false>(ctx, A, n_rows, b, X, Y, e);
+        if (e.X0) return spmm_sweep<true, true, false, false, false>(ctx, A, n_rows, b, X, Y, e);
+        if (e.Xself) return spmm_sweep<true, false, true, false, false>(ctx, A, n_rows, b, X, Y, e);
+        return spmm_sweep<true, false, false, false, false>(ctx, A, n_rows, b, X, Y, e);
+    }
+    if (e.X0 && e.Xself) return spmm_sweep<false, true, true, false, false>(ctx, A, n_rows, b, X, Y, e);
+    if (e.X0) return spmm_sweep<false, true, false, false, false>(ctx, A, n_rows, b, X, Y, e);
+    if (e.Xself) return spmm_sweep<false, false, true, false, false>(ctx, A, n_rows, b, X, Y, e);
+    return spmm_sweep<false, false, false, false, false>(ctx, A, n_rows, b, X, Y, e);
+}
+
+// a host block of `count` floats into a new device block (src null: none, dst stays null)
+static int stage(gemb_ctx *c, DeviceBuffer<float> &dst, const float *src, size_t count) {
+    if (!src) return GEMB_OK;
+    GEMB_CUDA(dst.alloc(count));
+    GEMB_CUDA(cudaMemcpyAsync(dst.get(), src, sizeof(float) * count, cudaMemcpyHostToDevice, c->stream));
+    return GEMB_OK;
+}
+
+// The sweep of the test hooks from host memory: X (all n rows) and the epilogue's blocks (the shard's rows) to the
+// device, one sweep of A or A^T over the shard, Y back.
+static int spmm_host(gemb_graph *g, int transpose, int b, const float *X, SpmmEpilogue e, float *Y) {
+    gemb_ctx *c = g->ctx;
+    GEMB_CUDA(cudaSetDevice(c->device));
+    DeviceBuffer<float> dX, dY, dXs, dX0, dX1, dS;
+    const size_t shard = (size_t)g->n_local * b;
+    GEMB_TRY(stage(c, dX, X, (size_t)g->n * b));
+    GEMB_TRY(stage(c, dXs, e.Xself, shard));
+    GEMB_TRY(stage(c, dX0, e.X0, shard));
+    GEMB_TRY(stage(c, dX1, e.X1, shard));
+    GEMB_TRY(stage(c, dS, e.rscale, (size_t)g->n_local));
+    GEMB_CUDA(dY.alloc(shard));
+    e.Xself = dXs.get(); e.X0 = dX0.get(); e.X1 = dX1.get(); e.rscale = dS.get();
+    GEMB_TRY(spmm_launch(c, transpose ? g->AT : g->A, g->n_local, b, dX.get(), dY.get(), e));
+    GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * shard, cudaMemcpyDeviceToHost, c->stream));
+    GEMB_CUDA(cudaStreamSynchronize(c->stream));
     return GEMB_OK;
 }
 
@@ -378,24 +324,8 @@ extern "C" int gemb_spmm4(gemb_graph *g, int transpose, int b, float alpha, cons
     GEMB_ARG(b > 0 && b % 4 == 0, "b must be a positive multiple of 4");
     GEMB_ARG(!X1 || (Xself && X0), "X1 needs Xself and X0");
     GEMB_ARG(!X1 || g->n_local == g->n, "the fourth epilogue operand is single-GPU");
-    gemb_ctx *c = g->ctx;
-    GEMB_CUDA(cudaSetDevice(c->device));
-    DeviceBuffer<float> dX, dY, dXs, dX0, dX1;
-    const size_t full = (size_t)g->n * b, shard = (size_t)g->n_local * b;
-    GEMB_CUDA(dX.alloc(full));
-    GEMB_CUDA(dY.alloc(shard));
-    if (Xself) GEMB_CUDA(dXs.alloc(shard));
-    if (X0) GEMB_CUDA(dX0.alloc(shard));
-    if (X1) GEMB_CUDA(dX1.alloc(shard));
-    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * full, cudaMemcpyHostToDevice, c->stream));
-    if (Xself) GEMB_CUDA(cudaMemcpyAsync(dXs.get(), Xself, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
-    if (X0) GEMB_CUDA(cudaMemcpyAsync(dX0.get(), X0, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
-    if (X1) GEMB_CUDA(cudaMemcpyAsync(dX1.get(), X1, sizeof(float) * shard, cudaMemcpyHostToDevice, c->stream));
-    GEMB_TRY(spmm4_launch(c, transpose ? g->AT : g->A, g->n_local, b, alpha, dX.get(), gamma, dXs.get(), delta, dX0.get(),
-                          eps, dX1.get(), dY.get()));
-    GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * shard, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+    return spmm_host(g, transpose, b, X,
+                     {.alpha = alpha, .gamma = gamma, .Xself = Xself, .delta = delta, .X0 = X0, .eps = eps, .X1 = X1}, Y);
 }
 
 extern "C" int gemb_spmm_scaled(gemb_graph *g, int transpose, int b, float alpha, const float *X, const float *rscale,
@@ -404,16 +334,5 @@ extern "C" int gemb_spmm_scaled(gemb_graph *g, int transpose, int b, float alpha
     GEMB_ARG(b > 0 && b % 4 == 0, "b must be a positive multiple of 4");
     gemb_ctx *c = g->ctx;
     GEMB_ARG(c->nranks == 1 && g->n_local == g->n, "gemb_spmm_scaled is single-GPU");
-    GEMB_CUDA(cudaSetDevice(c->device));
-    DeviceBuffer<float> dX, dS, dY;
-    const size_t full = (size_t)g->n * b;
-    GEMB_CUDA(dX.alloc(full));
-    GEMB_CUDA(dS.alloc((size_t)std::max<int64_t>(g->n, 1)));
-    GEMB_CUDA(dY.alloc(full));
-    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * full, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(dS.get(), rscale, sizeof(float) * g->n, cudaMemcpyHostToDevice, c->stream));
-    GEMB_TRY(spmm_scaled_launch(c, transpose ? g->AT : g->A, g->n, b, alpha, dX.get(), dS.get(), dY.get()));
-    GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * full, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+    return spmm_host(g, transpose, b, X, {.alpha = alpha, .rscale = rscale}, Y);
 }
