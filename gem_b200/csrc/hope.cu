@@ -134,14 +134,17 @@ static int comm_allgather(HopeWork &W, const float *shard_src, int width) {
     return GEMB_OK;
 }
 
-static int comm_allreduce_f64(HopeWork &W, double *buf, size_t count) {
+// in-place all-reduce of `count` values over the ranks (nothing on one GPU); `what` names it in the error message.  timed:
+// counted as communication (t_comm), as every reduction of the solvers is; the set-up's one-off ones are not.
+static int comm_allreduce(HopeWork &W, void *buf, size_t count, ncclDataType_t type = ncclDouble, ncclRedOp_t op = ncclSum,
+                          bool timed = true, const char *what = "ncclAllReduce") {
     if (W.c->nranks == 1) return GEMB_OK;
     NcclApi *api = nccl_api();
     if (!api) return GEMB_ERR_NCCL;
-    GEMB_TRY(W.c->t_comm.begin(W.c->stream));
-    ncclResult_t r = api->AllReduce(buf, buf, count, ncclDouble, ncclSum, (ncclComm_t)W.c->comm, W.c->stream);
-    if (r != ncclSuccess) { set_error("ncclAllReduce: %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
-    GEMB_TRY(W.c->t_comm.end(W.c->stream));
+    if (timed) GEMB_TRY(W.c->t_comm.begin(W.c->stream));
+    ncclResult_t r = api->AllReduce(buf, buf, count, type, op, (ncclComm_t)W.c->comm, W.c->stream);
+    if (r != ncclSuccess) { set_error("%s: %s", what, api->GetErrorString(r)); return GEMB_ERR_NCCL; }
+    if (timed) GEMB_TRY(W.c->t_comm.end(W.c->stream));
     return GEMB_OK;
 }
 
@@ -258,7 +261,7 @@ static int gram_full(HopeWork &W, const float *P, const float *Q, double *G) {
     GEMB_TRY(W.c->t_dense.begin(W.c->stream));
     GEMB_TRY(gram_launch(W.c, W.rows, P, W.b, Q, W.b, G));
     GEMB_TRY(W.c->t_dense.end(W.c->stream));
-    GEMB_TRY(comm_allreduce_f64(W, G, (size_t)W.b * W.b));
+    GEMB_TRY(comm_allreduce(W, G, (size_t)W.b * W.b));
     return GEMB_OK;
 }
 
@@ -428,15 +431,6 @@ static int inv_degree(HopeWork &W) {
     return GEMB_OK;
 }
 
-static int comm_allreduce_max_f64(HopeWork &W, double *buf, size_t count) {
-    if (W.c->nranks == 1) return GEMB_OK;
-    NcclApi *api = nccl_api();
-    if (!api) return GEMB_ERR_NCCL;
-    ncclResult_t r = api->AllReduce(buf, buf, count, ncclDouble, ncclMax, (ncclComm_t)W.c->comm, W.c->stream);
-    if (r != ncclSuccess) { set_error("ncclAllReduce(max): %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
-    return GEMB_OK;
-}
-
 // ||A||_inf and the sign of the weights in one pass over the CSR shard
 static int rowsum_bound(HopeWork &W, double *norm_inf, bool *nonneg) {
     gemb_ctx *c = W.c;
@@ -446,7 +440,7 @@ static int rowsum_bound(HopeWork &W, double *norm_inf, bool *nonneg) {
         GEMB_CUDA(cudaGetLastError());
         count_launch();
     }
-    GEMB_TRY(comm_allreduce_max_f64(W, W.scal.get(), 2));
+    GEMB_TRY(comm_allreduce(W, W.scal.get(), 2, ncclDouble, ncclMax, false, "ncclAllReduce(max)"));
     double h[2];
     GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
     *norm_inf = h[0];
@@ -454,48 +448,25 @@ static int rowsum_bound(HopeWork &W, double *norm_inf, bool *nonneg) {
     return GEMB_OK;
 }
 
-// ||A||_2 by power iteration on A^T A with a 4-column block
-static int estimate_norm2(HopeWork &W, uint64_t seed, float *x, float *y, float *z, double *out) {
-    gemb_ctx *c = W.c;
-    gemb_graph *g = W.g;
-    const int pw = 4;
-    GEMB_TRY(randn_launch(c, W.rows, pw, seed ^ 0x5bd1e995u, (uint64_t)g->row0, x));
-    double est = 0.0, prev = -1.0;
-    for (int it = 0; it < 16; it++) {
-        double h[2];
-        GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal.get()));
-        GEMB_TRY(publish(W, x, pw));
-        GEMB_TRY(dist_spmm(W, false, pw, x, {}, y, false, true));
-        GEMB_TRY(dist_spmm(W, true, pw, y, {}, z, false));
-        GEMB_TRY(sumsq_launch(c, W.rows * pw, z, W.scal.get() + 1));
-        GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 2));
-        GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
-        if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }  // A^T A x = 0 (empty graph)
-        est = sqrt(sqrt(h[1] / h[0]));   // ||A^T A x|| / ||x|| -> sigma_max^2
-        GEMB_TRY(scale_launch(c, W.rows * pw, (float)(1.0 / sqrt(h[1])), z));
-        std::swap(x, z);
-        if (prev > 0 && fabs(est - prev) <= 1e-3 * est && it >= 3) break;
-        prev = est;
-    }
-    *out = est;
-    return GEMB_OK;
-}
-
-// spectral_mode 2: ||M||_2^2 = ||M^T M||_2 by power iteration on the composite operator with a 4-column block.  From
-// below, like estimate_norm2: hope_symmetric raises it to the largest |Ritz value| (SpecMap::observe).
-static int estimate_composite_norm(HopeWork &W, uint64_t seed, float *x, float *y, double *out) {
+// ||B||_2 of a positive semi-definite B (apply(x, y): y = B x) by at most `cap` power steps on a width-4 block in work
+// blocks 3 and 2; `root`: its square root (B = A^T A: ||A||_2).  From below; 0 when B x = 0 (an empty graph; M = 0).
+template <class Apply>
+static int power_norm(HopeWork &W, uint64_t seed, int cap, bool root, Apply apply, double *out) {
     gemb_ctx *c = W.c;
     const int pw = 4;
+    float *x = W.buf[3], *y = W.buf[2];
     GEMB_TRY(randn_launch(c, W.rows, pw, seed ^ 0x5bd1e995u, (uint64_t)W.g->row0, x));
     double est = 0.0, prev = -1.0;
-    for (int it = 0; it < 32; it++) {
+    for (int it = 0; it < cap; it++) {
         double h[2];
         GEMB_TRY(sumsq_launch(c, W.rows * pw, x, W.scal.get()));
-        GEMB_TRY(op_apply(W, pw, x, {}, y, false));
+        GEMB_TRY(apply(x, y));
         GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get() + 1));
+        GEMB_TRY(comm_allreduce(W, W.scal.get(), 2));
         GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
-        if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }   // M^T M x = 0 (M = 0: P = I)
-        est = sqrt(h[1] / h[0]);                                      // ||M^T M x|| / ||x|| -> ||M||_2^2
+        if (!(h[0] > 0.0) || !(h[1] > 0.0)) { est = 0.0; break; }
+        est = sqrt(h[1] / h[0]);
+        if (root) est = sqrt(est);
         GEMB_TRY(scale_launch(c, W.rows * pw, (float)(1.0 / sqrt(h[1])), y));
         std::swap(x, y);
         if (prev > 0 && fabs(est - prev) <= 1e-3 * est && it >= 3) break;
@@ -503,6 +474,24 @@ static int estimate_composite_norm(HopeWork &W, uint64_t seed, float *x, float *
     }
     *out = est;
     return GEMB_OK;
+}
+
+// ||A||_2: at most 16 power steps on A^T A (sweep 1 into work block 4)
+static int estimate_norm2(HopeWork &W, uint64_t seed, double *out) {
+    float *t = W.buf[4];
+    return power_norm(W, seed, 16, true, [&](const float *x, float *y) {
+        GEMB_TRY(publish(W, x, 4));
+        GEMB_TRY(dist_spmm(W, false, 4, x, {}, t, false, true));
+        return dist_spmm(W, true, 4, t, {}, y, false);
+    }, out);
+}
+
+constexpr int kMaxSeriesTerms = 4096;
+
+// terms J of a series whose terms decay at least like x^j until they fall below tol: ceil(log tol / log x), capped
+static int series_terms(double x, double tol) {
+    if (x <= 1e-30) return 1;
+    return std::max(1, std::min((int)ceil(log(tol) / log(x)), kMaxSeriesTerms));
 }
 
 // beta * ||A||_2 >= 1 does not mean the Katz series diverges: it converges iff beta * rho(A) < 1, and a directed graph
@@ -524,7 +513,7 @@ static int probe_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t s
             double h = 0.0;
             GEMB_TRY(dist_spmm(W, tr == 1, pw, x, {.alpha = beta}, y, false));
             GEMB_TRY(sumsq_launch(c, W.rows * pw, y, W.scal.get()));
-            GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), 1));
+            GEMB_TRY(comm_allreduce(W, W.scal.get(), 1));
             GEMB_TRY(copy_sync(c, &h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
             const double nt = sqrt(h);
             if (prev > 0.0) *rho_est = std::max(*rho_est * (j > 8 ? 0.0 : 1.0), nt / prev / (double)beta);
@@ -537,7 +526,7 @@ static int probe_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t s
         if (!done) return GEMB_ERR_DIVERGE;
         Jbest = std::max(Jbest, j);
     }
-    *J_out = std::min(4096, Jbest + Jbest / 8 + 2);
+    *J_out = std::min(kMaxSeriesTerms, Jbest + Jbest / 8 + 2);
     return GEMB_OK;
 }
 
@@ -549,25 +538,29 @@ struct Opts {
     uint64_t seed = 1234;
 };
 
-static int katz_terms_for(double beta, double nrm, double katz_tol) {
-    const double x1 = beta * nrm * 1.02;
-    if (x1 <= 1e-30) return 1;
-    int J = (int)ceil(log(katz_tol) / log(x1));
-    return std::max(1, std::min(J, 4096));
-}
+// What a solve starts from, decided once before it (hope_setup)
+struct Setup {
+    float beta;                 // the beta the solve runs with: beta < 0 asks for |beta| / ||A||_2
+    int J;                      // general solver: the series' terms (opts.katz_terms when given)
+    double norm2 = 0.0;         // the power-iteration estimate: ||A||_2, or ||M||_2^2 (composite); 0: none ran
+    double norm_inf = 0.0;      // ||A||_inf (rowsum_bound); 0: not measured
+    bool ritz_bound = false;    // symmetric A >= 0 inside the Katz radius: Ritz values bound the spectrum
+    // the symmetric solver's a priori bound on |l| (SpecMap::symmetric)
+    double spectrum_norm() const { return ritz_bound ? norm_inf : norm2; }
+};
 
 // The Katz terms J of S = sum_{j=1..J} (beta A)^j for the general solver and the 'SVD error' diagnostic: ||A||_2 by
-// power iteration; beta ||A||_2 * 1.02 < 1 bounds the terms a priori (katz_terms_for).  Above that bound the series
+// power iteration; beta ||A||_2 * 1.02 < 1 bounds the terms a priori (series_terms).  Above that bound the series
 // still converges when beta rho(A) < 1, and rho(A) of a directed graph can lie far below ||A||_2 (a DAG: rho = 0), so
 // probe_katz_terms measures the decay of the terms; GEMB_ERR_DIVERGE only when they do not decay.  probe = false
 // (symmetric A, where ||A||_2 = rho(A); the halo exchange) refuses at the bound.  Leaves work blocks 2..4 dirty.
 static int general_katz_terms(HopeWork &W, float beta, double katz_tol, uint64_t seed, bool probe, double *nrm_out,
                               int *J_out) {
     double nrm = 0.0;
-    GEMB_TRY(estimate_norm2(W, seed, W.buf[3], W.buf[4], W.buf[2], &nrm));
+    GEMB_TRY(estimate_norm2(W, seed, &nrm));
     *nrm_out = nrm;
     if ((double)beta * nrm * 1.02 < 1.0) {
-        *J_out = katz_terms_for(beta, nrm, katz_tol);
+        *J_out = series_terms((double)beta * nrm * 1.02, katz_tol);
         return GEMB_OK;
     }
     double rho = nrm;
@@ -593,7 +586,7 @@ static int residual_check(HopeWork &W, float beta, int J, const float *P, const 
     coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(W.rows, b, scr0, Qs, W.scal.get());
     GEMB_CUDA(cudaGetLastError());
     count_launch();
-    GEMB_TRY(comm_allreduce_f64(W, W.scal.get(), b));
+    GEMB_TRY(comm_allreduce(W, W.scal.get(), b));
     std::vector<double> rs(b);
     GEMB_TRY(copy_sync(c, rs.data(), W.scal.get(), sizeof(double) * b, cudaMemcpyDeviceToHost));
     double rm = 0.0;
@@ -625,7 +618,7 @@ static int ritz_eigh(HopeWork &W, float tol, bool symmetrize, std::vector<double
         GEMB_TRY(s);
         GEMB_CUDA(cudaEventRecord(W.fork_join[1], c->side));
         GEMB_CUDA(cudaStreamWaitEvent(c->stream, W.fork_join[1], 0));
-        GEMB_TRY(comm_allreduce_f64(W, W.G.get(), (size_t)b * b));
+        GEMB_TRY(comm_allreduce(W, W.G.get(), (size_t)b * b));
         ritz_quadform_kernel<<<b, 128, sizeof(double) * b, c->stream>>>(b, W.G.get(), W.Z.get(), W.w.get() + b);
         GEMB_CUDA(cudaGetLastError());
         count_launch();
@@ -821,24 +814,38 @@ static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t 
 struct SpecMap {
     double beta;
     bool katz;
-    double norm;    // a priori bound on |l|: ||A||_inf, or the power-iteration ||A||_2
-    double bound;   // current bound on |l|
-    bool estimated = false;   // norm is the power-iteration estimate, which can lie below ||A||_2 (a cluster of top values)
-    bool negdef = false;      // spectral_mode 2: the operator is negative semi-definite; the wanted end is 0
-    SpecMap(double beta, bool katz, double norm) : beta(beta), katz(katz), norm(norm), bound(norm * 1.02 + 1e-30) {}
-    // an estimated norm is raised to max |l| over the Ritz values l[0..n) (all inside the spectrum), so that the clamp
-    // never moves a Ritz value; false when then beta * norm >= 1 (the Katz series diverges)
-    bool observe(const double *l, int n) {
-        if (!estimated) return true;
-        for (int i = 0; i < n; i++) norm = std::max(norm, fabs(l[i]));
+    double norm;       // a priori bound on |l|: ||A||_inf, or the power-iteration estimate
+    double bound;      // current bound on |l|
+    bool estimated;    // norm is the power-iteration estimate, which can lie below ||A||_2 (a cluster of top values)
+    bool negdef;       // spectral_mode 2: the operator is negative semi-definite; the wanted end is 0
+    double growth;     // a true norm: the bound is this factor over the largest |Ritz value|
+    SpecMap(double beta, bool katz, double norm, bool estimated, bool negdef, double growth)
+        : beta(beta), katz(katz), norm(norm), bound(norm * 1.02 + 1e-30), estimated(estimated), negdef(negdef),
+          growth(growth) {}
+    // The Chebyshev solver's map.  With ritz_bound, A is symmetric with non-negative weights and norm = ||A||_inf; then
+    // lambda_max = rho(A) >= |lambda_min| (Perron-Frobenius), so 1.05 * (largest Ritz value) bounds the spectrum on both
+    // sides.  Otherwise norm is the power-iteration estimate of ||A||_2 (||M||_2^2 for the composite).
+    static SpecMap symmetric(const Setup &s, Mode mode) {
+        return SpecMap(s.beta, mode == Mode::katz, s.spectrum_norm(), !s.ritz_bound, mode == Mode::composite, 1.05);
+    }
+    // the Lanczos solver's map: ||A||_inf (the estimate when no row sum was measured), tightened to 1.02 * max |Ritz value|
+    static SpecMap lanczos(const Setup &s) {
+        return SpecMap(s.beta, true, s.norm_inf > 0.0 ? s.norm_inf : s.norm2, false, false, 1.02);
+    }
+    // one round's update from the Ritz values l[0..n) (all inside the spectrum): a true norm gives the bound
+    // growth * max |l|, never above the a priori one; an estimated norm is raised to max |l|, so that the clamp never
+    // moves a Ritz value.  false when then beta * norm >= 1 (the Katz series diverges)
+    bool update(const double *l, int n) {
+        double amax = 0.0;
+        for (int i = 0; i < n; i++) amax = std::max(amax, fabs(l[i]));
+        if (!estimated) { bound = std::min(norm * 1.02, growth * amax) + 1e-30; return true; }
+        norm = std::max(norm, amax);
         bound = std::max(bound, norm * 1.02 + 1e-30);
         return !katz || beta * norm < 1.0;
     }
-    // bound from the Ritz values l[0..n): growth * max |l|, never above the a priori one
-    void tighten(const double *l, int n, double growth) {
-        double amax = 0.0;
-        for (int i = 0; i < n; i++) amax = std::max(amax, fabs(l[i]));
-        bound = std::min(norm * 1.02, growth * amax) + 1e-30;
+    // the Katz terms of compute_residual's check: the rule of the a priori bound, on the bound the map ended with
+    int residual_terms(double katz_tol) const {
+        return series_terms(beta * (estimated ? norm : bound / 1.02) * 1.02, katz_tol);
     }
     double clamp(double l) const { return std::max(-bound, std::min(negdef ? 0.0 : bound, l)); }
     double f(double l) const { return beta * l / (1.0 - beta * l); }
@@ -884,10 +891,7 @@ static int diverge_error(const SpecMap &map) {
     return GEMB_ERR_DIVERGE;
 }
 
-// ritz_bound: A is symmetric with non-negative weights and map.norm = ||A||_inf; then lambda_max = rho(A) >= |lambda_min|
-// (Perron-Frobenius), so 1.05 * (largest Ritz value) bounds the spectrum on both sides and the 2 x 16 narrow SpMM sweeps
-// of the power iteration are not needed.  Otherwise map.norm is a tight estimate of ||A||_2 (power iteration).
-static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map, bool ritz_bound, HopeResult &R) {
+static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map, HopeResult &R) {
     gemb_ctx *c = W.c;
     const bool eigen = eigen_output(o.mode);
     const int b = W.b;
@@ -970,8 +974,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map,
         // round's interval costs two extra rounds -- 75 instead of 56 SpMM sweeps -- and is slower overall;
         // the eigen-decomposition therefore stays on the critical path.)
         GEMB_TRY(ritz_eigh(W, o.tol, true, lam, o.stop_rule == 1 ? AV : nullptr));
-        if (ritz_bound) map.tighten(lam.data(), b, 1.05);
-        else if (!map.observe(lam.data(), b)) return diverge_error(map);
+        if (!map.update(lam.data(), b)) return diverge_error(map);
         R.norm = map.norm;
         for (int i = 0; i < b; i++) gval[i] = map.key(lam[i]);
         std::iota(order.begin(), order.end(), 0);
@@ -1086,7 +1089,7 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map,
     if (eigen || !o.compute_residual) return GEMB_OK;
 
     // check the triplets against the Katz operator itself: || S^T u - sigma v || / sigma_max
-    const int J = katz_terms_for(map.beta, ritz_bound ? map.bound / 1.02 : map.norm, o.katz_tol);
+    const int J = map.residual_terms(o.katz_tol);
     std::vector<float> MP((size_t)b * b, 0.f), MQ((size_t)b * b, 0.f);
     for (int col = 0; col < b; col++) {
         const SpecMap::Column t = map.column(lam[col]);
@@ -1189,7 +1192,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
         GEMB_TRY(c->t_dense.begin(c->stream));
         GEMB_TRY(gram_launch(c, rows, P, b1, Qp, b2, G));
         GEMB_TRY(c->t_dense.end(c->stream));
-        return comm_allreduce_f64(W, G, (size_t)b1 * b2);
+        return comm_allreduce(W, G, (size_t)b1 * b2);
     };
     // CholeskyQR2 of the n x p block `src` in place (scratch Tb); Rout (p x p, host, row-major upper) = R2 * R1
     std::vector<double> Rh((size_t)p * p), R1((size_t)p * p), R2((size_t)p * p), Ginv((size_t)p * p);
@@ -1287,7 +1290,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
         GEMB_TRY(c->t_dense.end(c->stream));
         GEMB_CUDA(cudaMemcpyAsync(theta.data(), wd.get(), sizeof(double) * m, cudaMemcpyDeviceToHost, c->stream));
         GEMB_TRY(copy_sync(c, Y.data(), Yd.get(), sizeof(double) * m * m, cudaMemcpyDeviceToHost));
-        map.tighten(theta.data(), m, 1.02);
+        if (!map.update(theta.data(), m)) return diverge_error(map);
         for (int i = 0; i < m; i++) fabsv[i] = map.key(theta[i]);
         std::iota(order.begin(), order.begin() + m, 0);
         std::sort(order.begin(), order.begin() + m, [&](int a2, int b2) { return fabsv[a2] > fabsv[b2]; });
@@ -1526,7 +1529,7 @@ static int hope_options(gemb_graph *g, float *beta, const gemb_hope_opts *uo, Op
 
 // The set-up of spectral_modes 3-5 on the device, before the first application of S (W's scalars allocated):
 // modes 4 and 5 refuse negative weights and mode 5 a row sum of P above 1 (one pass over the CSR, csr_rowsum_kernel),
-// mode 4 builds D (inv_degree), mode 5 takes J = ceil(log katz_tol / log alpha) unless katz_terms gave one.  *J: in,
+// mode 4 builds D (inv_degree), mode 5 takes J = series_terms(alpha) unless katz_terms gave one.  *J: in,
 // opts.katz_terms (0: not given); out, the series' terms (0 for modes 3 and 4).  No norm estimate: modes 3 and 4 are
 // two sweeps per application, and ||alpha P||_inf <= alpha bounds the rooted PageRank series a priori.
 static int proximity_setup(HopeWork &W, const Opts &o, float beta, int *J) {
@@ -1542,8 +1545,45 @@ static int proximity_setup(HopeWork &W, const Opts &o, float beta, int *J) {
         return GEMB_OK;
     }
     GEMB_ARG(pinf <= 1.0 + 1e-5, "spectral_mode 5 needs P = D_out^-1 A (every row sum <= 1)");
-    if (*J <= 0) *J = std::max(1, std::min(4096, (int)ceil(log((double)o.katz_tol) / log((double)beta))));
+    if (*J <= 0) *J = series_terms(beta, o.katz_tol);
     return GEMB_OK;
+}
+
+// The set-up of gemb_hope, once before the solve (W allocated; leaves work blocks 2..4 zeroed).  Beta < 0 is relative to
+// the spectral radius (BASELINE.json configs[3]: "beta = 0.5 / rho_hat"), ||A||_2 standing in for it.  The symmetric
+// solvers need no norm estimate when the Ritz values bound the spectrum (SpecMap::symmetric); else one estimate of ||A||_2
+// serves both the bound and J, and general_katz_terms probes the series of a directed A past the a priori bound.
+static int hope_setup(HopeWork &W, const Opts &o, int algo, float beta, Setup *s) {
+    *s = Setup{beta, o.katz_terms};
+    if (general_only(W.mode)) return proximity_setup(W, o, beta, &s->J);
+    if (W.mode == Mode::composite) {            // ||M||_2^2, 32 steps on M^T M
+        GEMB_TRY(power_norm(W, o.seed, 32, false, [&](const float *x, float *y) { return op_apply(W, 4, x, {}, y, false); },
+                            &s->norm2));
+        if (!(s->norm2 > 0.0)) s->norm2 = 1.0;     // M = 0: the spectrum is {0}, any positive bound holds it
+        return clear_scratch(W);
+    }
+    if (beta < 0.f) {
+        GEMB_TRY(estimate_norm2(W, o.seed, &s->norm2));
+        if (!(s->norm2 > 0.0)) { set_error("beta < 0 asks for beta = |beta| / ||A||_2, but ||A||_2 = 0 (empty graph)"); return GEMB_ERR_ARG; }
+        s->beta = (float)(-(double)beta / s->norm2);
+        GEMB_TRY(clear_scratch(W));
+    }
+    if (algo >= 2) {
+        bool nonneg = false;
+        GEMB_TRY(rowsum_bound(W, &s->norm_inf, &nonneg));
+        s->ritz_bound = nonneg && (double)s->beta * s->norm_inf * 1.02 < 1.0;
+        if (s->ritz_bound) return GEMB_OK;
+    }
+    if (beta < 0.f) {
+        if ((double)s->beta * s->norm2 * 1.02 >= 1.0) { set_error("|beta| / ||A||_2 with |beta| >= 0.98: outside the Katz convergence radius"); return GEMB_ERR_DIVERGE; }
+        if (s->J <= 0) s->J = series_terms((double)s->beta * s->norm2 * 1.02, o.katz_tol);
+        return GEMB_OK;
+    }
+    if (algo == 1 && s->J > 0) return GEMB_OK;  // opts.katz_terms: no estimate
+    int J = 0;
+    GEMB_TRY(general_katz_terms(W, s->beta, o.katz_tol, o.seed, algo == 1, &s->norm2, &J));
+    if (s->J <= 0) s->J = J;
+    return clear_scratch(W);
 }
 
 }  // namespace gemb
@@ -1576,15 +1616,12 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     if (c->nranks > 1 && algo >= 2 && !mg_allgather) {
         int hs = halo_build(g);
         if (hs == GEMB_OK) hs = halo_buffers(g, 5, b);
-        NcclApi *api = nccl_api();
-        if (!api) return GEMB_ERR_NCCL;
         int hflag = (hs == GEMB_OK) ? 1 : 0;
         DeviceBuffer<int> flag;
         GEMB_CUDA(flag.alloc(1));
         GEMB_CUDA(cudaMemcpyAsync(flag.get(), &hflag, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-        ncclResult_t r = api->AllReduce(flag.get(), flag.get(), 1, ncclInt, ncclMin, (ncclComm_t)c->comm, c->stream);
+        GEMB_TRY(comm_allreduce(W, flag.get(), 1, ncclInt, ncclMin, false, "ncclAllReduce(halo agreement)"));
         GEMB_TRY(copy_sync(c, &hflag, flag.get(), sizeof(int), cudaMemcpyDeviceToHost));
-        if (r != ncclSuccess) { set_error("ncclAllReduce(halo agreement): %s", api->GetErrorString(r)); return GEMB_ERR_NCCL; }
         W.halo = hflag == 1;
         if (!W.halo && o.verbose) fprintf(stderr, "[gemb_hope] halo exchange unavailable (%s); all-gather per sweep\n", gemb_last_error());
     }
@@ -1617,59 +1654,18 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
     GEMB_CUDA(ev.create());
     GEMB_CUDA(cudaEventRecord(ev[0], c->stream));
 
-    double nrm = 0.0, hard_bound = 0.0;
-    int J = o.katz_terms;
-    bool have_nrm = false, ritz_bound = false;
-    if (beta < 0.f) {
-        // beta given relative to the spectral radius: beta = |beta| / ||A||_2 (= rho(A) for the symmetric graphs of
-        // BASELINE.json configs[3]: "beta = 0.5 / rho_hat"), ||A||_2 by power iteration on a width-4 block
-        GEMB_TRY(estimate_norm2(W, o.seed, W.buf[3], W.buf[4], W.buf[2], &nrm));
-        if (!(nrm > 0.0)) { set_error("beta < 0 asks for beta = |beta| / ||A||_2, but ||A||_2 = 0 (empty graph)"); return GEMB_ERR_ARG; }
-        beta = (float)(-(double)beta / nrm);
-        have_nrm = true;
-        GEMB_TRY(clear_scratch(W));
-    }
-    bool need_power = (J <= 0 && algo == 1) && !have_nrm && !general_only(W.mode);
-    if (general_only(W.mode)) {
-        GEMB_TRY(proximity_setup(W, o, beta, &J));
-    } else if (W.mode == Mode::composite) {
-        // the Perron-Frobenius shortcut (ritz_bound) does not apply to -M^T M: ||M||_2^2 by power iteration
-        GEMB_TRY(estimate_composite_norm(W, o.seed, W.buf[3], W.buf[4], &nrm));
-        if (!(nrm > 0.0)) nrm = 1.0;                       // M = 0: the spectrum is {0}, any positive bound holds it
-        GEMB_TRY(clear_scratch(W));
-    } else if (algo >= 2) {
-        bool nonneg = false;
-        GEMB_TRY(rowsum_bound(W, &hard_bound, &nonneg));
-        if (nonneg && (double)beta * hard_bound * 1.02 < 1.0) ritz_bound = true;   // spectrum bounds from Ritz values
-        else need_power = !have_nrm;
-    }
-    if (have_nrm && !ritz_bound) {
-        if ((double)beta * nrm * 1.02 >= 1.0) { set_error("|beta| / ||A||_2 with |beta| >= 0.98: outside the Katz convergence radius"); return GEMB_ERR_DIVERGE; }
-        if (J <= 0) J = katz_terms_for(beta, nrm, o.katz_tol);
-        if (hard_bound <= 0.0) hard_bound = nrm;
-    }
-    if (need_power) {
-        int Jg = 0;
-        GEMB_TRY(general_katz_terms(W, beta, o.katz_tol, o.seed, algo == 1 && !W.halo, &nrm, &Jg));
-        if (J <= 0) J = Jg;
-        if (hard_bound <= 0.0) hard_bound = nrm;
-        GEMB_TRY(clear_scratch(W));
-    }
+    Setup setup;
+    GEMB_TRY(hope_setup(W, o, algo, beta, &setup));
 
     HopeResult R;
     int s;
     // thick-restart Lanczos needs room for its basis (k + 16 kept + expansions); tiny graphs take the subspace solver
     const bool lanczos_fits = g->n >= 2048;
-    // a priori spectrum bound: ||A||_inf for Lanczos; for Chebyshev see hope_symmetric
-    const SpecMap lanczos_map(beta, true, hard_bound);
-    SpecMap sym_map(beta, o.mode == Mode::katz, ritz_bound ? hard_bound : nrm);
-    sym_map.estimated = !ritz_bound;                              // else ||A||_inf: a true bound
-    sym_map.negdef = o.mode == Mode::composite;
-    if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, lanczos_map, R);
+    if (algo == 3 && lanczos_fits) s = hope_lanczos(W, o, d, SpecMap::lanczos(setup), R);
     else if (algo >= 2) {
-        s = hope_symmetric(W, o, d, k, sym_map, ritz_bound, R);
-        if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, lanczos_map, R); }
-    } else s = hope_general(W, o, d, beta, J, R);
+        s = hope_symmetric(W, o, d, k, SpecMap::symmetric(setup, o.mode), R);
+        if (s == GEMB_SWITCH_TO_LANCZOS) { R = HopeResult(); s = hope_lanczos(W, o, d, SpecMap::lanczos(setup), R); }
+    } else s = hope_general(W, o, d, setup.beta, setup.J, R);
     if (s != GEMB_OK) return s;
 
     GEMB_CUDA(cudaEventRecord(ev[1], c->stream));
@@ -1722,9 +1718,9 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         stats->total_ms = total_ms;
         stats->h2d_ms = 0.0;
         stats->d2h_ms = d2h_ms;
-        /* ||A||_inf when no power iteration ran; else the power-iteration estimate, raised to the largest |Ritz value| */
-        stats->norm2_A = (float)(ritz_bound ? hard_bound : std::max(nrm, R.norm));
-        stats->beta_used = beta;
+        /* ||A||_inf when Ritz values bound the spectrum; else the power-iteration estimate, raised to the largest |Ritz value| */
+        stats->norm2_A = (float)std::max(setup.spectrum_norm(), R.norm);
+        stats->beta_used = setup.beta;
         stats->ritz_change = (float)R.change;
         stats->resid_max = R.resid_max;
     }

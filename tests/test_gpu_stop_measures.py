@@ -12,7 +12,7 @@ B  the converged contract  converged == 1 => every wanted pair's fp64 Katz resid
 C  ritz_change fidelity    solves are bit-reproducible, so max_iters = m - 1 returns round m - 1's values: the ritz_change of
                         the max_iters = m run equals value_change of the two runs' sigma within 1e-3 ref + 2e-7.
 D  resid_max            = fp64 max ||S^T u - sigma v|| / sigma_max within 0.05 ref + 1e-5.
-E  Katz terms           power iteration ran: 0.98 ||A||_2 <= norm2_A <= (1 + 1e-5) ||A||_2 (the margin katz_terms_for
+E  Katz terms           power iteration ran: 0.98 ||A||_2 <= norm2_A <= (1 + 1e-5) ||A||_2 (the margin series_terms
                         assumes); it did not: norm2_A = ||A||_inf; algorithm 1: (beta ||A||_2)^J <= 1.5 katz_tol.
 
 Floors, from the fp32 error model (u = 2^-24 = 6.0e-8, the unit roundoff of the stored blocks):
