@@ -159,10 +159,7 @@ static int apply_tc_launch_t(gemb_ctx *ctx, const ApplyTcParams &p, int grid, si
         GEMB_CUDA(cudaFuncSetAttribute(apply_tc_kernel<TILE_M, NPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
         attr_bytes = smem_bytes;
     }
-    apply_tc_kernel<TILE_M, NPAD><<<grid, 384, smem_bytes, ctx->stream>>>(p);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, apply_tc_kernel<TILE_M, NPAD>, grid, 384, smem_bytes, p);
 }
 
 template <int TILE_M>

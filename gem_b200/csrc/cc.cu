@@ -200,11 +200,6 @@ cc_gather_kernel(int64_t k, int64_t m, const int64_t *__restrict__ out_ptr, cons
     }
 }
 
-static int cc_grid(gemb_ctx *c, int64_t items) {
-    const int64_t g = std::min<int64_t>((items + CC_THREADS - 1) / CC_THREADS, (int64_t)c->sm_count * 16);
-    return (int)std::max<int64_t>(g, 1);
-}
-
 // out[0..count) = exclusive prefix sums of in[0..count)
 template <class T>
 static int cc_exclusive_sum(gemb_ctx *c, const T *in, T *out, int64_t count) {
@@ -241,17 +236,15 @@ int gemb_cc_create(gemb_ctx *c, int64_t n, const int64_t *indptr, const int32_t 
     DeviceBuffer<unsigned long long> dred;   // [0] LCC key, [1] LCC stored edges
     CallEvents<2> ev;
     GEMB_CUDA(ev.create());
-    GEMB_CUDA(dptr.alloc((size_t)n + 1));
-    GEMB_CUDA(dix.alloc((size_t)std::max<int64_t>(nnz, 1)));
+    cudaStream_t st = c->stream;
+    GEMB_CUDA(dptr.upload(indptr, (size_t)n + 1, st));
+    GEMB_CUDA(dix.upload(indices, (size_t)nnz, st));
     GEMB_CUDA(parent.alloc((size_t)std::max<int64_t>(n, 1)));
     GEMB_CUDA(root.alloc((size_t)std::max<int64_t>(n, 1)));
     GEMB_CUDA(is_root.alloc((size_t)n + 1));
     GEMB_CUDA(comp.alloc((size_t)n + 1));
     GEMB_CUDA(size.alloc((size_t)std::max<int64_t>(n, 1)));
     GEMB_CUDA(dred.alloc(2));
-    cudaStream_t st = c->stream;
-    GEMB_CUDA(cudaMemcpyAsync(dptr.get(), indptr, sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, st));
-    if (nnz) GEMB_CUDA(cudaMemcpyAsync(dix.get(), indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, st));
     unsigned long long red[2] = {0, 0};
     int32_t n_comp = 0;
     GEMB_CUDA(cudaEventRecord(ev[0], st));
@@ -259,26 +252,16 @@ int gemb_cc_create(gemb_ctx *c, int64_t n, const int64_t *indptr, const int32_t 
         GEMB_CUDA(cudaMemsetAsync(size.get(), 0, sizeof(uint32_t) * (size_t)n, st));
         GEMB_CUDA(cudaMemsetAsync(is_root.get() + n, 0, sizeof(int32_t), st));
         GEMB_CUDA(cudaMemsetAsync(dred.get(), 0, 2 * sizeof(unsigned long long), st));
-        cc_init_kernel<<<cc_grid(c, n), CC_THREADS, 0, st>>>(n, parent.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-        if (nnz) {
-            cc_hook_kernel<<<(unsigned)((nnz + CC_TILE - 1) / CC_TILE), CC_THREADS, 0, st>>>(n, nnz, dptr.get(), dix.get(),
-                                                                                         parent.get());
-            GEMB_CUDA(cudaGetLastError());
-            count_launch();
-        }
-        cc_flatten_kernel<<<cc_grid(c, n), CC_THREADS, 0, st>>>(n, parent.get(), root.get(), is_root.get(), size.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-        cc_lcc_key_kernel<<<cc_grid(c, n), CC_THREADS, 0, st>>>(n, is_root.get(), size.get(), dred.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        const int grid = grid_stride(c, n, CC_THREADS, 16);
+        GEMB_TRY(launch(c, cc_init_kernel, grid, CC_THREADS, 0, n, parent.get()));
+        if (nnz)
+            GEMB_TRY(launch(c, cc_hook_kernel, (unsigned)((nnz + CC_TILE - 1) / CC_TILE), CC_THREADS, 0, n, nnz, dptr.get(),
+                            dix.get(), parent.get()));
+        GEMB_TRY(launch(c, cc_flatten_kernel, grid, CC_THREADS, 0, n, parent.get(), root.get(), is_root.get(), size.get()));
+        GEMB_TRY(launch(c, cc_lcc_key_kernel, grid, CC_THREADS, 0, n, is_root.get(), size.get(), dred.get()));
         GEMB_TRY(cc_exclusive_sum(c, is_root.get(), comp.get(), n + 1));
-        cc_relabel_kernel<<<cc_grid(c, n), CC_THREADS, 0, st>>>(n, dptr.get(), comp.get(), dred.get(), root.get(),
-                                                                dred.get() + 1);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, cc_relabel_kernel, grid, CC_THREADS, 0, n, dptr.get(), comp.get(), dred.get(), root.get(),
+                        dred.get() + 1));
         GEMB_CUDA(cudaMemcpyAsync(red, dred.get(), sizeof(red), cudaMemcpyDeviceToHost, st));
         GEMB_CUDA(cudaMemcpyAsync(&n_comp, comp.get() + n, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     }
@@ -286,10 +269,7 @@ int gemb_cc_create(gemb_ctx *c, int64_t n, const int64_t *indptr, const int32_t 
     GEMB_CUDA(cudaStreamSynchronize(st));
     const int64_t lcc_root = n ? (int64_t)(uint32_t)~(uint32_t)red[0] : -1;
     int32_t lcc_label = -1;   // the LCC's component number = the number of roots before its root
-    if (n) {
-        GEMB_CUDA(cudaMemcpyAsync(&lcc_label, comp.get() + lcc_root, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
-    }
+    if (n) GEMB_TRY(copy_sync(c, &lcc_label, comp.get() + lcc_root, sizeof(int32_t), cudaMemcpyDeviceToHost));
     gemb_cc *r = new gemb_cc();
     r->ctx = c; r->n = n; r->nnz = nnz;
     r->n_comp = n_comp;
@@ -336,9 +316,7 @@ int gemb_cc_labels(gemb_cc *r, int32_t *comp_out) {
     if (r->n == 0) return GEMB_OK;
     gemb_ctx *c = r->ctx;
     GEMB_CUDA(cudaSetDevice(c->device));
-    GEMB_CUDA(cudaMemcpyAsync(comp_out, r->labels, sizeof(int32_t) * (size_t)r->n, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+    return copy_sync(c, comp_out, r->labels, sizeof(int32_t) * (size_t)r->n, cudaMemcpyDeviceToHost);
 }
 
 int gemb_cc_lcc(gemb_cc *r, const double *data, int64_t *node_l_out, int64_t *indptr_out, int32_t *indices_out,
@@ -366,28 +344,21 @@ int gemb_cc_lcc(gemb_cc *r, const double *data, int64_t *node_l_out, int64_t *in
     GEMB_CUDA(oix.alloc((size_t)std::max<int64_t>(m, 1)));
     const bool weighted = data && m;
     if (weighted) {
-        GEMB_CUDA(ddata.alloc((size_t)r->nnz));
+        GEMB_CUDA(ddata.upload(data, (size_t)r->nnz, st));
         GEMB_CUDA(odata.alloc((size_t)m));
-        GEMB_CUDA(cudaMemcpyAsync(ddata.get(), data, sizeof(double) * (size_t)r->nnz, cudaMemcpyHostToDevice, st));
     }
     GEMB_CUDA(cudaEventRecord(ev[0], st));
-    cc_member_kernel<<<cc_grid(c, n + 1), CC_THREADS, 0, st>>>(n, r->labels, r->lcc_label, in_lcc.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, cc_member_kernel, grid_stride(c, n + 1, CC_THREADS, 16), CC_THREADS, 0, n, r->labels, r->lcc_label,
+                    in_lcc.get()));
     GEMB_TRY(cc_exclusive_sum(c, in_lcc.get(), new_id.get(), n + 1));
     GEMB_CUDA(cudaMemsetAsync(deg.get() + k, 0, sizeof(int64_t), st));
-    cc_keep_rows_kernel<<<cc_grid(c, n), CC_THREADS, 0, st>>>(n, r->indptr, in_lcc.get(), new_id.get(), node_l.get(),
-                                                              deg.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, cc_keep_rows_kernel, grid_stride(c, n, CC_THREADS, 16), CC_THREADS, 0, n, r->indptr, in_lcc.get(),
+                    new_id.get(), node_l.get(), deg.get()));
     GEMB_TRY(cc_exclusive_sum(c, deg.get(), optr.get(), k + 1));
-    if (m) {
-        cc_gather_kernel<<<(unsigned)((m + CC_TILE - 1) / CC_TILE), CC_THREADS, 0, st>>>(
-            k, m, optr.get(), node_l.get(), r->indptr, r->indices, new_id.get(), weighted ? ddata.get() : nullptr,
-            oix.get(), odata.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
+    if (m)
+        GEMB_TRY(launch(c, cc_gather_kernel, (unsigned)((m + CC_TILE - 1) / CC_TILE), CC_THREADS, 0, k, m, optr.get(),
+                        node_l.get(), r->indptr, r->indices, new_id.get(), weighted ? ddata.get() : nullptr, oix.get(),
+                        odata.get()));
     GEMB_CUDA(cudaEventRecord(ev[1], st));
     GEMB_CUDA(cudaMemcpyAsync(node_l_out, node_l.get(), sizeof(int64_t) * (size_t)k, cudaMemcpyDeviceToHost, st));
     GEMB_CUDA(cudaMemcpyAsync(indptr_out, optr.get(), sizeof(int64_t) * (size_t)(k + 1), cudaMemcpyDeviceToHost, st));

@@ -3,7 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <algorithm>
 #include <string>
+#include <utility>
 #include <vector>
 #include "../../include/gemb200.h"
 
@@ -66,6 +68,12 @@ template <class T> class DeviceBuffer {
     }
     ~DeviceBuffer() { reset(); }
     cudaError_t alloc(size_t count) { reset(); return dmalloc(&p_, sizeof(T) * count); }   // count 0: a minimal block
+    // alloc(count), then the copy of src[0, count) to the block on stream s (none when count is 0)
+    cudaError_t upload(const T *src, size_t count, cudaStream_t s) {
+        const cudaError_t e = alloc(count);
+        if (e != cudaSuccess || count == 0) return e;
+        return cudaMemcpyAsync(p_, src, sizeof(T) * count, cudaMemcpyHostToDevice, s);
+    }
     T *get() const { return p_; }
     T *release() { T *p = p_; p_ = nullptr; return p; }
     void reset() { dfree(p_); p_ = nullptr; }
@@ -193,6 +201,26 @@ struct gemb_graph {
 };
 
 namespace gemb {
+
+// ---- kernel launches.  Every kernel of this library is launched through `launch`: on ctx->stream as it is at the call
+//      (ritz_eigh swaps stream and side to run the Gram on the side stream), checked with GEMB_CUDA's rules and, when it
+//      was accepted, counted once (gemb_launch_count).  The kernel's parameters and the arguments are separate packs, so
+//      the arguments convert exactly as in a launch written out by hand.  Only the CUB calls count their own launches.
+int launch_status(const void *kernel);   // core.cu: cudaGetLastError() after a launch of `kernel`; counts it on success
+template <class... Params, class... Args>
+int launch(const gemb_ctx *ctx, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, Args &&...args) {
+    kernel<<<grid, block, smem, ctx->stream>>>(std::forward<Args>(args)...);
+    return launch_status((const void *)kernel);
+}
+
+// Grid of a grid-stride loop over `items` work items, `per_block` per CTA: enough CTAs for one pass, at least one, and at
+// most per_sm per SM.
+inline int grid_stride(const gemb_ctx *ctx, int64_t items, int64_t per_block, int per_sm) {
+    return (int)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, (int64_t)ctx->sm_count * per_sm));
+}
+
+// One copy on ctx->stream, then wait for the stream.
+int copy_sync(gemb_ctx *ctx, void *dst, const void *src, size_t bytes, cudaMemcpyKind kind);
 
 // ---- spmm.cu
 // The fused epilogue of one sweep:  Y = alpha * diag(rscale) * A * X + gamma * Xself + delta * X0 + eps * X1, and with

@@ -24,6 +24,25 @@ void set_error(const char *fmt, ...) {
     va_end(ap);
 }
 
+int launch_status(const void *kernel) {
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        count_launch();
+        return GEMB_OK;
+    }
+    const char *name = nullptr;
+    if (cudaFuncGetName(&name, kernel) != cudaSuccess || !name) name = "a kernel";
+    set_error("launch of %s failed: %s", name, cudaGetErrorString(e));
+    (void)cudaGetLastError();   // clear a non-sticky error for later calls
+    return GEMB_ERR_CUDA;
+}
+
+int copy_sync(gemb_ctx *ctx, void *dst, const void *src, size_t bytes, cudaMemcpyKind kind) {
+    GEMB_CUDA(cudaMemcpyAsync(dst, src, bytes, kind, ctx->stream));
+    GEMB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return GEMB_OK;
+}
+
 int Timer::begin(cudaStream_t s) {
     if (used + 2 > ev.size()) {
         size_t old = ev.size();
@@ -324,10 +343,8 @@ static int upload_csr(gemb_ctx *c, int64_t n, int64_t n_local, const int32_t *in
         int h = 0;
         GEMB_CUDA(flags.alloc(1));
         GEMB_CUDA(cudaMemsetAsync(flags.get(), 0, sizeof(int), c->stream));
-        csr_validate_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n_local, nnz, n, d->indptr, d->indices, flags.get());
-        count_launch();
-        GEMB_CUDA(cudaMemcpyAsync(&h, flags.get(), sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(launch(c, csr_validate_kernel, c->sm_count * 4, 256, 0, n_local, nnz, n, d->indptr, d->indices, flags.get()));
+        GEMB_TRY(copy_sync(c, &h, flags.get(), sizeof(int), cudaMemcpyDeviceToHost));
         if (h) {
             set_error("malformed CSR:%s%s", (h & 1) ? " row offsets are not monotone;" : "",
                       (h & 2) ? " a column id lies outside [0, n)" : "");

@@ -132,11 +132,7 @@ __global__ void __launch_bounds__(256) sum_partials_kernel(int parts, int64_t co
 
 int sum_partials_launch(gemb_ctx *ctx, int parts, int64_t count, const double *part, double *out) {
     if (count == 0) return GEMB_OK;
-    const int grid = (int)std::min<int64_t>((count + 31) / 32, (int64_t)ctx->sm_count * 16);
-    sum_partials_kernel<<<grid, dim3(32, 8), 0, ctx->stream>>>(parts, count, part, out);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, sum_partials_kernel, grid_stride(ctx, count, 32, 16), dim3(32, 8), 0, parts, count, part, out);
 }
 
 int gram_fp32_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const float *Q, int b2, double *G) {
@@ -155,14 +151,8 @@ int gram_fp32_launch(gemb_ctx *ctx, int64_t n, const float *P, int b1, const flo
     dim3 grid(gx, tiles_m * tiles_n), block(256);
     double *part = nullptr;
     GEMB_TRY(red_scratch(ctx, (size_t)gx * b1 * b2, &part));
-    switch (TM) {
-        case 4: gram_kernel<4><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
-        case 5: gram_kernel<5><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
-        case 6: gram_kernel<6><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
-        default: gram_kernel<8><<<grid, block, 0, ctx->stream>>>(n, P, b1, Q, b2, part, tiles_n); break;
-    }
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    const auto kernel = TM == 4 ? gram_kernel<4> : TM == 5 ? gram_kernel<5> : TM == 6 ? gram_kernel<6> : gram_kernel<8>;
+    GEMB_TRY(launch(ctx, kernel, grid, block, 0, n, P, b1, Q, b2, part, tiles_n));
     return sum_partials_launch(ctx, gx, (int64_t)b1 * b2, part, G);
 }
 
@@ -239,15 +229,8 @@ int apply_fp32_launch(gemb_ctx *ctx, int64_t n, const float *Q, int b1, const fl
     const int TN = pick_tm(b2);
     const int BN = 16 * TN;
     dim3 grid((unsigned)((n + 63) / 64), (b2 + BN - 1) / BN), block(256);
-    switch (TN) {
-        case 4: apply_kernel<4><<<grid, block, 0, ctx->stream>>>(n, Q, b1, M, ldm, b2, Out, ldo); break;
-        case 5: apply_kernel<5><<<grid, block, 0, ctx->stream>>>(n, Q, b1, M, ldm, b2, Out, ldo); break;
-        case 6: apply_kernel<6><<<grid, block, 0, ctx->stream>>>(n, Q, b1, M, ldm, b2, Out, ldo); break;
-        default: apply_kernel<8><<<grid, block, 0, ctx->stream>>>(n, Q, b1, M, ldm, b2, Out, ldo); break;
-    }
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    const auto kernel = TN == 4 ? apply_kernel<4> : TN == 5 ? apply_kernel<5> : TN == 6 ? apply_kernel<6> : apply_kernel<8>;
+    return launch(ctx, kernel, grid, block, 0, n, Q, b1, M, ldm, b2, Out, ldo);
 }
 
 // ------------------------------------------------------------------------------------ chol_inverse
@@ -361,11 +344,9 @@ int chol_inverse_launch(gemb_ctx *ctx, int b, double *G, float *Minv, int *rank_
         GEMB_CUDA(cudaFuncSetAttribute(chol_inverse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, v));
         optin = v;
     }
-    if (smem <= (size_t)optin) chol_inverse_kernel<true><<<1, 1024, smem, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
-    else chol_inverse_kernel<false><<<1, 1024, vecs, ctx->stream>>>(b, G, Minv, Minv64, rank_out_dev);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    const bool in_smem = smem <= (size_t)optin;
+    return launch(ctx, in_smem ? chol_inverse_kernel<true> : chol_inverse_kernel<false>, 1, 1024, in_smem ? smem : vecs,
+                  b, G, Minv, Minv64, rank_out_dev);
 }
 
 // ------------------------------------------------------------------------------------ eigh
@@ -550,12 +531,11 @@ int eigh_launch(gemb_ctx *ctx, int b, double *G, double *w, double *Z, double *Z
         GEMB_CUDA(cudaFuncSetAttribute(eigh_jacobi_kernel<JAC_ZT_GLOBAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap));
         attr_set = true;
     }
-    if (base + 2 * mat <= cap) eigh_jacobi_kernel<JAC_SHARED><<<1, 1024, base + 2 * mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
-    else if (base + mat <= cap) eigh_jacobi_kernel<JAC_ZT_GLOBAL><<<1, 1024, base + mat, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
-    else eigh_jacobi_kernel<JAC_GLOBAL><<<1, 1024, base, ctx->stream>>>(b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    auto kernel = eigh_jacobi_kernel<JAC_GLOBAL>;
+    size_t smem = base;
+    if (base + 2 * mat <= cap) { kernel = eigh_jacobi_kernel<JAC_SHARED>; smem = base + 2 * mat; }
+    else if (base + mat <= cap) { kernel = eigh_jacobi_kernel<JAC_ZT_GLOBAL>; smem = base + mat; }
+    return launch(ctx, kernel, 1, 1024, smem, b, G, w, Z, Zscratch, 30, rel_tol, symmetrize);
 }
 
 // ------------------------------------------------------------------------------------ small b x b products
@@ -574,10 +554,7 @@ small_gemm_kernel(int b, const double *__restrict__ A, int transA, const double 
 }
 
 int small_gemm_launch(gemb_ctx *ctx, int b, const double *A, int transA, const double *B, double *C, float *C32) {
-    small_gemm_kernel<<<1, 1024, 0, ctx->stream>>>(b, A, transA, B, C, C32);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, small_gemm_kernel, 1, 1024, 0, b, A, transA, B, C, C32);
 }
 
 // ------------------------------------------------------------------------------------ misc
@@ -604,10 +581,7 @@ __global__ void randn_kernel(int64_t n, int b, uint64_t seed, uint64_t row_offse
 int randn_launch(gemb_ctx *ctx, int64_t n, int b, uint64_t seed, uint64_t row_offset, float *X) {
     const int64_t tot = n * b;
     if (tot == 0) return GEMB_OK;
-    randn_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, ctx->stream>>>(n, b, seed, row_offset, X);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, randn_kernel, (unsigned)((tot + 255) / 256), 256, 0, n, b, seed, row_offset, X);
 }
 
 // block sums of squares -> part[blockIdx.x] (blockDim.x = 256)
@@ -634,13 +608,10 @@ int sumsq_launch(gemb_ctx *ctx, int64_t count, const float *X, double *out_dev) 
         GEMB_CUDA(cudaMemsetAsync(out_dev, 0, sizeof(double), ctx->stream));
         return GEMB_OK;
     }
-    int grid = ctx->sm_count * 8;
-    if ((int64_t)grid * 256 > count) grid = (int)((count + 255) / 256);
+    const int grid = grid_stride(ctx, count, 256, 8);
     double *part = nullptr;
     GEMB_TRY(red_scratch(ctx, (size_t)grid, &part));
-    sumsq_kernel<<<grid, 256, 0, ctx->stream>>>(count, X, part);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(ctx, sumsq_kernel, grid, 256, 0, count, X, part));
     return sum_partials_launch(ctx, grid, 1, part, out_dev);
 }
 
@@ -652,12 +623,7 @@ __global__ void scale_kernel(int64_t count, float s, float *__restrict__ X) {
 
 int scale_launch(gemb_ctx *ctx, int64_t count, float s, float *X) {
     if (count == 0) return GEMB_OK;
-    int grid = ctx->sm_count * 8;
-    if ((int64_t)grid * 256 > count) grid = (int)((count + 255) / 256);
-    scale_kernel<<<grid, 256, 0, ctx->stream>>>(count, s, X);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, scale_kernel, grid_stride(ctx, count, 256, 8), 256, 0, count, s, X);
 }
 
 // Y += a * X over count floats
@@ -667,10 +633,7 @@ __global__ void axpy_kernel(int64_t count, float a, const float *__restrict__ X,
 }
 
 int axpy_launch(gemb_ctx *ctx, int64_t count, float a, const float *X, float *Y) {
-    axpy_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(count, a, X, Y);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, axpy_kernel, ctx->sm_count * 8, 256, 0, count, a, X, Y);
 }
 
 }  // namespace gemb
@@ -682,12 +645,8 @@ extern "C" int gemb_gram(gemb_ctx *c, int64_t n, const float *P, int b1, const f
     GEMB_CUDA(cudaSetDevice(c->device));
     DeviceBuffer<float> dP, dQ;
     DeviceBuffer<double> dG;
-    GEMB_CUDA(dP.alloc((size_t)std::max<int64_t>(n, 1) * b1));
-    GEMB_CUDA(cudaMemcpyAsync(dP.get(), P, sizeof(float) * (size_t)n * b1, cudaMemcpyHostToDevice, c->stream));
-    if (Q) {
-        GEMB_CUDA(dQ.alloc((size_t)std::max<int64_t>(n, 1) * b2));
-        GEMB_CUDA(cudaMemcpyAsync(dQ.get(), Q, sizeof(float) * (size_t)n * b2, cudaMemcpyHostToDevice, c->stream));
-    }
+    GEMB_CUDA(dP.upload(P, (size_t)n * b1, c->stream));
+    if (Q) GEMB_CUDA(dQ.upload(Q, (size_t)n * b2, c->stream));
     GEMB_CUDA(dG.alloc((size_t)b1 * b2));
     const float *dQP = Q ? dQ.get() : dP.get();
     const int s = use_tensor_cores ? gram_tc_launch(c, n, dP.get(), b1, dQP, b2, dG.get())
@@ -711,11 +670,10 @@ extern "C" int gemb_chol_inverse(gemb_ctx *c, int b, const double *G, double *Mi
     DeviceBuffer<double> dG, dM64;
     DeviceBuffer<float> dM32;
     DeviceBuffer<int> dRank;
-    GEMB_CUDA(dG.alloc(bb));
+    GEMB_CUDA(dG.upload(G, bb, c->stream));
     GEMB_CUDA(dM64.alloc(bb));
     GEMB_CUDA(dM32.alloc(bb));
     GEMB_CUDA(dRank.alloc(1));
-    GEMB_CUDA(cudaMemcpyAsync(dG.get(), G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream));
     GEMB_TRY(chol_inverse_launch(c, b, dG.get(), dM32.get(), dRank.get(), dM64.get()));
     GEMB_CUDA(cudaMemcpyAsync(Minv64_out, dM64.get(), sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(Minv32_out, dM32.get(), sizeof(float) * bb, cudaMemcpyDeviceToHost, c->stream));
@@ -730,11 +688,10 @@ extern "C" int gemb_eigh(gemb_ctx *c, int b, const double *G, double rel_tol, do
     GEMB_CUDA(cudaSetDevice(c->device));
     const size_t bb = (size_t)b * b;
     DeviceBuffer<double> dG, dw, dZ, dZs;
-    GEMB_CUDA(dG.alloc(bb));
+    GEMB_CUDA(dG.upload(G, bb, c->stream));
     GEMB_CUDA(dw.alloc(b));
     GEMB_CUDA(dZ.alloc(bb));
     GEMB_CUDA(dZs.alloc(bb));
-    GEMB_CUDA(cudaMemcpyAsync(dG.get(), G, sizeof(double) * bb, cudaMemcpyHostToDevice, c->stream));
     GEMB_TRY(eigh_launch(c, b, dG.get(), dw.get(), dZ.get(), dZs.get(), rel_tol));
     GEMB_CUDA(cudaMemcpyAsync(w_out, dw.get(), sizeof(double) * b, cudaMemcpyDeviceToHost, c->stream));
     GEMB_CUDA(cudaMemcpyAsync(Z_out, dZ.get(), sizeof(double) * bb, cudaMemcpyDeviceToHost, c->stream));
@@ -748,11 +705,9 @@ extern "C" int gemb_apply(gemb_ctx *c, int64_t n, const float *Q, int b1, const 
     GEMB_ARG(c && Q && M && Out && n >= 0 && b1 > 0 && b2 > 0, "ctx/Q/M/Out/n/b");
     GEMB_CUDA(cudaSetDevice(c->device));
     DeviceBuffer<float> dQ, dM, dO;
-    GEMB_CUDA(dQ.alloc((size_t)std::max<int64_t>(n, 1) * b1));
-    GEMB_CUDA(dM.alloc((size_t)b1 * b2));
+    GEMB_CUDA(dQ.upload(Q, (size_t)n * b1, c->stream));
+    GEMB_CUDA(dM.upload(M, (size_t)b1 * b2, c->stream));
     GEMB_CUDA(dO.alloc((size_t)std::max<int64_t>(n, 1) * b2));
-    GEMB_CUDA(cudaMemcpyAsync(dQ.get(), Q, sizeof(float) * (size_t)n * b1, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(dM.get(), M, sizeof(float) * (size_t)b1 * b2, cudaMemcpyHostToDevice, c->stream));
     const int s = use_tensor_cores ? apply_tc_launch(c, n, dQ.get(), b1, dM.get(), b2, b2, dO.get(), b2)
                                    : apply_fp32_launch(c, n, dQ.get(), b1, dM.get(), b2, b2, dO.get(), b2);
     if (s == GEMB_ERR_UNSUPPORTED) set_error("gemb_apply: shape (n=%lld, b1=%d, b2=%d) not supported by the tensor-core kernel", (long long)n, b1, b2);

@@ -93,53 +93,40 @@ extern "C" int gemb_gf(gemb_ctx *ctx, int64_t n, int64_t m, const int32_t *src, 
     DeviceBuffer<float> d_w, Xa, Xb;
     DeviceBuffer<int64_t> d_rp;
     const size_t xb = sizeof(float) * (size_t)n * d;
-    GEMB_CUDA(d_dst.alloc(std::max<int64_t>(m, 1)));
-    GEMB_CUDA(cudaMemcpyAsync(d_dst.get(), dst, sizeof(int32_t) * m, cudaMemcpyHostToDevice, st));
-    if (w) { GEMB_CUDA(d_w.alloc(std::max<int64_t>(m, 1))); GEMB_CUDA(cudaMemcpyAsync(d_w.get(), w, sizeof(float) * m, cudaMemcpyHostToDevice, st)); }
-    GEMB_CUDA(Xa.alloc((size_t)n * d));
-    GEMB_CUDA(cudaMemcpyAsync(Xa.get(), X0, xb, cudaMemcpyHostToDevice, st));
+    GEMB_CUDA(d_dst.upload(dst, m, st));
+    if (w) GEMB_CUDA(d_w.upload(w, m, st));
+    GEMB_CUDA(Xa.upload(X0, (size_t)n * d, st));
     if (mode == 0) {
-        GEMB_CUDA(d_src.alloc(std::max<int64_t>(m, 1)));
-        GEMB_CUDA(cudaMemcpyAsync(d_src.get(), src, sizeof(int32_t) * m, cudaMemcpyHostToDevice, st));
+        GEMB_CUDA(d_src.upload(src, m, st));
     } else {
         rowptr.assign(n + 1, 0);
         for (int64_t e = 0; e < m; e++) rowptr[src[e] + 1]++;
         for (int64_t i = 0; i < n; i++) rowptr[i + 1] += rowptr[i];
-        GEMB_CUDA(d_rp.alloc(n + 1));
-        GEMB_CUDA(cudaMemcpyAsync(d_rp.get(), rowptr.data(), sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice, st));
+        GEMB_CUDA(d_rp.upload(rowptr.data(), n + 1, st));
         GEMB_CUDA(Xb.alloc((size_t)n * d));
     }
     CallEvents<2> ev;
     GEMB_CUDA(ev.create());
     GEMB_CUDA(cudaEventRecord(ev[0], st));
-    const int nv = (d + 31) / 32;
+    int vi = 0;                                   // the instantiation: NV = 2^vi >= ceil(d / 32)
+    while ((32 << vi) < d) vi++;
     float *cur = Xa.get();
-#define GF_DISPATCH(CALL)                                                                     \
-    do {                                                                                      \
-        if (nv <= 1) { CALL(1); } else if (nv <= 2) { CALL(2); } else if (nv <= 4) { CALL(4); } \
-        else if (nv <= 8) { CALL(8); } else if (nv <= 16) { CALL(16); } else { CALL(32); } \
-    } while (0)
     if (mode == 0) {
         if (m > 0 && max_iter > 0) {
-#define SEQ(NV) gf_sequential_kernel<NV><<<1, 32, 0, st>>>(m, d_src.get(), d_dst.get(), d_w.get(), d, eta, regu, max_iter, Xa.get())
-            GF_DISPATCH(SEQ);
-#undef SEQ
-            GEMB_CUDA(cudaGetLastError());
-            count_launch();
+            decltype(&gf_sequential_kernel<1>) const seq[] = {gf_sequential_kernel<1>, gf_sequential_kernel<2>, gf_sequential_kernel<4>,
+                                                              gf_sequential_kernel<8>, gf_sequential_kernel<16>, gf_sequential_kernel<32>};
+            GEMB_TRY(launch(ctx, seq[vi], 1, 32, 0, m, d_src.get(), d_dst.get(), d_w.get(), d, eta, regu, max_iter, Xa.get()));
         }
     } else {
-        const int grid = (int)std::min<int64_t>((n * 32 + 255) / 256, (int64_t)ctx->sm_count * 16);
+        decltype(&gf_rows_kernel<1>) const rows[] = {gf_rows_kernel<1>, gf_rows_kernel<2>, gf_rows_kernel<4>,
+                                                     gf_rows_kernel<8>, gf_rows_kernel<16>, gf_rows_kernel<32>};
+        const int grid = grid_stride(ctx, n * 32, 256, 16);
         float *nxt = Xb.get();
         for (int ep = 0; ep < max_iter; ep++) {
-#define ROWS(NV) gf_rows_kernel<NV><<<grid, 256, 0, st>>>(n, d_rp.get(), d_dst.get(), d_w.get(), d, eta, regu, cur, nxt)
-            GF_DISPATCH(ROWS);
-#undef ROWS
+            GEMB_TRY(launch(ctx, rows[vi], grid, 256, 0, n, d_rp.get(), d_dst.get(), d_w.get(), d, eta, regu, cur, nxt));
             std::swap(cur, nxt);
         }
-        GEMB_CUDA(cudaGetLastError());
-        count_launch(max_iter);
     }
-#undef GF_DISPATCH
     GEMB_CUDA(cudaEventRecord(ev[1], st));
     GEMB_CUDA(cudaMemcpyAsync(X_out, cur, xb, cudaMemcpyDeviceToHost, st));
     GEMB_CUDA(cudaStreamSynchronize(st));

@@ -190,10 +190,7 @@ static int gram_tc_launch_t(gemb_ctx *ctx, const GramTcParams &p, int grid, size
         GEMB_CUDA(cudaFuncSetAttribute(gram_tc_kernel<QRAW, BSEP, NPAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
         attr_bytes = smem_bytes;
     }
-    gram_tc_kernel<QRAW, BSEP, NPAD><<<grid, 384, smem_bytes, ctx->stream>>>(p);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(ctx, gram_tc_kernel<QRAW, BSEP, NPAD>, grid, 384, smem_bytes, p);
 }
 
 template <bool QRAW, bool BSEP>

@@ -78,12 +78,10 @@ static int ipc_exchange(gemb_ctx *c, void *const *mine, int count, void **peers 
     for (int i = 0; i < count; i++) GEMB_CUDA(cudaIpcGetMemHandle(&h[i], mine[i]));
     DeviceBuffer<char> dsend, drecv;
     const size_t bytes = sizeof(cudaIpcMemHandle_t) * count;
-    GEMB_CUDA(dsend.alloc(bytes));
+    GEMB_CUDA(dsend.upload((const char *)h.data(), bytes, c->stream));
     GEMB_CUDA(drecv.alloc(bytes * P));
-    GEMB_CUDA(cudaMemcpyAsync(dsend.get(), h.data(), bytes, cudaMemcpyHostToDevice, c->stream));
     NCCL_TRY(api->AllGather(dsend.get(), drecv.get(), bytes, ncclChar, (ncclComm_t)c->comm, c->stream), "ncclAllGather(ipc handles)");
-    GEMB_CUDA(cudaMemcpyAsync(all.data(), drecv.get(), bytes * P, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, all.data(), drecv.get(), bytes * P, cudaMemcpyDeviceToHost));
     dsend.reset(); drecv.reset();
     for (int i = 0; i < count; i++)
         for (int q = 0; q < P; q++) {
@@ -137,13 +135,11 @@ static int halo_plan(gemb_graph *g, NcclApi *api) {
     long long n_rem = 0, n_H = 0;
     if (nnz > 0) {
         GEMB_CUDA(cub::DeviceSelect::If(tmp.get(), tb, g->A.indices, rem.get(), d_num.get(), nnz, pred, st));
-        GEMB_CUDA(cudaMemcpyAsync(&n_rem, d_num.get(), sizeof n_rem, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
+        GEMB_TRY(copy_sync(c, &n_rem, d_num.get(), sizeof n_rem, cudaMemcpyDeviceToHost));
         if (n_rem > 0) {
             GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.get(), tb, rem.get(), rem_sorted.get(), n_rem, 0, 32, st));
             GEMB_CUDA(cub::DeviceSelect::Unique(tmp.get(), tb, rem_sorted.get(), Hd.get(), d_num.get(), n_rem, st));
-            GEMB_CUDA(cudaMemcpyAsync(&n_H, d_num.get(), sizeof n_H, cudaMemcpyDeviceToHost, st));
-            GEMB_CUDA(cudaStreamSynchronize(st));
+            GEMB_TRY(copy_sync(c, &n_H, d_num.get(), sizeof n_H, cudaMemcpyDeviceToHost));
         }
     }
     count_launch(3);
@@ -152,19 +148,16 @@ static int halo_plan(gemb_graph *g, NcclApi *api) {
 
     // ---- remapped column ids
     GEMB_CUDA(dmalloc(&H.indices_ext, sizeof(int32_t) * (std::max<int64_t>(nnz, 1) + 4)));   // + the x4 padding the bulk copies of spmm.cu read
-    if (nnz > 0) {
-        halo_remap_kernel<<<c->sm_count * 8, 256, 0, st>>>(nnz, g->A.indices, lo, hi, Hd.get(), n_H, (int32_t)g->n_shard, H.indices_ext);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
+    if (nnz > 0)
+        GEMB_TRY(launch(c, halo_remap_kernel, c->sm_count * 8, 256, 0, nnz, g->A.indices, lo, hi, Hd.get(), n_H, (int32_t)g->n_shard,
+                        H.indices_ext));
 
     // ---- everyone's halo lists -> who needs my rows
     long long *d_cnt_all = d_num.get() + 2;                 // [P]
     long long h_cnt_all[GEMB_MAX_RANKS];
     GEMB_CUDA(cudaMemcpyAsync(d_num.get(), &n_H, sizeof n_H, cudaMemcpyHostToDevice, st));
     NCCL_TRY(api->AllGather(d_num.get(), d_cnt_all, 1, ncclInt64, (ncclComm_t)c->comm, st), "ncclAllGather(halo counts)");
-    GEMB_CUDA(cudaMemcpyAsync(h_cnt_all, d_cnt_all, sizeof(long long) * P, cudaMemcpyDeviceToHost, st));
-    GEMB_CUDA(cudaStreamSynchronize(st));
+    GEMB_TRY(copy_sync(c, h_cnt_all, d_cnt_all, sizeof(long long) * P, cudaMemcpyDeviceToHost));
     long long maxH = 1;
     for (int q = 0; q < P; q++) maxH = std::max(maxH, h_cnt_all[q]);
     DeviceBuffer<int32_t> Hpad, Hall;
@@ -175,12 +168,9 @@ static int halo_plan(gemb_graph *g, NcclApi *api) {
     NCCL_TRY(api->AllGather(Hpad.get(), Hall.get(), (size_t)maxH, ncclInt32, (ncclComm_t)c->comm, st), "ncclAllGather(halo lists)");
     DeviceBuffer<long long> seg_dev;
     GEMB_CUDA(seg_dev.alloc(2 * GEMB_MAX_RANKS));
-    halo_segments_kernel<<<1, 32, 0, st>>>(P, Hall.get(), maxH, d_cnt_all, lo, hi, seg_dev.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, halo_segments_kernel, 1, 32, 0, P, Hall.get(), maxH, d_cnt_all, lo, hi, seg_dev.get()));
     long long seg[2 * GEMB_MAX_RANKS];
-    GEMB_CUDA(cudaMemcpyAsync(seg, seg_dev.get(), sizeof(long long) * 2 * P, cudaMemcpyDeviceToHost, st));
-    GEMB_CUDA(cudaStreamSynchronize(st));
+    GEMB_TRY(copy_sync(c, seg, seg_dev.get(), sizeof(long long) * 2 * P, cudaMemcpyDeviceToHost));
 
     DeviceBuffer<int32_t> cnt;
     const int64_t nl = g->n_local;
@@ -193,10 +183,8 @@ static int halo_plan(gemb_graph *g, NcclApi *api) {
         const long long m = seg[2 * q + 1] - seg[2 * q];
         total += m;
         if (m <= 0) continue;
-        const int grid = (int)std::min<long long>((m + 255) / 256, c->sm_count * 8);
-        halo_pushlist_kernel<0><<<grid, 256, 0, st>>>(q, Hall.get() + (int64_t)q * maxH, seg[2 * q], seg[2 * q + 1], lo, cnt.get(), nullptr, nullptr);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, halo_pushlist_kernel<0>, grid_stride(c, m, 256, 8), 256, 0, q, Hall.get() + (int64_t)q * maxH, seg[2 * q],
+                        seg[2 * q + 1], lo, cnt.get(), nullptr, nullptr));
     }
     GEMB_ARG(total < ((long long)1 << 31), "push list too long");
     H.push_total = total;
@@ -211,10 +199,8 @@ static int halo_plan(gemb_graph *g, NcclApi *api) {
         if (q == c->rank) continue;
         const long long m = seg[2 * q + 1] - seg[2 * q];
         if (m <= 0) continue;
-        const int grid = (int)std::min<long long>((m + 255) / 256, c->sm_count * 8);
-        halo_pushlist_kernel<1><<<grid, 256, 0, st>>>(q, Hall.get() + (int64_t)q * maxH, seg[2 * q], seg[2 * q + 1], lo, cnt.get(), H.push_ptr, H.push_dst);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, halo_pushlist_kernel<1>, grid_stride(c, m, 256, 8), 256, 0, q, Hall.get() + (int64_t)q * maxH, seg[2 * q],
+                        seg[2 * q + 1], lo, cnt.get(), H.push_ptr, H.push_dst));
     }
     GEMB_CUDA(cudaStreamSynchronize(st));
     return GEMB_OK;
@@ -279,11 +265,9 @@ int halo_buffers(gemb_graph *g, int nbuf, int width) {
     // of the need, so every rank takes the same branch
     long long need = (long long)(rows * (size_t)width);
     DeviceBuffer<long long> d_need;
-    GEMB_CUDA(d_need.alloc(1));
-    GEMB_CUDA(cudaMemcpyAsync(d_need.get(), &need, sizeof need, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(d_need.upload(&need, 1, c->stream));
     NCCL_TRY(api->AllReduce(d_need.get(), d_need.get(), 1, ncclInt64, ncclMax, (ncclComm_t)c->comm, c->stream), "ncclAllReduce(halo block size)");
-    GEMB_CUDA(cudaMemcpyAsync(&need, d_need.get(), sizeof need, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, &need, d_need.get(), sizeof need, cudaMemcpyDeviceToHost));
     d_need.reset();
     if (PL.nbuf < nbuf || PL.cap_floats < (size_t)need) {
         GEMB_TRY(halo_pool_drop_blocks(c));
@@ -347,10 +331,8 @@ int halo_push_launch(gemb_graph *g, int bi, int width) {
     const int rpc = 256 / G;
     HaloPushArgs P;
     halo_push_args(g, bi, &P);
-    halo_push_kernel<<<(unsigned)((g->n_local + rpc - 1) / rpc), 256, 0, c->stream>>>(g->n_local, G, rpc, (const float4 *)g->halo.buf[bi], P);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(c, halo_push_kernel, (unsigned)((g->n_local + rpc - 1) / rpc), 256, 0, g->n_local, G, rpc,
+                  (const float4 *)g->halo.buf[bi], P);
 }
 
 struct BarrierArgs {
@@ -381,18 +363,14 @@ int halo_barrier(gemb_graph *g) {
     BarrierArgs A;
     for (int q = 0; q < GEMB_MAX_RANKS; q++) A.peer[q] = H.peer_flags[q];
     c->halo_pool.epoch++;
-    halo_barrier_kernel<<<1, 32, 0, c->stream>>>(A, H.flags, c->halo_pool.epoch, c->rank, c->nranks, H.timeout_flag);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(c, halo_barrier_kernel, 1, 32, 0, A, H.flags, c->halo_pool.epoch, c->rank, c->nranks, H.timeout_flag);
 }
 
 int halo_check_timeout(gemb_graph *g) {
     gemb_halo &H = g->halo;
     if (!H.ready) return GEMB_OK;
     int h = 0;
-    GEMB_CUDA(cudaMemcpyAsync(&h, H.timeout_flag, sizeof h, cudaMemcpyDeviceToHost, g->ctx->stream));
-    GEMB_CUDA(cudaStreamSynchronize(g->ctx->stream));
+    GEMB_TRY(copy_sync(g->ctx, &h, H.timeout_flag, sizeof h, cudaMemcpyDeviceToHost));
     if (h) {
         set_error("multi-GPU HOPE: a peer did not reach the sweep barrier within 2 s (rank %d of %d)", g->ctx->rank, g->ctx->nranks);
         return GEMB_ERR_NCCL;

@@ -98,12 +98,6 @@ struct HopeResult {
 };
 
 // host <-> device staging: the copy, then a stream synchronise (the host reads the result, or its buffer goes out of scope)
-static int copy_sync(gemb_ctx *c, void *dst, const void *src, size_t bytes, cudaMemcpyKind kind) {
-    GEMB_CUDA(cudaMemcpyAsync(dst, src, bytes, kind, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
-}
-
 // the width-4 probes (norm estimate, Katz series probe) leave their vectors in work blocks 2..4: zero them again, as
 // alloc_blocks left them
 static int clear_scratch(HopeWork &W) {
@@ -285,8 +279,7 @@ static int cholqr2(HopeWork &W, const float *src, float *tmp, float *dst) {
 
 // M1[i][j] = Z[i][b-k+j] * theta_j^(p1),  M2 likewise with p2   (theta ascending, top k)
 __global__ void ritz_maps_kernel(int b, int k, const double *__restrict__ w, const double *__restrict__ Z,
-                                 float *__restrict__ M1, float *__restrict__ M2, double p1, double p2,
-                                 double rel_floor = 1e-28) {
+                                 float *__restrict__ M1, float *__restrict__ M2, double p1, double p2, double rel_floor) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= b * k) return;
     const int i = idx / k, j = idx - i * k;
@@ -368,21 +361,14 @@ static int axpby_launch(HopeWork &W, float a, const float *P, float c, const flo
         GEMB_ARG(bo >= 0 && G <= 256, "axpby output is not a work block");
         HaloPushArgs H;
         halo_push_args(W.g, bo, &H);
-        if (W.rows > 0) {
-            axpby_push_kernel<<<(unsigned)((W.rows + rpc - 1) / rpc), 256, 0, W.c->stream>>>(
-                W.rows, G, rpc, a, (const float4 *)P, c, (const float4 *)Q, (float4 *)Y, H);
-            GEMB_CUDA(cudaGetLastError());
-            count_launch();
-        }
+        if (W.rows > 0)
+            GEMB_TRY(launch(W.c, axpby_push_kernel, (unsigned)((W.rows + rpc - 1) / rpc), 256, 0, W.rows, G, rpc, a, (const float4 *)P,
+                            c, (const float4 *)Q, (float4 *)Y, H));
         return end_push(W, W.b);
     }
     if (count == 0) return GEMB_OK;
-    int grid = W.c->sm_count * 8;
-    if ((int64_t)grid * 256 > count) grid = (int)((count + 255) / 256);
-    axpby_kernel<<<grid, 256, 0, W.c->stream>>>(count, a, (const float4 *)P, c, (const float4 *)Q, (float4 *)Y);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(W.c, axpby_kernel, grid_stride(W.c, count, 256, 8), 256, 0, count, a, (const float4 *)P, c, (const float4 *)Q,
+                  (float4 *)Y);
 }
 
 // out[0] = max_i sum_j |a_ij| (= ||A||_inf), out[1] = max(0, -min_ij a_ij)  (0 <=> all weights >= 0)
@@ -423,23 +409,15 @@ static int inv_degree(HopeWork &W) {
     gemb_ctx *c = W.c;
     GEMB_CUDA(W.rscale.alloc((size_t)std::max<int64_t>(W.rows, 1)));
     if (W.rows == 0) return GEMB_OK;
-    const int grid = (int)std::min<int64_t>((W.rows + 255) / 256, (int64_t)c->sm_count * 8);
-    inv_degree_kernel<<<grid, 256, 0, c->stream>>>(W.rows, W.g->A.indptr, W.g->A.data, W.g->AT.indptr, W.g->AT.data,
-                                                   W.rscale.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(c, inv_degree_kernel, grid_stride(c, W.rows, 256, 8), 256, 0, W.rows, W.g->A.indptr, W.g->A.data, W.g->AT.indptr,
+                  W.g->AT.data, W.rscale.get());
 }
 
 // ||A||_inf and the sign of the weights in one pass over the CSR shard
 static int rowsum_bound(HopeWork &W, double *norm_inf, bool *nonneg) {
     gemb_ctx *c = W.c;
     GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, 2 * sizeof(double), c->stream));
-    if (W.rows > 0) {
-        csr_rowsum_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(W.rows, W.g->A.indptr, W.g->A.data, W.scal.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
+    if (W.rows > 0) GEMB_TRY(launch(c, csr_rowsum_kernel, c->sm_count * 8, 256, 0, W.rows, W.g->A.indptr, W.g->A.data, W.scal.get()));
     GEMB_TRY(comm_allreduce(W, W.scal.get(), 2, ncclDouble, ncclMax, false, "ncclAllReduce(max)"));
     double h[2];
     GEMB_TRY(copy_sync(c, h, W.scal.get(), sizeof h, cudaMemcpyDeviceToHost));
@@ -583,9 +561,7 @@ static int residual_check(HopeWork &W, float beta, int J, const float *P, const 
     GEMB_TRY(apply_S(W, true, beta, J, P, scr0, scr1, scr2));    // scr0 = S^T P
     GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, sizeof(double) * b, c->stream));
     const int threads = (256 / b) * b > 0 ? (256 / b) * b : b;
-    coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(W.rows, b, scr0, Qs, W.scal.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, coldiff_sumsq_kernel, c->sm_count * 4, threads, 0, W.rows, b, scr0, Qs, W.scal.get()));
     GEMB_TRY(comm_allreduce(W, W.scal.get(), b));
     std::vector<double> rs(b);
     GEMB_TRY(copy_sync(c, rs.data(), W.scal.get(), sizeof(double) * b, cudaMemcpyDeviceToHost));
@@ -619,9 +595,7 @@ static int ritz_eigh(HopeWork &W, float tol, bool symmetrize, std::vector<double
         GEMB_CUDA(cudaEventRecord(W.fork_join[1], c->side));
         GEMB_CUDA(cudaStreamWaitEvent(c->stream, W.fork_join[1], 0));
         GEMB_TRY(comm_allreduce(W, W.G.get(), (size_t)b * b));
-        ritz_quadform_kernel<<<b, 128, sizeof(double) * b, c->stream>>>(b, W.G.get(), W.Z.get(), W.w.get() + b);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, ritz_quadform_kernel, b, 128, sizeof(double) * b, b, W.G.get(), W.Z.get(), W.w.get() + b));
     }
     GEMB_TRY(c->t_dense.end(c->stream));
     return copy_sync(c, lam.data(), W.w.get(), sizeof(double) * (AV ? 2 * b : b), cudaMemcpyDeviceToHost);
@@ -686,9 +660,8 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
         // T1 = U Z Theta^-1/2: exactly orthonormal columns (Z diagonalises U^T U), ordered by sigma, so the
         // next block S^T T1 ~ V Z Sigma has nearly orthogonal columns whatever the spread of sigma is
         GEMB_TRY(c->t_dense.begin(c->stream));
-        ritz_maps_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, b, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.5, 0.5, 1e-10);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, ritz_maps_kernel, (b * b + 255) / 256, 256, 0, b, b, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.5, 0.5,
+                        1e-10));
         GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), b, b, T1, b));
         GEMB_TRY(c->t_dense.end(c->stream));
         GEMB_TRY(apply_S(W, true, beta, J, T1, Wk, Hscr, T2));        // Wk = S^T T1   (stop_rule 0: U is scratch now)
@@ -716,21 +689,17 @@ static int hope_general(HopeWork &W, const Opts &o, int d, float beta, int J, Ho
     // extraction: X = [U Z_k theta^-1/4 | V Z_k theta^1/4]; U = S V (un-normalised), V orthonormal
     GEMB_TRY(place_output(W, R, T1, d));
     GEMB_TRY(c->t_dense.begin(c->stream));
-    ritz_maps_kernel<<<(b * k + 255) / 256, 256, 0, c->stream>>>(b, k, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.25, 0.25);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, ritz_maps_kernel, (b * k + 255) / 256, 256, 0, b, k, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.25,
+                    0.25, 1e-28));
     GEMB_TRY(apply_launch(c, W.rows, U, b, W.M1.get(), k, k, R.Xd, d));
     GEMB_TRY(apply_launch(c, W.rows, V, b, W.M2.get(), k, k, R.Xd + k, d));
-    sqrt_top_kernel<<<(k + 127) / 128, 128, 0, c->stream>>>(b, k, W.w.get(), R.sig_dev);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, sqrt_top_kernel, (k + 127) / 128, 128, 0, b, k, W.w.get(), R.sig_dev));
     GEMB_TRY(c->t_dense.end(c->stream));
 
     if (o.compute_residual) {
         // left vectors P = U Z theta^-1/2 (all b Ritz pairs), right Q sigma = V Z theta^1/2
-        ritz_maps_kernel<<<(b * b + 255) / 256, 256, 0, c->stream>>>(b, b, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.5, 0.5);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, ritz_maps_kernel, (b * b + 255) / 256, 256, 0, b, b, W.w.get(), W.Z.get(), W.M1.get(), W.M2.get(), -0.5,
+                        0.5, 1e-28));
         float *Pm = Wk, *Qs = T1;
         const size_t blk = (size_t)W.shard * b;
         DeviceBuffer<float> Qalloc, STP;
@@ -792,12 +761,7 @@ static int refill_dropped(HopeWork &W, float *V, float *s1, float *s2, uint64_t 
     GEMB_TRY(randn_launch(c, W.rows, b, seed, (uint64_t)W.g->row0, s1));
     GEMB_TRY(gram_full(W, V, V, W.G.get()));
     const int64_t count = W.rows * (int64_t)b;
-    if (count > 0) {
-        const int grid = (int)std::min<int64_t>((count + 255) / 256, (int64_t)c->sm_count * 8);
-        refill_cols_kernel<<<grid, 256, 0, c->stream>>>(count, b, W.G.get(), s1, V);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
+    if (count > 0) GEMB_TRY(launch(c, refill_cols_kernel, grid_stride(c, count, 256, 8), 256, 0, count, b, W.G.get(), s1, V));
     GEMB_TRY(gram_full(W, V, V, W.G.get()));
     GEMB_TRY(cholqr_pass(W, W.G.get(), V, s2));
     GEMB_TRY(gram_full(W, s2, s2, W.G.get()));
@@ -1101,8 +1065,8 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map,
     }
     DeviceBuffer<float> dMP, dMQ, Palloc, Q, STP;
     const size_t blk = (size_t)W.shard * b;
-    GEMB_CUDA(dMP.alloc(b * b));
-    GEMB_CUDA(dMQ.alloc(b * b));
+    GEMB_CUDA(dMP.upload(MP.data(), b * b, c->stream));
+    GEMB_CUDA(dMQ.upload(MQ.data(), b * b, c->stream));
     // every SpMM INPUT must be a work block in halo mode (its rows travel to the peers): P lives in AV, the Horner
     // scratch in pool[1] / pool[2]; pool[0] may hold the result X and stays untouched
     float *P = AV;
@@ -1115,8 +1079,6 @@ static int hope_symmetric(HopeWork &W, const Opts &o, int d, int k, SpecMap map,
     GEMB_CUDA(STP.alloc(blk));
     GEMB_CUDA(cudaMemsetAsync(Q.get(), 0, sizeof(float) * blk, c->stream));
     GEMB_CUDA(cudaMemsetAsync(STP.get(), 0, sizeof(float) * blk, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(dMP.get(), MP.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(dMQ.get(), MQ.data(), sizeof(float) * b * b, cudaMemcpyHostToDevice, c->stream));
     GEMB_TRY(apply_launch(c, W.rows, V, b, dMP.get(), b, b, P, b));
     GEMB_TRY(apply_launch(c, W.rows, V, b, dMQ.get(), b, b, Q.get(), b));
     GEMB_TRY(publish(W, P, b));
@@ -1238,9 +1200,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
     bool done = false;
     while (!done) {
         // ---- append q_j, expand
-        put_cols_kernel<<<grid_el, 256, 0, c->stream>>>(rows, p, Vcur, Q[m / cw].get(), cw, m % cw);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, put_cols_kernel, grid_el, 256, 0, rows, p, Vcur, Q[m / cw].get(), cw, m % cw));
         const int j0 = m;
         m += p;
         steps++;
@@ -1252,9 +1212,7 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
             for (int cc = 0; cc < nc_live; cc++) {
                 GEMB_TRY(gram_ar(Q[cc].get(), cw, Wb, p, Gd.get()));                               // H_c = Q_c^T W   (cw x p)
                 GEMB_TRY(c->t_dense.begin(c->stream));
-                f64_to_f32_kernel<<<(cw * p + 255) / 256, 256, 0, c->stream>>>(cw * p, Gd.get(), M32.get());
-                GEMB_CUDA(cudaGetLastError());
-                count_launch();
+                GEMB_TRY(launch(c, f64_to_f32_kernel, (cw * p + 255) / 256, 256, 0, cw * p, Gd.get(), M32.get()));
                 GEMB_TRY(apply_launch(c, rows, Q[cc].get(), cw, M32.get(), p, p, Tb, p));           // Q_c H_c
                 GEMB_TRY(axpy_launch(c, rows * (int64_t)p, -1.f, Tb, Wb));
                 GEMB_TRY(c->t_dense.end(c->stream));
@@ -1354,9 +1312,8 @@ static int hope_lanczos(HopeWork &W, const Opts &o, int d, SpecMap map, HopeResu
                     GEMB_TRY(copy_sync(c, M32.get(), (half == 0 ? Ms : Mt).data(), sizeof(float) * cw * cw, cudaMemcpyHostToDevice));
                     GEMB_TRY(apply_launch(c, rows, Qn[oc].get(), cw, M32.get(), cw, cw, Tmp64.get(), cw));
                     // reversed column order into X: source column q -> X column (half*k) + k-1-(oc*cw+q)
-                    reverse_put_kernel<<<grid_el, 256, 0, c->stream>>>(rows, ow, Tmp64.get(), cw, R.Xd, d, half * k + k - 1 - oc * cw);
-                    GEMB_CUDA(cudaGetLastError());
-                    count_launch();
+                    GEMB_TRY(launch(c, reverse_put_kernel, grid_el, 256, 0, rows, ow, Tmp64.get(), cw, R.Xd, d,
+                                    half * k + k - 1 - oc * cw));
                 }
             }
             GEMB_TRY(copy_sync(c, R.sig_dev, sig.data(), sizeof(float) * k, cudaMemcpyHostToDevice));
@@ -1420,13 +1377,10 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
     GEMB_CUDA(W.G.alloc((size_t)k * w));
     GEMB_CUDA(W.M1.alloc((size_t)k * w));
     DeviceBuffer<float> Xd, L, Rr;
-    GEMB_CUDA(Xd.alloc((size_t)n * d));
+    GEMB_CUDA(Xd.upload(X, (size_t)n * d, c->stream));
     GEMB_CUDA(L.alloc((size_t)n * k));
     GEMB_CUDA(Rr.alloc((size_t)n * k));
-    GEMB_CUDA(cudaMemcpyAsync(Xd.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
-    split_halves_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n, d, Xd.get(), L.get(), Rr.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, split_halves_kernel, c->sm_count * 4, 256, 0, n, d, Xd.get(), L.get(), Rr.get()));
     c->t_spmm.reset(); c->t_dense.reset(); c->t_comm.reset();
     double nrm = 0.0;
     int J = 0;
@@ -1439,19 +1393,13 @@ extern "C" int gemb_hope_svd_error(gemb_graph *g, int d, float beta, const float
     const int threads = (256 / w) * w > 0 ? (256 / w) * w : w;
     for (int64_t p0 = 0; p0 < total_cols; p0 += w) {
         const int live = (int)std::min<int64_t>(w, total_cols - p0);
-        probe_block_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(n, w, p0, probe ? 1 : 0, seed, Z);
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, probe_block_kernel, c->sm_count * 4, 256, 0, n, w, p0, probe ? 1 : 0, seed, Z));
         GEMB_TRY(katz(W, false, beta, J, Z, SZ, W.buf[3], W.buf[4]));             // S Z
         GEMB_TRY(gram_launch(c, n, Rr.get(), k, Z, w, W.G.get()));                            // X2^T Z   (k x w, fp64)
-        f64_to_f32_kernel<<<(k * w + 255) / 256, 256, 0, c->stream>>>(k * w, W.G.get(), W.M1.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, f64_to_f32_kernel, (k * w + 255) / 256, 256, 0, k * w, W.G.get(), W.M1.get()));
         GEMB_TRY(apply_launch(c, n, L.get(), k, W.M1.get(), w, w, LZ, w));                    // X1 (X2^T Z)
         GEMB_CUDA(cudaMemsetAsync(W.scal.get(), 0, sizeof(double) * w, c->stream));
-        coldiff_sumsq_kernel<<<c->sm_count * 4, threads, 0, c->stream>>>(n, w, LZ, SZ, W.scal.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, coldiff_sumsq_kernel, c->sm_count * 4, threads, 0, n, w, LZ, SZ, W.scal.get()));
         GEMB_TRY(copy_sync(c, rs.data(), W.scal.get(), sizeof(double) * w, cudaMemcpyDeviceToHost));
         for (int j = 0; j < live; j++) acc += rs[j];
     }
@@ -1618,8 +1566,7 @@ extern "C" int gemb_hope(gemb_graph *g, int d, float beta, const gemb_hope_opts 
         if (hs == GEMB_OK) hs = halo_buffers(g, 5, b);
         int hflag = (hs == GEMB_OK) ? 1 : 0;
         DeviceBuffer<int> flag;
-        GEMB_CUDA(flag.alloc(1));
-        GEMB_CUDA(cudaMemcpyAsync(flag.get(), &hflag, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+        GEMB_CUDA(flag.upload(&hflag, 1, c->stream));
         GEMB_TRY(comm_allreduce(W, flag.get(), 1, ncclInt, ncclMin, false, "ncclAllReduce(halo agreement)"));
         GEMB_TRY(copy_sync(c, &hflag, flag.get(), sizeof(int), cudaMemcpyDeviceToHost));
         W.halo = hflag == 1;

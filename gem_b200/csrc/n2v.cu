@@ -477,19 +477,13 @@ static int check_graph_for_n2v(gemb_graph *g) {
 static int build_alias(gemb_graph *g, const double *weights64, double p, double q, N2VDev &D) {
     gemb_ctx *c = g->ctx;
     const int64_t nnz = g->A.nnz, n = g->n;
-    if (weights64 && nnz) {
-        GEMB_CUDA(D.w.alloc(nnz));
-        GEMB_CUDA(cudaMemcpyAsync(D.w.get(), weights64, sizeof(double) * nnz, cudaMemcpyHostToDevice, c->stream));
-    }
+    if (weights64 && nnz) GEMB_CUDA(D.w.upload(weights64, nnz, c->stream));
     if (p == 1.0 && q == 1.0) {
         GEMB_CUDA(D.K.alloc(std::max<int64_t>(nnz, 1)));
         GEMB_CUDA(D.U.alloc(std::max<int64_t>(nnz, 1)));
         GEMB_CUDA(D.scratch.alloc(std::max<int64_t>(nnz, 1)));
-        alias_build_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c->stream>>>(n, g->A.indptr, D.w.get(), D.K.get(),
-                                                                                D.U.get(), D.scratch.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-        return GEMB_OK;
+        return launch(c, alias_build_kernel, (unsigned)((n + 127) / 128), 128, 0, n, g->A.indptr, D.w.get(), D.K.get(), D.U.get(),
+                      D.scratch.get());
     }
     GEMB_CUDA(D.off2.alloc(nnz + 1));
     long long T = 0;
@@ -497,19 +491,14 @@ static int build_alias(gemb_graph *g, const double *weights64, double p, double 
         DeviceBuffer<long long> deg;
         GEMB_CUDA(deg.alloc(nnz + 1));
         GEMB_CUDA(cudaMemsetAsync(deg.get(), 0, sizeof(long long) * (nnz + 1), c->stream));
-        if (nnz) {
-            edge_degree_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(nnz, g->A.indptr, g->A.indices, deg.get());
-            GEMB_CUDA(cudaGetLastError());
-            count_launch();
-        }
+        if (nnz) GEMB_TRY(launch(c, edge_degree_kernel, c->sm_count * 8, 256, 0, nnz, g->A.indptr, g->A.indices, deg.get()));
         size_t tb = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, tb, deg.get(), D.off2.get(), nnz + 1, c->stream);
         DeviceBuffer<char> tmp;
         GEMB_CUDA(tmp.alloc(tb));
         GEMB_CUDA(cub::DeviceScan::ExclusiveSum(tmp.get(), tb, deg.get(), D.off2.get(), nnz + 1, c->stream));
         count_launch();
-        GEMB_CUDA(cudaMemcpyAsync(&T, D.off2.get() + nnz, sizeof T, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(copy_sync(c, &T, D.off2.get() + nnz, sizeof T, cudaMemcpyDeviceToHost));
     }
     // the reference needs the same sum_(t->v) outdeg(v) entries in host hash maps; here they must fit in HBM
     size_t free_b = 0, total_b = 0;
@@ -523,13 +512,9 @@ static int build_alias(gemb_graph *g, const double *weights64, double p, double 
     GEMB_CUDA(D.K.alloc(std::max<long long>(T, 1)));
     GEMB_CUDA(D.U.alloc(std::max<long long>(T, 1)));
     GEMB_CUDA(D.scratch.alloc(std::max<long long>(T, 1)));
-    if (nnz) {
-        alias2_build_kernel<<<(unsigned)((nnz + 127) / 128), 128, 0, c->stream>>>(n, nnz, g->A.indptr, g->A.indices, D.w.get(),
-                                                                                 D.off2.get(), p, q, D.K.get(), D.U.get(),
-                                                                                 D.scratch.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
+    if (nnz)
+        GEMB_TRY(launch(c, alias2_build_kernel, (unsigned)((nnz + 127) / 128), 128, 0, n, nnz, g->A.indptr, g->A.indices, D.w.get(),
+                        D.off2.get(), p, q, D.K.get(), D.U.get(), D.scratch.get()));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     D.scratch.reset();   // 4 of the 16 bytes per entry: freed before the walks allocate theirs
     return GEMB_OK;
@@ -553,18 +538,14 @@ static int alias_and_walks(gemb_graph *g, const double *weights64, double p, dou
     std::vector<int32_t> order((size_t)num_walks * N);
     shuffle_rounds(nids, N, num_walks, walk_len, seed, order.data());
     const double sh_ms = ms_since(t0);
-    GEMB_CUDA(D.order.alloc(std::max<size_t>(order.size(), 1)));
-    GEMB_CUDA(cudaMemcpyAsync(D.order.get(), order.data(), sizeof(int32_t) * order.size(), cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(D.order.upload(order.data(), order.size(), c->stream));
     const int64_t cnt = w_end - w_begin;
     GEMB_CUDA(D.walks.alloc(std::max<int64_t>(cnt * walk_len, 1)));
     if (cnt > 0) {
         const long long *off2 = D.off2.get();
         auto walk = off2 ? walk_kernel<true> : walk_kernel<false>;
-        walk<<<(unsigned)((cnt + 127) / 128), 128, 0, c->stream>>>(g->A.indptr, g->A.indices, D.K.get(), D.U.get(), off2,
-                                                                   D.order.get(), N, walk_len, seed, w_begin, w_end,
-                                                                   D.walks.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, walk, (unsigned)((cnt + 127) / 128), 128, 0, g->A.indptr, g->A.indices, D.K.get(), D.U.get(), off2,
+                        D.order.get(), N, walk_len, seed, w_begin, w_end, D.walks.get()));
     }
     GEMB_CUDA(cudaEventRecord(ev[2], c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));  // `order` (host) must outlive the async copy
@@ -583,36 +564,21 @@ static int alias_and_walks(gemb_graph *g, const double *weights64, double p, dou
 // Every warp stages its walk in shared memory: warps x walk_len int32.
 static size_t sgns_smem_bytes(int threads, int walk_len) { return sizeof(int32_t) * (threads / 32) * (size_t)walk_len; }
 
-template <int NV, bool VEC>
 static int launch_sgns(gemb_ctx *c, const SgnsParams &P, int blocks, int threads) {
+    const int d = P.d, nv = (d + 31) / 32;
+    auto kernel = sgns_kernel<16, false>;
+    if (d % 128 == 0 && d <= 512)
+        kernel = d == 128 ? sgns_kernel<4, true> : d == 256 ? sgns_kernel<8, true> : d == 384 ? sgns_kernel<12, true> : sgns_kernel<16, true>;
+    else if (nv <= 8)
+        kernel = nv <= 1 ? sgns_kernel<1, false> : nv <= 2 ? sgns_kernel<2, false> : nv <= 4 ? sgns_kernel<4, false> : sgns_kernel<8, false>;
+    else if (nv > 16) {
+        set_error("node2vec: d = %d is not supported (d <= 512)", d);
+        return GEMB_ERR_UNSUPPORTED;
+    }
     const size_t sh = sgns_smem_bytes(threads, P.walk_len);
     // beyond the default 48 KB the kernel has to opt in (gemb_node2vec checked sh against the device's opt-in limit)
-    if (sh > 48 * 1024)
-        GEMB_CUDA(cudaFuncSetAttribute(sgns_kernel<NV, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
-    sgns_kernel<NV, VEC><<<blocks, threads, sh, c->stream>>>(P);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
-}
-
-static int dispatch_sgns(gemb_ctx *c, const SgnsParams &P, int blocks, int threads) {
-    const int d = P.d;
-    if (d % 128 == 0 && d <= 512) {
-        switch (d / 128) {
-            case 1: return launch_sgns<4, true>(c, P, blocks, threads);
-            case 2: return launch_sgns<8, true>(c, P, blocks, threads);
-            case 3: return launch_sgns<12, true>(c, P, blocks, threads);
-            default: return launch_sgns<16, true>(c, P, blocks, threads);
-        }
-    }
-    const int nv = (d + 31) / 32;
-    if (nv <= 1) return launch_sgns<1, false>(c, P, blocks, threads);
-    if (nv <= 2) return launch_sgns<2, false>(c, P, blocks, threads);
-    if (nv <= 4) return launch_sgns<4, false>(c, P, blocks, threads);
-    if (nv <= 8) return launch_sgns<8, false>(c, P, blocks, threads);
-    if (nv <= 16) return launch_sgns<16, false>(c, P, blocks, threads);
-    set_error("node2vec: d = %d is not supported (d <= 512)", d);
-    return GEMB_ERR_UNSUPPORTED;
+    if (sh > 48 * 1024) GEMB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh));
+    return launch(c, kernel, blocks, threads, sh, P);
 }
 
 }  // namespace gemb
@@ -709,12 +675,9 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     GEMB_CUDA(D.cnt.alloc(n_ids));
     GEMB_CUDA(cudaMemsetAsync(D.first_pos.get(), 0xff, sizeof(unsigned long long) * n_ids, c->stream));
     GEMB_CUDA(cudaMemsetAsync(D.cnt.get(), 0, sizeof(unsigned long long) * n_ids, c->stream));
-    if (n_local > 0) {
-        vocab_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(D.walks.get(), n_local * walk_len, w_begin * walk_len,
-                                                             D.first_pos.get(), D.cnt.get());
-        GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    }
+    if (n_local > 0)
+        GEMB_TRY(launch(c, vocab_kernel, c->sm_count * 8, 256, 0, D.walks.get(), n_local * walk_len, w_begin * walk_len,
+                        D.first_pos.get(), D.cnt.get()));
     if (c->nranks > 1) {
         NcclApi *api = nccl_api();
         if (!api) return GEMB_ERR_NCCL;
@@ -749,12 +712,9 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
         while (t < 2147483647LL && (double)t / 2147483647.0 < u) t++;
         ent[i] = make_uint4((uint32_t)t, (uint32_t)tok2node[i], (uint32_t)tok2node[KT[i]], 0u);
     }
-    GEMB_CUDA(D.ent.alloc(V));
-    GEMB_CUDA(cudaMemcpyAsync(D.ent.get(), ent.data(), sizeof(uint4) * V, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(D.KT.alloc(V));
-    GEMB_CUDA(D.tok2node.alloc(V));
-    GEMB_CUDA(cudaMemcpyAsync(D.KT.get(), KT.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(D.tok2node.get(), tok2node.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(D.ent.upload(ent.data(), V, c->stream));
+    GEMB_CUDA(D.KT.upload(KT.data(), V, c->stream));
+    GEMB_CUDA(D.tok2node.upload(tok2node.data(), V, c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     const double vocab_ms = ms_since(tv0);
     GEMB_CUDA(cudaEventRecord(ev[3], c->stream));
@@ -765,16 +725,13 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
     GEMB_CUDA(D.syn_neg.alloc(tab));
     GEMB_CUDA(cudaMemsetAsync(D.syn_pos.get(), 0, sizeof(float) * tab, c->stream));
     GEMB_CUDA(cudaMemsetAsync(D.syn_neg.get(), 0, sizeof(float) * tab, c->stream));
-    init_pos_kernel<<<(unsigned)((V + 127) / 128), 128, 0, c->stream>>>(V, d, (uint32_t)seed, D.tok2node.get(), D.syn_pos.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, init_pos_kernel, (unsigned)((V + 127) / 128), 128, 0, V, d, (uint32_t)seed, D.tok2node.get(), D.syn_pos.get()));
     GEMB_CUDA(D.pairs.alloc(1));
     GEMB_CUDA(cudaMemsetAsync(D.pairs.get(), 0, sizeof(unsigned long long), c->stream));
     GEMB_CUDA(D.seq_state.alloc(1));
     {
         const uint32_t st0 = lcg_skip((uint32_t)seed, (uint64_t)V * (uint64_t)d);  // after InitPosEmb's V*d draws
-        GEMB_CUDA(cudaMemcpyAsync(D.seq_state.get(), &st0, sizeof st0, cudaMemcpyHostToDevice, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(copy_sync(c, D.seq_state.get(), &st0, sizeof st0, cudaMemcpyHostToDevice));
     }
     if (c->nranks > 1) {
         GEMB_CUDA(D.pos0.alloc(tab));
@@ -804,7 +761,7 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
             GEMB_CUDA(cudaMemcpyAsync(pos0, syn_pos, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
             GEMB_CUDA(cudaMemcpyAsync(delta, syn_neg, sizeof(float) * tab, cudaMemcpyDeviceToDevice, c->stream));
         }
-        if (n_local > 0) GEMB_TRY(dispatch_sgns(c, P, blocks, threads));
+        if (n_local > 0) GEMB_TRY(launch_sgns(c, P, blocks, threads));
         if (c->nranks > 1) {
             // embedding-"gradient" all-reduce once per epoch: table <- table0 + sum_ranks (table_r - table0)
             NcclApi *api = nccl_api();

@@ -296,10 +296,6 @@ __global__ void __launch_bounds__(256) nc_topk_kernel(int64_t rows, int64_t row0
     }
 }
 
-static int launch_grid(gemb_ctx *ctx, int64_t work, int per_block) {
-    return (int)std::max<int64_t>(1, std::min<int64_t>((work + per_block - 1) / per_block, (int64_t)ctx->sm_count * 8));
-}
-
 }  // namespace gemb
 
 using namespace gemb;
@@ -333,12 +329,9 @@ extern "C" int gemb_nc_fit(gemb_ctx *ctx, int64_t n, int d, const float *X, cons
     DeviceBuffer<double> dG, dSums, dBias, dVec, dHist, dScal;
     DeviceBuffer<int> dInts;
     const int PM = NC_PANEL;
-    GEMB_CUDA(dX.alloc((size_t)n * d));
-    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, ctx->stream));
-    GEMB_CUDA(dIndptr.alloc(n + 1));
-    GEMB_CUDA(cudaMemcpyAsync(dIndptr.get(), indptr, sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
-    GEMB_CUDA(dLab.alloc(std::max<int64_t>(nnz, 1)));
-    if (nnz) GEMB_CUDA(cudaMemcpyAsync(dLab.get(), labels, sizeof(int32_t) * nnz, cudaMemcpyHostToDevice, ctx->stream));
+    GEMB_CUDA(dX.upload(X, (size_t)n * d, ctx->stream));
+    GEMB_CUDA(dIndptr.upload(indptr, n + 1, ctx->stream));
+    GEMB_CUDA(dLab.upload(labels, nnz, ctx->stream));
     GEMB_CUDA(dZ.alloc((size_t)n * PM));
     GEMB_CUDA(dWf.alloc((size_t)d * PM));
     GEMB_CUDA(dG.alloc((size_t)d * PM));
@@ -348,7 +341,7 @@ extern "C" int gemb_nc_fit(gemb_ctx *ctx, int64_t n, int d, const float *X, cons
     GEMB_CUDA(dHist.alloc((size_t)2 * NC_M * PM * D1 + (size_t)NC_M * PM));
     GEMB_CUDA(dScal.alloc((size_t)5 * PM));
     GEMB_CUDA(dInts.alloc((size_t)7 * PM));
-    const int grid_res = launch_grid(ctx, n, 8);
+    const int grid_res = grid_stride(ctx, n, 8, 8);
     std::vector<int> init(PM), status(PM), iters(PM);
     std::vector<double> xh((size_t)PM * D1);
     int64_t evals = 0, unconverged = 0, constant = 0;
@@ -369,27 +362,22 @@ extern "C" int gemb_nc_fit(gemb_ctx *ctx, int64_t n, int d, const float *X, cons
         for (int c = 0; c < P; c++)
             init[c] = (c >= nc || npos[c0 + c] == 0 || npos[c0 + c] == n) ? NC_CONSTANT : NC_RUNNING;
         GEMB_CUDA(cudaMemcpyAsync(d_init, init.data(), sizeof(int) * P, cudaMemcpyHostToDevice, ctx->stream));
-        nc_init_kernel<<<launch_grid(ctx, (int64_t)P * D1, 256), 256, 0, ctx->stream>>>(st, d, d_init, dWf.get(), dBias.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(ctx, nc_init_kernel, grid_stride(ctx, (int64_t)P * D1, 256, 8), 256, 0, st, d, d_init, dWf.get(),
+                        dBias.get()));
         bool running = std::count(init.begin(), init.begin() + P, (int)NC_RUNNING) > 0;
         while (running) {
             GEMB_TRY(apply_launch(ctx, n, dX.get(), d, dWf.get(), P, P, dZ.get(), P));
             double *part = nullptr;
             GEMB_TRY(red_scratch(ctx, (size_t)grid_res * 2 * P, &part));
-            nc_residual_kernel<<<grid_res, 256, 0, ctx->stream>>>(n, P, c0, dIndptr.get(), dLab.get(), dBias.get(), dZ.get(), part);
-            GEMB_CUDA(cudaGetLastError());
-            count_launch();
+            GEMB_TRY(launch(ctx, nc_residual_kernel, grid_res, 256, 0, n, P, c0, dIndptr.get(), dLab.get(), dBias.get(), dZ.get(),
+                            part));
             GEMB_TRY(sum_partials_launch(ctx, grid_res, 2 * P, part, dSums.get()));
             GEMB_TRY(gram_launch(ctx, n, dX.get(), d, dZ.get(), P, dG.get()));
-            nc_step_kernel<<<P, 256, 0, ctx->stream>>>(st, d, C, tol, max_iter, dG.get(), dSums.get(), dWf.get(), dBias.get());
-            GEMB_CUDA(cudaGetLastError());
-            count_launch();
+            GEMB_TRY(launch(ctx, nc_step_kernel, P, 256, 0, st, d, C, tol, max_iter, dG.get(), dSums.get(), dWf.get(), dBias.get()));
             evals++;
             // compulsory bytes: apply (X in, Z out), residual (Z in, R out, labels), Gram (X and R in)
             bytes += (double)n * (8.0 * d + 16.0 * P + 8.0) + 4.0 * (double)nnz;
-            GEMB_CUDA(cudaMemcpyAsync(status.data(), st.status, sizeof(int) * P, cudaMemcpyDeviceToHost, ctx->stream));
-            GEMB_CUDA(cudaStreamSynchronize(ctx->stream));
+            GEMB_TRY(copy_sync(ctx, status.data(), st.status, sizeof(int) * P, cudaMemcpyDeviceToHost));
             running = std::count(status.begin(), status.begin() + P, (int)NC_RUNNING) > 0;
         }
         GEMB_CUDA(cudaMemcpyAsync(status.data(), st.status, sizeof(int) * P, cudaMemcpyDeviceToHost, ctx->stream));
@@ -447,24 +435,17 @@ extern "C" int gemb_nc_topk(gemb_ctx *ctx, int64_t m, int d, const float *X, int
     DeviceBuffer<double> dB;
     DeviceBuffer<int64_t> dK;
     DeviceBuffer<int32_t> dOut;
-    GEMB_CUDA(dX.alloc((size_t)m * d));
-    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * (size_t)m * d, cudaMemcpyHostToDevice, ctx->stream));
-    GEMB_CUDA(dW.alloc(wf.size()));
-    GEMB_CUDA(cudaMemcpyAsync(dW.get(), wf.data(), sizeof(float) * wf.size(), cudaMemcpyHostToDevice, ctx->stream));
-    GEMB_CUDA(dB.alloc(Lp));
-    GEMB_CUDA(cudaMemcpyAsync(dB.get(), bias.data(), sizeof(double) * Lp, cudaMemcpyHostToDevice, ctx->stream));
-    GEMB_CUDA(dK.alloc(m + 1));
-    GEMB_CUDA(cudaMemcpyAsync(dK.get(), koff, sizeof(int64_t) * (m + 1), cudaMemcpyHostToDevice, ctx->stream));
+    GEMB_CUDA(dX.upload(X, (size_t)m * d, ctx->stream));
+    GEMB_CUDA(dW.upload(wf.data(), wf.size(), ctx->stream));
+    GEMB_CUDA(dB.upload(bias.data(), Lp, ctx->stream));
+    GEMB_CUDA(dK.upload(koff, m + 1, ctx->stream));
     GEMB_CUDA(dOut.alloc(total));
     GEMB_CUDA(dZ.alloc((size_t)chunk * Lp));
     for (int64_t r0 = 0; r0 < m; r0 += chunk) {
         const int64_t rows = std::min(chunk, m - r0);
         GEMB_TRY(apply_launch(ctx, rows, dX.get() + (size_t)r0 * d, d, dW.get(), Lp, Lp, dZ.get(), Lp));
-        nc_topk_kernel<<<launch_grid(ctx, rows, 8), 256, 0, ctx->stream>>>(rows, r0, L, Lp, dZ.get(), dB.get(), dK.get(), dOut.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(ctx, nc_topk_kernel, grid_stride(ctx, rows, 8, 8), 256, 0, rows, r0, L, Lp, dZ.get(), dB.get(), dK.get(),
+                        dOut.get()));
     }
-    GEMB_CUDA(cudaMemcpyAsync(pred_out, dOut.get(), sizeof(int32_t) * total, cudaMemcpyDeviceToHost, ctx->stream));
-    GEMB_CUDA(cudaStreamSynchronize(ctx->stream));
-    return GEMB_OK;
+    return copy_sync(ctx, pred_out, dOut.get(), sizeof(int32_t) * total, cudaMemcpyDeviceToHost);
 }

@@ -313,25 +313,14 @@ __global__ void recon_swap_kernel(int64_t m, const int64_t *__restrict__ off, fl
     }
 }
 
-static int grid_for(gemb_ctx *c, int64_t items, int per_block) {
-    int64_t g = (items + per_block - 1) / per_block;
-    const int64_t cap = (int64_t)c->sm_count * 16;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-
 static int count_ge(gemb_recon *r, int undirected, uint32_t bits, unsigned long long *dcounter, int64_t *out) {
     gemb_ctx *c = r->ctx;
     GEMB_CUDA(cudaMemsetAsync(dcounter, 0, sizeof(unsigned long long), c->stream));
     const int64_t n_panels = r->n_pad / PW;
-    recon_select_kernel<false><<<grid_for(c, n_panels * r->n * 32, 256), 256, 0, c->stream>>>(
-        r->n, n_panels, undirected, bits, r->adj, dcounter, 0, nullptr, nullptr, nullptr);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, recon_select_kernel<false>, grid_stride(c, n_panels * r->n * 32, 256, 16), 256, 0, r->n, n_panels,
+                    undirected, bits, r->adj, dcounter, 0, nullptr, nullptr, nullptr));
     unsigned long long h = 0;
-    GEMB_CUDA(cudaMemcpyAsync(&h, dcounter, sizeof h, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
+    GEMB_TRY(copy_sync(c, &h, dcounter, sizeof h, cudaMemcpyDeviceToHost));
     *out = (int64_t)h;
     return GEMB_OK;
 }
@@ -339,19 +328,13 @@ static int count_ge(gemb_recon *r, int undirected, uint32_t bits, unsigned long 
 // Gaussian kind: turn the m keys at w (device) into delta before they are copied out; a no-op for the other kinds
 static int decode_out(const gemb_recon *r, int64_t m, float *w) {
     if (r->kind != GEMB_RECON_GAUSS || m == 0) return GEMB_OK;
-    recon_key_to_delta_kernel<<<grid_for(r->ctx, m, 256), 256, 0, r->ctx->stream>>>(m, w);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(r->ctx, recon_key_to_delta_kernel, grid_stride(r->ctx, m, 256, 16), 256, 0, m, w);
 }
 
 static int swap_excluded(gemb_recon *r) {
     const int64_t m = r->ex_nnz;
     if (m == 0) return GEMB_OK;
-    recon_swap_kernel<<<grid_for(r->ctx, m, 256), 256, 0, r->ctx->stream>>>(m, r->ex_off, r->ex_saved, r->adj);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
-    return GEMB_OK;
+    return launch(r->ctx, recon_swap_kernel, grid_stride(r->ctx, m, 256, 16), 256, 0, m, r->ex_off, r->ex_saved, r->adj);
 }
 
 // run body() on the panels with the excluded entries set to 0, and restore them whatever body() returns; the first
@@ -371,12 +354,9 @@ extern "C" {
 
 static int recon_create_gauss(gemb_ctx *c, const float *X, int64_t n, int d, int64_t n_pad, float *adj) {
     DeviceBuffer<float> dX;
-    GEMB_CUDA(dX.alloc((size_t)n * d));
-    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
+    GEMB_CUDA(dX.upload(X, (size_t)n * d, c->stream));
     const int64_t row_tiles = (n + SQD_ROWS - 1) / SQD_ROWS;
-    recon_sqdist_kernel<<<(unsigned)(row_tiles * (n_pad / PW)), SQD_THREADS, 0, c->stream>>>(n, d, row_tiles, dX.get(), adj);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, recon_sqdist_kernel, (unsigned)(row_tiles * (n_pad / PW)), SQD_THREADS, 0, n, d, row_tiles, dX.get(), adj));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     return GEMB_OK;
 }
@@ -416,29 +396,20 @@ int gemb_recon_create(gemb_ctx *c, const float *X, int64_t n, int d, int kind, g
         return GEMB_OK;
     }
     DeviceBuffer<float> dX, L, Rt, adj;
-    GEMB_CUDA(dX.alloc((size_t)n * d));
+    GEMB_CUDA(dX.upload(X, (size_t)n * d, c->stream));
     GEMB_CUDA(Rt.alloc((size_t)n_pad * k));
     GEMB_CUDA(adj.alloc((size_t)n * n_pad));
-    GEMB_CUDA(cudaMemcpyAsync(dX.get(), X, sizeof(float) * (size_t)n * d, cudaMemcpyHostToDevice, c->stream));
     const float *Lp = dX.get();
     if (split) {
         GEMB_CUDA(L.alloc((size_t)n * k));
-        recon_left_kernel<<<grid_for(c, n * k, 256), 256, 0, c->stream>>>(n, d, k, dX.get(), L.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, recon_left_kernel, grid_stride(c, n * k, 256, 16), 256, 0, n, d, k, dX.get(), L.get()));
         Lp = L.get();
     }
-    {
-        dim3 grid((unsigned)((n_pad + 31) / 32), (unsigned)((k + 31) / 32)), block(32, 8);
-        recon_right_t_kernel<<<grid, block, 0, c->stream>>>(n, n_pad, d, k, split ? k : 0, dX.get(), Rt.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
-    }
+    GEMB_TRY(launch(c, recon_right_t_kernel, dim3((unsigned)((n_pad + 31) / 32), (unsigned)((k + 31) / 32)), dim3(32, 8), 0, n,
+                    n_pad, d, k, split ? k : 0, dX.get(), Rt.get()));
     for (int64_t p = 0; p < n_pad / PW; p++)
         GEMB_TRY(apply_launch(c, n, Lp, k, Rt.get() + p * PW, (int)n_pad, PW, adj.get() + (size_t)p * n * PW, PW));
-    recon_zero_diag_kernel<<<grid_for(c, n, 256), 256, 0, c->stream>>>(n, adj.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, recon_zero_diag_kernel, grid_stride(c, n, 256, 16), 256, 0, n, adj.get()));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     gemb_recon *r = new gemb_recon();
     r->ctx = c; r->n = n; r->n_pad = n_pad; r->k = k; r->kind = kind;
@@ -467,12 +438,9 @@ int gemb_recon_dense(gemb_recon *r, float *adj_out) {
     GEMB_CUDA(buf.alloc((size_t)rows * n));
     for (int64_t r0 = 0; r0 < n; r0 += rows) {
         const int64_t nr = std::min(rows, n - r0);
-        recon_rowmajor_kernel<<<grid_for(c, nr * n, 256), 256, 0, c->stream>>>(n, r0, nr, r->adj, buf.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, recon_rowmajor_kernel, grid_stride(c, nr * n, 256, 16), 256, 0, n, r0, nr, r->adj, buf.get()));
         GEMB_TRY(decode_out(r, nr * n, buf.get()));
-        GEMB_CUDA(cudaMemcpyAsync(adj_out + (size_t)r0 * n, buf.get(), sizeof(float) * (size_t)nr * n, cudaMemcpyDeviceToHost, c->stream));
-        GEMB_CUDA(cudaStreamSynchronize(c->stream));
+        GEMB_TRY(copy_sync(c, adj_out + (size_t)r0 * n, buf.get(), sizeof(float) * (size_t)nr * n, cudaMemcpyDeviceToHost));
     }
     return GEMB_OK;
 }
@@ -486,18 +454,12 @@ int gemb_recon_pairs(gemb_recon *r, const int32_t *pi, const int32_t *pj, int64_
         GEMB_ARG(pi[t] >= 0 && pi[t] < r->n && pj[t] >= 0 && pj[t] < r->n, "pair index out of range");
     DeviceBuffer<int32_t> di, dj;
     DeviceBuffer<float> dout;
-    GEMB_CUDA(di.alloc((size_t)m));
-    GEMB_CUDA(dj.alloc((size_t)m));
+    GEMB_CUDA(di.upload(pi, (size_t)m, c->stream));
+    GEMB_CUDA(dj.upload(pj, (size_t)m, c->stream));
     GEMB_CUDA(dout.alloc((size_t)m));
-    GEMB_CUDA(cudaMemcpyAsync(di.get(), pi, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->stream));
-    GEMB_CUDA(cudaMemcpyAsync(dj.get(), pj, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->stream));
-    recon_pairs_kernel<<<grid_for(c, m, 256), 256, 0, c->stream>>>(r->n, m, di.get(), dj.get(), r->adj, dout.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(c, recon_pairs_kernel, grid_stride(c, m, 256, 16), 256, 0, r->n, m, di.get(), dj.get(), r->adj, dout.get()));
     GEMB_TRY(decode_out(r, m, dout.get()));
-    GEMB_CUDA(cudaMemcpyAsync(out, dout.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+    return copy_sync(c, out, dout.get(), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost);
 }
 
 int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indices, int is_undirected,
@@ -511,16 +473,12 @@ int gemb_recon_ranks(gemb_recon *r, const int32_t *indptr, const int32_t *indice
     for (int64_t t = 0; t < nnz; t++) GEMB_ARG(indices[t] >= 0 && indices[t] < n, "column id out of range");
     return with_exclusion_masked(r, [&]() -> int {
         DeviceBuffer<int32_t> dp, dix, drank, dnp;
-        GEMB_CUDA(dp.alloc((size_t)(n + 1)));
-        GEMB_CUDA(dix.alloc((size_t)std::max<int64_t>(nnz, 1)));
+        GEMB_CUDA(dp.upload(indptr, (size_t)(n + 1), c->stream));
+        GEMB_CUDA(dix.upload(indices, (size_t)nnz, c->stream));
         GEMB_CUDA(drank.alloc((size_t)std::max<int64_t>(nnz, 1)));
         GEMB_CUDA(dnp.alloc((size_t)n));
-        GEMB_CUDA(cudaMemcpyAsync(dp.get(), indptr, sizeof(int32_t) * (size_t)(n + 1), cudaMemcpyHostToDevice, c->stream));
-        if (nnz) GEMB_CUDA(cudaMemcpyAsync(dix.get(), indices, sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, c->stream));
-        recon_rank_kernel<<<grid_for(c, n * 32, 256), 256, 0, c->stream>>>(n, dp.get(), dix.get(), is_undirected ? 1 : 0,
-                                                                           r->adj, drank.get(), dnp.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, recon_rank_kernel, grid_stride(c, n * 32, 256, 16), 256, 0, n, dp.get(), dix.get(), is_undirected ? 1 : 0,
+                        r->adj, drank.get(), dnp.get()));
         if (nnz) GEMB_CUDA(cudaMemcpyAsync(rank_out, drank.get(), sizeof(int32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaMemcpyAsync(n_pred_row, dnp.get(), sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaStreamSynchronize(c->stream));
@@ -556,9 +514,8 @@ int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *e
     if (off.empty()) return GEMB_OK;
     DeviceBuffer<int64_t> doff;
     DeviceBuffer<float> dsaved;
-    GEMB_CUDA(doff.alloc(off.size()));
+    GEMB_CUDA(doff.upload(off.data(), off.size(), c->stream));
     GEMB_CUDA(dsaved.alloc(off.size()));
-    GEMB_CUDA(cudaMemcpyAsync(doff.get(), off.data(), sizeof(int64_t) * off.size(), cudaMemcpyHostToDevice, c->stream));
     GEMB_CUDA(cudaMemsetAsync(dsaved.get(), 0, sizeof(float) * off.size(), c->stream));
     GEMB_CUDA(cudaStreamSynchronize(c->stream));
     r->ex_off = doff.release();
@@ -610,10 +567,8 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
         GEMB_CUDA(dw.alloc((size_t)m));
         GEMB_CUDA(cudaMemsetAsync(dcounter.get(), 0, sizeof(unsigned long long), c->stream));
         const int64_t n_panels = r->n_pad / PW;
-        recon_select_kernel<true><<<grid_for(c, n_panels * r->n * 32, 256), 256, 0, c->stream>>>(
-            r->n, n_panels, und, r->top_bits, r->adj, dcounter.get(), m, di.get(), dj.get(), dw.get());
-        GEMB_CUDA(cudaGetLastError());
-        count_launch();
+        GEMB_TRY(launch(c, recon_select_kernel<true>, grid_stride(c, n_panels * r->n * 32, 256, 16), 256, 0, r->n, n_panels, und,
+                        r->top_bits, r->adj, dcounter.get(), m, di.get(), dj.get(), dw.get()));
         GEMB_TRY(decode_out(r, m, dw.get()));
         GEMB_CUDA(cudaMemcpyAsync(i_out, di.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));
         GEMB_CUDA(cudaMemcpyAsync(j_out, dj.get(), sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, c->stream));

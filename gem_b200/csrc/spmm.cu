@@ -232,11 +232,8 @@ static int spmm_sweep(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int 
     float4 *Y4 = (float4 *)Y;
     auto bulk = A.data ? spmm_bulk_kernel<true, HAS_PUSH, HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>
                        : spmm_bulk_kernel<false, HAS_PUSH, HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>;
-    bulk<<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta,
-                                                    tile_rows, e.alpha, e.gamma, e.delta, X4, XS4, X04, Y4,
-                                                    heavy ? SPMM_HEAVY_DEG : 0, PA, e.eps, X14, e.rscale);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch();
+    GEMB_TRY(launch(ctx, bulk, (unsigned)n_tiles, 256, 0, A.indptr, A.indices, A.data, n_rows, A.nnz, G, rows_per_cta, tile_rows,
+                    e.alpha, e.gamma, e.delta, X4, XS4, X04, Y4, heavy ? SPMM_HEAVY_DEG : 0, PA, e.eps, X14, e.rscale));
     if (!heavy) return GEMB_OK;
     const size_t need = sizeof(float) * (size_t)A.n_items * b;
     if (ctx->spmm_scratch_bytes < need) {
@@ -247,16 +244,11 @@ static int spmm_sweep(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int 
     }
     float4 *P4 = (float4 *)ctx->spmm_scratch;
     auto partial = A.data ? spmm_heavy_partial_kernel<true> : spmm_heavy_partial_kernel<false>;
-    partial<<<A.n_items, 256, 0, ctx->stream>>>(A.indptr, A.indices, A.data, A.item_row, A.item_beg, G, rows_per_cta,
-                                               SPMM_HEAVY_CHUNK, X4, P4);
-    GEMB_CUDA(cudaGetLastError());
+    GEMB_TRY(launch(ctx, partial, A.n_items, 256, 0, A.indptr, A.indices, A.data, A.item_row, A.item_beg, G, rows_per_cta,
+                    SPMM_HEAVY_CHUNK, X4, P4));
     const int fgrid = (int)(((int64_t)A.n_heavy * G + 255) / 256);
-    spmm_heavy_finish_kernel<HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE><<<fgrid, 256, 0, ctx->stream>>>(
-        A.n_heavy, A.heavy_row, A.heavy_first, G, e.alpha, e.gamma, e.delta, P4, XS4, X04, Y4, HAS_PUSH, PA, e.eps, X14,
-        e.rscale);
-    GEMB_CUDA(cudaGetLastError());
-    count_launch(2);
-    return GEMB_OK;
+    return launch(ctx, spmm_heavy_finish_kernel<HAS_X0, HAS_SELF, HAS_X1, HAS_SCALE>, fgrid, 256, 0, A.n_heavy, A.heavy_row,
+                  A.heavy_first, G, e.alpha, e.gamma, e.delta, P4, XS4, X04, Y4, HAS_PUSH, PA, e.eps, X14, e.rscale);
 }
 
 int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, const float *X, float *Y,
@@ -281,14 +273,6 @@ int spmm_launch(gemb_ctx *ctx, const gemb_csr_dev &A, int64_t n_rows, int b, con
     return spmm_sweep<false, false, false, false, false>(ctx, A, n_rows, b, X, Y, e);
 }
 
-// a host block of `count` floats into a new device block (src null: none, dst stays null)
-static int stage(gemb_ctx *c, DeviceBuffer<float> &dst, const float *src, size_t count) {
-    if (!src) return GEMB_OK;
-    GEMB_CUDA(dst.alloc(count));
-    GEMB_CUDA(cudaMemcpyAsync(dst.get(), src, sizeof(float) * count, cudaMemcpyHostToDevice, c->stream));
-    return GEMB_OK;
-}
-
 // The sweep of the test hooks from host memory: X (all n rows) and the epilogue's blocks (the shard's rows) to the
 // device, one sweep of A or A^T over the shard, Y back.
 static int spmm_host(gemb_graph *g, int transpose, int b, const float *X, SpmmEpilogue e, float *Y) {
@@ -296,17 +280,15 @@ static int spmm_host(gemb_graph *g, int transpose, int b, const float *X, SpmmEp
     GEMB_CUDA(cudaSetDevice(c->device));
     DeviceBuffer<float> dX, dY, dXs, dX0, dX1, dS;
     const size_t shard = (size_t)g->n_local * b;
-    GEMB_TRY(stage(c, dX, X, (size_t)g->n * b));
-    GEMB_TRY(stage(c, dXs, e.Xself, shard));
-    GEMB_TRY(stage(c, dX0, e.X0, shard));
-    GEMB_TRY(stage(c, dX1, e.X1, shard));
-    GEMB_TRY(stage(c, dS, e.rscale, (size_t)g->n_local));
+    GEMB_CUDA(dX.upload(X, (size_t)g->n * b, c->stream));
+    if (e.Xself) GEMB_CUDA(dXs.upload(e.Xself, shard, c->stream));   // an absent operand stays a null pointer
+    if (e.X0) GEMB_CUDA(dX0.upload(e.X0, shard, c->stream));
+    if (e.X1) GEMB_CUDA(dX1.upload(e.X1, shard, c->stream));
+    if (e.rscale) GEMB_CUDA(dS.upload(e.rscale, (size_t)g->n_local, c->stream));
     GEMB_CUDA(dY.alloc(shard));
     e.Xself = dXs.get(); e.X0 = dX0.get(); e.X1 = dX1.get(); e.rscale = dS.get();
     GEMB_TRY(spmm_launch(c, transpose ? g->AT : g->A, g->n_local, b, dX.get(), dY.get(), e));
-    GEMB_CUDA(cudaMemcpyAsync(Y, dY.get(), sizeof(float) * shard, cudaMemcpyDeviceToHost, c->stream));
-    GEMB_CUDA(cudaStreamSynchronize(c->stream));
-    return GEMB_OK;
+    return copy_sync(c, Y, dY.get(), sizeof(float) * shard, cudaMemcpyDeviceToHost);
 }
 
 }  // namespace gemb

@@ -97,47 +97,38 @@ static int rmat_generate(gemb_ctx *ctx, int scale, int edge_factor, double a, do
     cub::DeviceSelect::Unique(nullptr, need, keys2.get(), keys.get(), d_cnt.get(), nk, st); tb = std::max(tb, need);
     GEMB_CUDA(tmp.alloc(tb));
     if (permute) {
-        rmat_perm_keys_kernel<<<grid, 256, 0, st>>>(n, seed, pk.get(), pv.get());
-        GEMB_CUDA(cudaGetLastError());
+        GEMB_TRY(launch(ctx, rmat_perm_keys_kernel, grid, 256, 0, n, seed, pk.get(), pv.get()));
         GEMB_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tb, pk.get(), pk2.get(), pv.get(), perm.get(), n, 0, 64, st));
-        count_launch(2);
+        count_launch();
     }
     const uint32_t ta = (uint32_t)std::min(4294967295.0, a * 4294967296.0);
     const uint32_t tab = (uint32_t)std::min(4294967295.0, (a + b) * 4294967296.0);
     const uint32_t tabc = (uint32_t)std::min(4294967295.0, (a + b + c) * 4294967296.0);
-    rmat_pairs_kernel<<<grid, 256, 0, st>>>(m, scale, ta, tab, tabc, seed, permute ? perm.get() : nullptr, keys.get());
-    GEMB_CUDA(cudaGetLastError());
+    GEMB_TRY(launch(ctx, rmat_pairs_kernel, grid, 256, 0, m, scale, ta, tab, tabc, seed, permute ? perm.get() : nullptr, keys.get()));
     GEMB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.get(), tb, keys.get(), keys2.get(), nk, 0, 64, st));
     GEMB_CUDA(cub::DeviceSelect::Unique(tmp.get(), tb, keys2.get(), keys.get(), d_cnt.get(), nk, st));
-    count_launch(3);
+    count_launch(2);
     int64_t nu = 0;
-    GEMB_CUDA(cudaMemcpyAsync(&nu, d_cnt.get(), 8, cudaMemcpyDeviceToHost, st));
-    GEMB_CUDA(cudaStreamSynchronize(st));
+    GEMB_TRY(copy_sync(ctx, &nu, d_cnt.get(), 8, cudaMemcpyDeviceToHost));
     uint64_t last = 0;
     if (nu > 0) {
-        GEMB_CUDA(cudaMemcpyAsync(&last, keys.get() + (nu - 1), 8, cudaMemcpyDeviceToHost, st));
-        GEMB_CUDA(cudaStreamSynchronize(st));
+        GEMB_TRY(copy_sync(ctx, &last, keys.get() + (nu - 1), 8, cudaMemcpyDeviceToHost));
         if (last == ~0ull) nu--;                                   // the self-loop sentinel
     }
     if (nnz_total_out) *nnz_total_out = nu;
     GEMB_CUDA(d_ip.alloc(n_rows + 1));
-    rmat_rowptr_kernel<<<grid, 256, 0, st>>>(n_rows, row0, keys.get(), nu, d_ip.get(), d_cnt.get() + 1);
-    GEMB_CUDA(cudaGetLastError());
+    GEMB_TRY(launch(ctx, rmat_rowptr_kernel, grid, 256, 0, n_rows, row0, keys.get(), nu, d_ip.get(), d_cnt.get() + 1));
     int64_t ends[2] = {0, 0};
     GEMB_CUDA(cudaMemcpyAsync(&ends[0], d_ip.get(), 8, cudaMemcpyDeviceToHost, st));
     GEMB_CUDA(cudaMemcpyAsync(&ends[1], d_ip.get() + n_rows, 8, cudaMemcpyDeviceToHost, st));
     GEMB_CUDA(cudaStreamSynchronize(st));
     const int64_t cnt = ends[1] - ends[0];
     if (nnz_out) *nnz_out = cnt;
-    count_launch();
     if (!indices_out) return GEMB_OK;
     GEMB_ARG(indptr_out && cap >= cnt, "indptr_out / cap");
-    rmat_rebase_kernel<<<grid, 256, 0, st>>>(n_rows, d_ip.get(), d_cnt.get() + 1);
-    GEMB_CUDA(cudaGetLastError());
+    GEMB_TRY(launch(ctx, rmat_rebase_kernel, grid, 256, 0, n_rows, d_ip.get(), d_cnt.get() + 1));
     GEMB_CUDA(cols.alloc(std::max<int64_t>(cnt, 1)));
-    rmat_cols_kernel<<<grid, 256, 0, st>>>(cnt, keys.get() + ends[0], cols.get());
-    GEMB_CUDA(cudaGetLastError());
-    count_launch(2);
+    GEMB_TRY(launch(ctx, rmat_cols_kernel, grid, 256, 0, cnt, keys.get() + ends[0], cols.get()));
     GEMB_CUDA(cudaMemcpyAsync(indptr_out, d_ip.get(), 8 * (size_t)(n_rows + 1), cudaMemcpyDeviceToHost, st));
     GEMB_CUDA(cudaMemcpyAsync(indices_out, cols.get(), 4 * (size_t)cnt, cudaMemcpyDeviceToHost, st));
     GEMB_CUDA(cudaStreamSynchronize(st));
