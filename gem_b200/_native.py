@@ -22,7 +22,7 @@ EXPORTS = [
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
     'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
     'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk', 'gemb_cc_create', 'gemb_cc_info', 'gemb_cc_labels', 'gemb_cc_lcc',
-    'gemb_cc_times', 'gemb_cc_free',
+    'gemb_cc_times', 'gemb_cc_free', 'gemb_tsne', 'gemb_tsne_affinities', 'gemb_tsne_gradient',
 ]
 
 
@@ -69,6 +69,20 @@ class NCStats(_Stats):
 
 
 NC_CONVERGED, NC_CONSTANT, NC_MAXITER, NC_STALLED = 1, 2, 3, 4
+
+
+class TsneOpts(ctypes.Structure):
+    _fields_ = [('struct_size', ctypes.c_uint32), ('max_iter', ctypes.c_int32), ('n_iter_without_progress', ctypes.c_int32),
+                ('perplexity', ctypes.c_double), ('early_exaggeration', ctypes.c_double),
+                ('learning_rate', ctypes.c_double), ('min_grad_norm', ctypes.c_double), ('angle', ctypes.c_double)]
+
+
+class TsneStats(_Stats):
+    _fields_ = [('struct_size', ctypes.c_uint32), ('n_neighbors', ctypes.c_int32), ('n_iter', ctypes.c_int32),
+                ('nnz_P', ctypes.c_int64), ('kl_divergence', ctypes.c_double), ('knn_ms', ctypes.c_double),
+                ('calib_ms', ctypes.c_double), ('sym_ms', ctypes.c_double), ('pca_ms', ctypes.c_double),
+                ('opt_ms', ctypes.c_double), ('total_ms', ctypes.c_double), ('tree_ms', ctypes.c_double),
+                ('grad_ms', ctypes.c_double)]
 
 
 def lib():
@@ -141,6 +155,10 @@ def lib():
     L.gemb_cc_lcc.argtypes = [vp, vp, vp, vp, vp, vp]
     L.gemb_cc_times.argtypes = [vp, ctypes.POINTER(f64), ctypes.POINTER(f64)]
     L.gemb_cc_free.argtypes = [vp]
+    L.gemb_tsne.argtypes = [vp, i64, ctypes.c_int, vp, ctypes.POINTER(TsneOpts), vp, ctypes.POINTER(TsneStats)]
+    L.gemb_tsne_affinities.argtypes = [vp, i64, ctypes.c_int, vp, f64, i64, vp, vp, vp, vp, vp, vp, ctypes.POINTER(i32),
+                                       ctypes.POINTER(i64)]
+    L.gemb_tsne_gradient.argtypes = [vp, i64, vp, vp, vp, vp, f64, vp, ctypes.POINTER(f64)]
     _lib = L
     return L
 
@@ -555,6 +573,56 @@ def nc_topk(ctx, X, W, koff):
     out = np.empty(max(int(koff[-1]), 1), dtype=np.int32)
     check(lib().gemb_nc_topk(ctx._h, m, d, _ptr(X), W.shape[0], _ptr(W), _ptr(koff), _ptr(out)))
     return out[:int(koff[-1])]
+
+
+def tsne(ctx, X, perplexity, early_exaggeration, learning_rate, max_iter, n_iter_without_progress, min_grad_norm,
+         angle):
+    """gemb_tsne: the n x 2 float32 t-SNE positions of the rows of X, and the stats dict.  learning_rate is a number
+    (the caller resolves 'auto')."""
+    X = np.ascontiguousarray(X, dtype=np.float32)
+    n, d = X.shape
+    o = TsneOpts(struct_size=ctypes.sizeof(TsneOpts), max_iter=int(max_iter),
+                 n_iter_without_progress=int(n_iter_without_progress), perplexity=float(perplexity),
+                 early_exaggeration=float(early_exaggeration), learning_rate=float(learning_rate),
+                 min_grad_norm=float(min_grad_norm), angle=float(angle))
+    st = TsneStats(struct_size=ctypes.sizeof(TsneStats))
+    Y = np.empty((n, 2), dtype=np.float32)
+    check(lib().gemb_tsne(ctx._h, n, d, _ptr(X), ctypes.byref(o), _ptr(Y), ctypes.byref(st)))
+    return Y, st.as_dict()
+
+
+def tsne_affinities(ctx, X, perplexity):
+    """gemb_tsne_affinities: dict of knn_idx / knn_d2 (n x k, ascending by (d^2, index)), p_cond (n x k, same order)
+    and the joint P as CSR (p_indptr, p_indices, p_val)."""
+    X = np.ascontiguousarray(X, dtype=np.float32)
+    n, d = X.shape
+    k, nnz = ctypes.c_int32(0), ctypes.c_int64(0)
+    args = (ctx._h, n, d, _ptr(X), float(perplexity))
+    check(lib().gemb_tsne_affinities(*args, 0, None, None, None, None, None, None, ctypes.byref(k), ctypes.byref(nnz)))
+    k, m = int(k.value), int(nnz.value)
+    out = dict(knn_idx=np.empty((n, k), np.int32), knn_d2=np.empty((n, k), np.float32), p_cond=np.empty((n, k), np.float64),
+               p_indptr=np.empty(n + 1, np.int64), p_indices=np.empty(max(m, 1), np.int32), p_val=np.empty(max(m, 1), np.float64))
+    check(lib().gemb_tsne_affinities(*args, max(m, 1), *(_ptr(out[key]) for key in ('knn_idx', 'knn_d2', 'p_cond', 'p_indptr',
+                                                                                   'p_indices', 'p_val')),
+                                     ctypes.byref(ctypes.c_int32(0)), ctypes.byref(ctypes.c_int64(0))))
+    out['p_indices'], out['p_val'] = out['p_indices'][:m], out['p_val'][:m]
+    return out
+
+
+def tsne_gradient(ctx, Y, p_indptr, p_indices, p_val, angle):
+    """gemb_tsne_gradient: (grad n x 2 float32 including the factor 4, KL error) at positions Y for the CSR joint P."""
+    Y = np.ascontiguousarray(Y, dtype=np.float32)
+    n = Y.shape[0]
+    assert Y.shape == (n, 2)
+    p_indptr = np.ascontiguousarray(p_indptr, dtype=np.int64)
+    p_indices = np.ascontiguousarray(p_indices, dtype=np.int32)
+    p_val = np.ascontiguousarray(p_val, dtype=np.float64)
+    assert p_indptr.shape == (n + 1,) and p_indices.shape[0] >= int(p_indptr[-1]) and p_val.shape[0] >= int(p_indptr[-1])
+    g = np.empty((n, 2), dtype=np.float32)
+    kl = ctypes.c_double(0.0)
+    check(lib().gemb_tsne_gradient(ctx._h, n, _ptr(Y), _ptr(p_indptr), _ptr(p_indices), _ptr(p_val), float(angle), _ptr(g),
+                                   ctypes.byref(kl)))
+    return g, float(kl.value)
 
 
 class Components(_Handle):

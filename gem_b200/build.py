@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, 'csrc', 'build')
 LIB = os.path.join(HERE, 'libgemb200.so')
-SOURCES = ['core.cu', 'spmm.cu', 'dense.cu', 'gram_tc.cu', 'apply_tc.cu', 'hope.cu', 'halo.cu', 'n2v.cu', 'recon.cu', 'ingest.cu', 'synth.cu', 'gf.cu', 'nc.cu', 'cc.cu']
+SOURCES = ['core.cu', 'spmm.cu', 'dense.cu', 'gram_tc.cu', 'apply_tc.cu', 'hope.cu', 'halo.cu', 'n2v.cu', 'recon.cu', 'ingest.cu', 'synth.cu', 'gf.cu', 'nc.cu', 'cc.cu', 'tsne.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 CFLAGS = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=default',

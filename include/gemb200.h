@@ -447,6 +447,61 @@ int gemb_cc_lcc(gemb_cc *cc, const double *data, int64_t *node_l_out, int64_t *i
 int gemb_cc_times(gemb_cc *cc, double *label_ms, double *extract_ms);
 int gemb_cc_free(gemb_cc *cc);
 
+/* ---- t-SNE to two dimensions: the TSNE(n_components=2).fit_transform(node_pos) of plot_embedding2D
+ * (visualize_embedding.py:7-12), restated from sklearn 1.9's defaults (init='pca', method='barnes_hut', euclidean).
+ * X: host, n x d row-major fp32, finite, n >= 2, d >= 1.  Y_out: host, n x 2 fp32.
+ *   kNN          k = min(n - 1, floor(3 perplexity + 1)) exact nearest rows, selected by fp32 d^2 = sum_c (x_c - y_c)^2,
+ *                ties to the lower index, the row itself excluded (_t_sne.py TSNE._fit; NearestNeighbors is brute force
+ *                for d > 15); the k d^2 are then summed in fp64 and rounded to fp32, as sklearn rounds its fp64 distances.
+ *                k <= 320 (perplexity < 106.33 for n > 320), else GEMB_ERR_UNSUPPORTED.
+ *   calibration  _utils.pyx _binary_search_perplexity, in fp64.
+ *   joint P      _t_sne.py _joint_probabilities_nn: (P_cond + P_cond^T) / sum, fp64, exact zeros dropped.
+ *   start        PCA(n_components=2) scores with svd_flip(u_based_decision=False) signs, column 0 scaled to standard
+ *                deviation 1e-4 (TSNE._fit, init='pca').
+ *   gradient     _barnes_hut_tsne.pyx gradient on _quad_tree.pyx's cells, times c = 2 (dof + 1) / dof = 4.
+ *   optimiser    _t_sne.py _gradient_descent as TSNE._tsne runs it: 250 iterations (or max_iter, if fewer) at momentum
+ *                0.5 with P times early_exaggeration, then momentum 0.8 up to max_iter; the KL error and the
+ *                n_iter_without_progress / min_grad_norm stops every 50 iterations.  max_iter = 0 returns the start.
+ * Refused with GEMB_ERR_ARG before any device work: X not finite, perplexity outside (0, n), early_exaggeration or
+ * learning_rate <= 0 (the caller resolves sklearn's 'auto', max(n / early_exaggeration / 4, 50)), angle outside [0, 1],
+ * negative max_iter, n_iter_without_progress or min_grad_norm.  Two calls give the same bits. */
+typedef struct {
+    uint32_t struct_size;            /* = sizeof(gemb_tsne_opts) */
+    int32_t max_iter;                /* sklearn: 1000 */
+    int32_t n_iter_without_progress; /* sklearn: 300 */
+    double perplexity;               /* sklearn: 30 */
+    double early_exaggeration;       /* sklearn: 12 */
+    double learning_rate;            /* > 0 */
+    double min_grad_norm;            /* sklearn: 1e-7 */
+    double angle;                    /* sklearn: 0.5 */
+} gemb_tsne_opts;
+typedef struct {
+    uint32_t struct_size;  /* = sizeof(gemb_tsne_stats) */
+    int32_t n_neighbors;   /* k */
+    int32_t n_iter;        /* TSNE.n_iter_: the last iteration run (-1 when max_iter = 0) */
+    int64_t nnz_P;         /* entries of the joint P */
+    double kl_divergence;  /* the KL error of the last iteration (TSNE.kl_divergence_); 0 when max_iter = 0 */
+    double knn_ms, calib_ms, sym_ms, pca_ms, opt_ms, total_ms;   /* host clock per stage, each ending in a synchronise */
+    double tree_ms, grad_ms;   /* device time (events) summed over the iterations: quadtree build; repulsive walk,
+                                  attractive sweep and update */
+} gemb_tsne_stats;
+int gemb_tsne(gemb_ctx *ctx, int64_t n, int d, const float *X, const gemb_tsne_opts *opts, float *Y_out,
+              gemb_tsne_stats *stats);
+
+/* Test hook: the affinities of gemb_tsne.  Call with cap = 0 to get *k_out and *nnz_out, then with cap >= nnz and
+ * every array: knn_idx_out / knn_d2_out (n x k, each row ascending by (d^2, index)), p_cond_out (n x k, the conditional
+ * P of _binary_search_perplexity in the same order), and the joint P as CSR (p_indptr_out n + 1, p_indices_out and
+ * p_val_out nnz, column ids ascending per row). */
+int gemb_tsne_affinities(gemb_ctx *ctx, int64_t n, int d, const float *X, double perplexity, int64_t cap,
+                         int32_t *knn_idx_out, float *knn_d2_out, double *p_cond_out, int64_t *p_indptr_out,
+                         int32_t *p_indices_out, double *p_val_out, int32_t *k_out, int64_t *nnz_out);
+
+/* Test hook: _kl_divergence_bh at positions Y (host, n x 2 fp32) for the joint P given as CSR (host; p_indptr n + 1
+ * int64, p_indices int32, p_val fp64): grad_out (n x 2, including the factor 4) and *kl_out (may be NULL).  angle 0
+ * gives the exact gradient except for the pairs sklearn's tree also leaves out (points within 1e-6 of each other). */
+int gemb_tsne_gradient(gemb_ctx *ctx, int64_t n, const float *Y, const int64_t *p_indptr, const int32_t *p_indices,
+                       const double *p_val, double angle, float *grad_out, double *kl_out);
+
 /* ---- wire formats (SURVEY 8(f) rank 2): the reference's text files, read and written natively and in parallel.
  * HOST code only -- these entry points need no GPU.
  * Edge list: every non-blank line "src dst [weight]" (loadGraphFromEdgeListTxt, graph_util.py:143-158: exactly three
