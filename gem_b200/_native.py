@@ -20,7 +20,7 @@ EXPORTS = [
     'gemb_graph_free', 'gemb_spmm', 'gemb_spmm4', 'gemb_spmm_scaled', 'gemb_gram', 'gemb_apply', 'gemb_chol_inverse', 'gemb_eigh', 'gemb_hope',
     'gemb_hope_apply', 'gemb_hope_svd_error', 'gemb_n2v_alias', 'gemb_n2v_walks', 'gemb_node2vec',
     'gemb_edge_list_scan', 'gemb_edge_list_parse', 'gemb_edge_list_write', 'gemb_emb_read', 'gemb_emb_write',
-    'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
+    'gemb_synth_rmat', 'gemb_gf', 'gemb_recon_create', 'gemb_recon_create_blocked', 'gemb_recon_info', 'gemb_recon_free', 'gemb_recon_dense', 'gemb_recon_pairs', 'gemb_recon_ranks', 'gemb_recon_top',
     'gemb_recon_exclude', 'gemb_nc_fit', 'gemb_nc_topk', 'gemb_cc_create', 'gemb_cc_info', 'gemb_cc_labels', 'gemb_cc_lcc',
     'gemb_cc_times', 'gemb_cc_free', 'gemb_tsne', 'gemb_tsne_affinities', 'gemb_tsne_gradient',
 ]
@@ -140,6 +140,8 @@ def lib():
                                   ctypes.POINTER(i64), ctypes.POINTER(i64), vp, vp, i64]
     L.gemb_gf.argtypes = [vp, i64, i64, vp, vp, vp, ctypes.c_int, f32, f32, ctypes.c_int, ctypes.c_int, vp, vp, ctypes.POINTER(f64)]
     L.gemb_recon_create.argtypes = [vp, vp, i64, ctypes.c_int, ctypes.c_int, ctypes.POINTER(vp)]
+    L.gemb_recon_create_blocked.argtypes = [vp, vp, i64, ctypes.c_int, ctypes.c_int, i64, ctypes.POINTER(vp)]
+    L.gemb_recon_info.argtypes = [vp, ctypes.POINTER(i64), ctypes.POINTER(i64)]
     L.gemb_recon_free.argtypes = [vp]
     L.gemb_recon_dense.argtypes = [vp, vp]
     L.gemb_recon_pairs.argtypes = [vp, vp, vp, i64, vp]
@@ -481,10 +483,14 @@ class Reconstruction(_Handle):
     halves of the columns.  For both, dense / pairs / the w of top return A_hat (0 on the diagonal).
     kind 2: score exp(-delta) with delta = |x_i - x_j|^2 (fp32).  dense / pairs / the w of top return delta itself,
     +inf on the diagonal and where the fp64 score underflows to 0 (delta > 745.1332), so exp(-out) is the score
-    everywhere; ranks / top order by delta ascending.  A non-finite X raises."""
+    everywhere; ranks / top order by delta ascending.  A non-finite X raises.
+
+    The matrix is made of blocks of 64-column panels (gemb_recon_create_blocked): panels_per_block = 0 keeps it whole
+    on the device when it fits and otherwise regenerates it block by block in every call; a positive value forces
+    that block size (test hook).  `blocks` is the number of blocks (1: the matrix is kept)."""
     _destroy = 'gemb_recon_free'
 
-    def __init__(self, ctx, X, kind):
+    def __init__(self, ctx, X, kind, panels_per_block=0):
         X = np.ascontiguousarray(X, dtype=np.float32)
         assert X.ndim == 2
         self.ctx = ctx
@@ -492,7 +498,15 @@ class Reconstruction(_Handle):
         kind = int(kind)
         self.kind = kind if kind in (RECON_DOT, RECON_GAUSS) else RECON_SPLIT
         self._h = ctypes.c_void_p()
-        check(lib().gemb_recon_create(ctx._h, _ptr(X), self.n, self.d, self.kind, ctypes.byref(self._h)))
+        check(lib().gemb_recon_create_blocked(ctx._h, _ptr(X), self.n, self.d, self.kind, int(panels_per_block),
+                                              ctypes.byref(self._h)))
+        ppb, blocks = ctypes.c_int64(0), ctypes.c_int64(0)
+        check(lib().gemb_recon_info(self._h, ctypes.byref(ppb), ctypes.byref(blocks)))
+        self.panels_per_block, self._blocks = int(ppb.value), int(blocks.value)
+
+    @property
+    def blocks(self):
+        return self._blocks
 
     def dense(self, out=None):
         A = out if out is not None else np.empty((self.n, self.n), dtype=np.float32)

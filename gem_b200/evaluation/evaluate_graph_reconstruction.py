@@ -13,7 +13,9 @@ lle.py:37-40); a model says which through its `_recon_split` or `_recon_score` a
 device returns delta = |x_i - x_j|^2 and the order is delta ascending (stable), which is the reference's descending
 score order; the weighted error uses exp(-delta) in fp64.
 `max_k` (extra, optional): length of the precision curve to return; the reference always returns all
-n_pred entries (max_k = -1, default here too).
+n_pred entries (max_k = -1, default here too).  When the reconstruction does not fit in device memory it is
+regenerated block by block (gemb_recon_create); the full curve is then every positive entry of a matrix too large for
+the device, so max_k < 0 raises ValueError before any pass over it.
 """
 import numpy as np
 
@@ -42,6 +44,15 @@ def _true_csr(digraph, node_num):
     indptr = np.zeros(node_num + 1, dtype=np.int64)
     np.add.at(indptr, e[:, 0] + 1, 1)
     return np.cumsum(indptr), e[:, 1].copy()
+
+
+def check_max_k(rec, max_k):
+    """ValueError when the whole precision curve (max_k < 0) is asked of a reconstruction regenerated in blocks.
+    Stand-ins for the handle without `blocks` hold their matrix whole."""
+    blocks = getattr(rec, 'blocks', 1)
+    if max_k < 0 and blocks > 1:
+        raise ValueError('max_k = %d asks for every predicted edge of a %d x %d reconstruction that does not fit in '
+                         'device memory (regenerated in %d blocks); pass max_k >= 0' % (max_k, rec.n, rec.n, blocks))
 
 
 def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=None, file_suffix=None,
@@ -80,6 +91,7 @@ def evaluateStaticGraphReconstruction(digraph, graph_embedding, X_stat, node_l=N
             MAP = total / count if count else float('nan')
             prec_curv, _ = metrics.precision_curve(pi, pj, pw, has_edge)
         else:
+            check_max_k(rec, max_k)
             ranks, _ = rec.ranks(indptr, indices, is_undirected)
             MAP, _, _ = metrics.map_from_ranks(node_num, indptr, ranks, is_undirected)
             ti, tj, tw = rec.top(is_undirected, max_k)

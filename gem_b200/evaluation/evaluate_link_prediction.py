@@ -22,13 +22,15 @@ digraph: a networkx DiGraph with nodes 0..n-1 or a gem_b200.graph.HostCSR (then 
 CSR form: no networkx at any size).  The embedding's rows are taken as node ids, as evaluateStaticGraphReconstruction
 does.  With lcc=True the embedding is learned on the largest component, and node ids are its 0..k-1.  The default
 lcc=False keeps every node; on a training graph that is one component both give the same bits.  -> (MAP, prec_curv)
+A reconstruction too large for device memory is regenerated block by block; max_k < 0 then raises ValueError (as in
+evaluateStaticGraphReconstruction).
 """
 import numpy as np
 
 from gem_b200 import _native
 from gem_b200.embedding.static_graph_embedding import recon_kind
 from gem_b200.evaluation import metrics
-from gem_b200.evaluation.evaluate_graph_reconstruction import _true_csr
+from gem_b200.evaluation.evaluate_graph_reconstruction import _true_csr, check_max_k
 
 
 def split_and_sample(digraph, train_ratio=0.8, n_sample_nodes=None, is_undirected=True, rng=None, lcc=False,
@@ -100,6 +102,7 @@ def evaluateStaticLinkPrediction(digraph, graph_embedding, train_ratio=0.8, n_sa
             MAP = total / count if count else float('nan')
             prec_curv, _ = metrics.precision_curve(pi, pj, pw, in_test, max_k)
         else:
+            check_max_k(rec, max_k)
             rec.exclude(tr_indptr, tr_indices)
             ranks, _ = rec.ranks(te_indptr, te_indices, is_undirected)
             MAP, _, _ = metrics.map_from_ranks(n, te_indptr, ranks, False)

@@ -327,7 +327,15 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
 
 /* ---- reconstruction and its evaluation (SURVEY 8(f) rank 1; the step after learn_embedding in tests/fit_model.py:10).
  * gemb_recon_create replaces the n^2 get_edge_weight calls of static_graph_embedding.py:48-65: A_hat = L R^T with a
- * zero diagonal, kept ON THE DEVICE (n x n fp32; GEMB_ERR_NOMEM with a message when it does not fit).
+ * zero diagonal, ON THE DEVICE, made of 64-column panels (n x 64 fp32 each, n * 256 bytes) in BLOCKS of consecutive
+ * panels.  When the whole n x n matrix fits in 0.9 x (free + cached) device memory beside X and the factors, it is one
+ * block, made at create and kept: every call below reads it.  Otherwise the handle keeps X and the factors plus one
+ * block buffer of as many panels as fit (leaving 1 GiB + 16 bytes per node for the calls' scratch), and every call
+ * regenerates the blocks in order -- a PASS, costing the product once more (4 n^2 bytes written and read):
+ *   ranks: 2 passes (the true edges' scores, then the counting); top: 1 pass for the count when every candidate is
+ *   returned (max_k < 0 or max_k >= the count), else 2, and 1 more for the entries; pairs: the blocks that hold a
+ *   pair's column; dense: 1 pass.  The scores are the same bits in both modes.  GEMB_ERR_NOMEM only when not even one
+ *   panel fits.
  *   kind = 1 (or any value other than 0 and 2): L = X[:, :d/2], R = X[:, d/2:]
  *                                                 (HOPE.get_edge_weight, hope.py:43-44)
  *   kind = 0: L = R = X                          (node2vec.get_edge_weight, node2vec.py:56-57)
@@ -343,6 +351,13 @@ int gemb_node2vec(gemb_graph *g, const double *weights64, const int32_t *nids, i
 #define GEMB_RECON_GAUSS 2
 typedef struct gemb_recon gemb_recon;
 int gemb_recon_create(gemb_ctx *ctx, const float *X, int64_t n, int d, int kind, gemb_recon **out);
+/* gemb_recon_create with the block size given (test hook): panels_per_block > 0 makes blocks of that many panels (one
+ * block when they cover all ceil(n / 64) panels; GEMB_ERR_NOMEM when they do not fit), 0 chooses as gemb_recon_create
+ * does. */
+int gemb_recon_create_blocked(gemb_ctx *ctx, const float *X, int64_t n, int d, int kind, int64_t panels_per_block,
+                              gemb_recon **out);
+/* The block layout: panels per block and number of blocks (1: the matrix stays on the device between calls). */
+int gemb_recon_info(gemb_recon *r, int64_t *panels_per_block, int64_t *blocks);
 int gemb_recon_free(gemb_recon *r);
 
 /* The dense matrix get_reconstructed_adj returns (static_graph_embedding.py:48-65): adj_out host, n x n row-major
@@ -377,9 +392,9 @@ int gemb_recon_top(gemb_recon *r, int is_undirected, int64_t max_k, int64_t cap,
  * to the device; ex_indptr == NULL clears it.  While it is set, gemb_recon_ranks and gemb_recon_top report their
  * results over the candidates NOT in it: a true edge that is itself excluded gets rank 0, n_pred_row counts only the
  * remaining candidates, and top selects among them.  Without an exclusion both are unchanged.  Setting or clearing it
- * drops the cached top selection.  Cost: ranks and top run their usual passes with the excluded entries set to 0
- * for the length of the call -- one scatter over the exclusion before them and one after, which puts the values
- * back, so gemb_recon_dense and gemb_recon_pairs never see the zeros. */
+ * drops the cached top selection.  Cost: ranks and top run their usual passes with the excluded entries of each block
+ * set to 0 while that block is counted -- one scatter over the block's share of the exclusion before and one after,
+ * which puts the values back, so gemb_recon_dense and gemb_recon_pairs never see the zeros. */
 int gemb_recon_exclude(gemb_recon *r, const int32_t *ex_indptr, const int32_t *ex_indices);
 
 /* ---- node classification (upstream GEM's evaluateNodeClassification: OneVsRestClassifier(LogisticRegression()) and
