@@ -23,7 +23,10 @@
 //                   easier down the chain, so testing the deepest cell of the chain decides the same way.  A binary
 //                   node in the same quadtree cell as its parent (a split on the cell's second bit) is not a quadtree
 //                   cell and is passed through untested.  A cell is a leaf when all its points lie within 1e-6 of its
-//                   lowest-index point (sklearn inserts in index order, so that point is its leaf's barycentre).
+//                   lowest-index point (sklearn inserts in index order, so that point is its leaf's barycentre).  Points
+//                   whose 32-level paths are equal but which are not such duplicates (a root wider than ~2^32 * 1e-6)
+//                   are not a leaf: the walk goes on through the index-split nodes below, all in the same depth-32 cell
+//                   and so untested, to the single points, as sklearn's deeper cells separate them.
 //                   Counts, barycentres and bounding boxes are combined bottom-up, left child first (integer visit
 //                   counters, no floating-point atomics), and every sum is in a fixed order: two runs give the same bits.
 //   6. optimiser    _gradient_descent / TSNE._tsne: 250 iterations at momentum 0.5 with P exaggerated, then momentum 0.8;
@@ -42,6 +45,7 @@ namespace gemb {
 
 constexpr int KNN_QB = 64, KNN_CB = 128, KNN_KC = 32;   // query rows per CTA, candidate columns per tile, dims per stage
 constexpr int TSNE_KMAX = 320;                          // the row lists of a CTA fit in shared memory up to here
+constexpr int TSNE_DMAX = 1024;                         // the PCA start's eigh_launch: one Jacobi rotation pair per thread
 constexpr int TSNE_STACK = 128;                         // traversal depth: 64 key bits + 32 index bits of tie-break
 constexpr float TSNE_DUP_EPS = 1e-6f;                   // _quad_tree.pyx EPSILON
 constexpr float FLOAT32_TINY = 1.17549435e-38f;         // np.finfo(np.float32).tiny
@@ -534,7 +538,7 @@ __global__ void tsne_bottom_up_kernel(TsneTree T, const float *__restrict__ Y) {
         const float px = Y[2 * m], py = Y[2 * m + 1];
         const bool dup = bx.z - px <= TSNE_DUP_EPS && px - bx.x <= TSNE_DUP_EPS && bx.w - py <= TSNE_DUP_EPS &&
                          py - bx.y <= TSNE_DUP_EPS;
-        const bool lf = dl >= 64 || dup;
+        const bool lf = dup;      // equal keys alone are not a leaf: below 32 levels sklearn splits until points separate
         const float sqw = tsne_cell_sqw(r, T.keys[T.first[v]], L);
         T.cnt[v] = c;
         T.minidx[v] = m;
@@ -613,7 +617,7 @@ __global__ void __launch_bounds__(256) tsne_step_kernel(int64_t n, const int64_t
     __shared__ double red[8];
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     double err = 0.0, gn = 0.0;
-    const double sQ = *sum_q;
+    const double sQ = fmax(*sum_q, 2.220446049250313e-16);     // compute_gradient_negative's floor (FLOAT64_EPS)
     float g[2] = {0.f, 0.f};
     if (i < n) {
         const float xi = Y[2 * i], yi = Y[2 * i + 1];
@@ -940,6 +944,10 @@ extern "C" int gemb_tsne(gemb_ctx *ctx, int64_t n, int d, const float *X, const 
              "max_iter, n_iter_without_progress, min_grad_norm >= 0");
     if (tsne_k(n, o.perplexity) > TSNE_KMAX) {
         set_error("k = min(n - 1, 3 perplexity + 1) = %d exceeds %d", tsne_k(n, o.perplexity), TSNE_KMAX);
+        return GEMB_ERR_UNSUPPORTED;
+    }
+    if (d > TSNE_DMAX) {
+        set_error("d = %d exceeds %d, the width of the PCA start's Jacobi eigensolver", d, TSNE_DMAX);
         return GEMB_ERR_UNSUPPORTED;
     }
     GEMB_CUDA(cudaSetDevice(ctx->device));

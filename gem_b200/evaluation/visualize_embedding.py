@@ -24,7 +24,8 @@ def _positive(name, v):
 def tsne(X, perplexity=30.0, early_exaggeration=12.0, learning_rate='auto', max_iter=1000, n_iter_without_progress=300,
          min_grad_norm=1e-7, angle=0.5, device=None, stats=None):
     """The n x 2 float32 t-SNE positions of the rows of X (sklearn's TSNE(n_components=2).fit_transform(X) with the
-    same parameters).  learning_rate 'auto' is sklearn's max(n / early_exaggeration / 4, 50).
+    same parameters).  learning_rate 'auto' is sklearn's max(n / early_exaggeration / 4, 50).  X has at most 1024
+    columns (the width of the PCA start's eigensolver).
     stats: an optional dict, filled with kl_divergence, n_iter, learning_rate, n_neighbors, nnz_P and the host-clock
     milliseconds of every stage (knn_ms, calib_ms, sym_ms, pca_ms, opt_ms, total_ms; tree_ms and grad_ms are the
     device time of the quadtree builds and of the gradient steps, summed over the iterations) and of the whole call
@@ -34,6 +35,8 @@ def tsne(X, perplexity=30.0, early_exaggeration=12.0, learning_rate='auto', max_
         raise ValueError('X must be an n x d matrix with n >= 2 and d >= 1, got shape %s' % (X.shape,))
     if not np.issubdtype(X.dtype, np.number) or not np.all(np.isfinite(X)):
         raise ValueError('X must be finite')
+    if X.shape[1] > 1024:
+        raise ValueError('X has %d columns; the Jacobi eigensolver of the PCA start takes at most 1024' % X.shape[1])
     n = X.shape[0]
     perplexity = _positive('perplexity', perplexity)
     if perplexity >= n:

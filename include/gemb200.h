@@ -472,7 +472,8 @@ int gemb_cc_free(gemb_cc *cc);
  *   calibration  _utils.pyx _binary_search_perplexity, in fp64.
  *   joint P      _t_sne.py _joint_probabilities_nn: (P_cond + P_cond^T) / sum, fp64, exact zeros dropped.
  *   start        PCA(n_components=2) scores with svd_flip(u_based_decision=False) signs, column 0 scaled to standard
- *                deviation 1e-4 (TSNE._fit, init='pca').
+ *                deviation 1e-4 (TSNE._fit, init='pca').  d <= 1024 (the width of the Jacobi eigensolver), else
+ *                GEMB_ERR_UNSUPPORTED.
  *   gradient     _barnes_hut_tsne.pyx gradient on _quad_tree.pyx's cells, times c = 2 (dof + 1) / dof = 4.
  *   optimiser    _t_sne.py _gradient_descent as TSNE._tsne runs it: 250 iterations (or max_iter, if fewer) at momentum
  *                0.5 with P times early_exaggeration, then momentum 0.8 up to max_iter; the KL error and the

@@ -31,6 +31,7 @@ X = np.random.RandomState(0).randn(40, 5)
     dict(X=X[:, :0]),                                    # d < 1
     dict(X=np.where(X > 1, np.nan, X)),                  # not finite
     dict(X=np.where(X > 1, np.inf, X)),
+    dict(X=np.random.RandomState(1).randn(100, 1025).astype(np.float32)),   # d above the PCA eigensolver's 1024
     dict(perplexity=40.0),                               # perplexity >= n
     dict(perplexity=0.0),
     dict(perplexity=-3.0),
@@ -42,7 +43,7 @@ X = np.random.RandomState(0).randn(40, 5)
     dict(learning_rate='fast'),
     dict(early_exaggeration=0.0),
     dict(min_grad_norm=-1.0),
-], ids=['x1d', 'n1', 'd0', 'nan', 'inf', 'perp-n', 'perp0', 'perp-neg', 'max_iter', 'angle-neg', 'angle-big', 'lr0',
+], ids=['x1d', 'n1', 'd0', 'nan', 'inf', 'd1025', 'perp-n', 'perp0', 'perp-neg', 'max_iter', 'angle-neg', 'angle-big', 'lr0',
         'lr-neg', 'lr-str', 'exag0', 'min_grad_norm'])
 def test_value_errors_before_any_device_call(no_device, bad):
     from gem_b200.evaluation.visualize_embedding import tsne
